@@ -2,13 +2,13 @@
 """Benchmark of the phys-optim hot path (BASELINE.json metric: optimised frames/sec of the batched staged
 physics optimisation) and of the other two BASELINE configurations.
 
-    python bench.py --gpus N --steps K --warmup W            # product arm (hand-written sm_100a kernels)
+    python bench.py --gpus N --steps K --warmup W            # product arm (hand-written sm_90a kernels)
     python bench.py --impl reference --gpus N --steps K ...   # CPU arm: the oracle port of the reference algorithm
     python bench.py --workload long | contact ...             # BASELINE configs[4] / configs[2], same line schema
 
 Default workload (`phys`): one "step" = one full staged solve (stages 1.1, 1.2, 2.1, 2.2, 3 and -- only for sequences
 whose stage 3 did not succeed -- 4 of phys_optim.cpp:554-749) of a batch of synthetic 120-frame / 2-end-effector
-sequences: BASELINE.json configs[1], batch 64 on one B200; 64 per GPU under torchrun (weak scaling, sequences are
+sequences: BASELINE.json configs[1], batch 64 on one H100; 64 per GPU under torchrun (weak scaling, sequences are
 independent NLPs; sharding, the solve, the device-side sampling into the send buffer and the one NCCL gather go through
 the product's `chd.parallel.ShardedSolver`).  At 8 GPUs the named configuration of BASELINE.json configs[3]
 (1024 sequences = 128 per GPU) is timed as well and reported under `named_config_1024`.
@@ -16,6 +16,10 @@ the product's `chd.parallel.ShardedSolver`).  At 8 GPUs the named configuration 
 value : whole-job frames/s with the problem tables already resident in HBM (device-side reset of the iterate).
 e2e   : the same metric through the public host API with host buffers: layout build + H2D + solve + gather + D2H of
         the solved trajectories inside the timed region.
+
+--dump-outputs DIR writes what the last timed step returned (solved trajectories, frame counts, success flags, per-stage
+status and iteration counts) as DIR/<name>.npy in float64; the inputs are seeded, so two builds can be compared array by
+array.
 """
 import argparse
 import json
@@ -48,16 +52,16 @@ def _env_int(name, default):
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons during the timed region, with the card's name and power limit."""
 
     def __init__(self, gpu):
         super().__init__(daemon=True)
         self.gpu, self.samples, self.reasons, self.stop_flag = gpu, [], set(), False
-        self.max_mhz = None
+        self.max_mhz = self.name = self.power_limit_w = None
 
     def run(self):
         q = "clocks.sm,clocks.max.sm,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown," \
-            "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
+            "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap,name,power.limit"
         names = ["hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"]
         while not self.stop_flag:
             try:
@@ -65,7 +69,8 @@ class ClockSampler(threading.Thread):
                                      capture_output=True, text=True, timeout=5).stdout.strip().split(",")
                 self.samples.append(float(out[0]))
                 self.max_mhz = float(out[1])
-                for n, v in zip(names, out[2:]):
+                self.name, self.power_limit_w = out[6].strip(), float(out[7])
+                for n, v in zip(names, out[2:6]):
                     if "Active" in v and "Not" not in v:
                         self.reasons.add(n)
             except Exception:
@@ -73,7 +78,8 @@ class ClockSampler(threading.Thread):
             time.sleep(0.2)
 
     def result(self):
-        return {"sm_mhz": float(np.median(self.samples)) if self.samples else None, "sm_max_mhz": self.max_mhz,
+        return {"gpu": self.name, "power_limit_w": self.power_limit_w,
+                "sm_mhz": float(np.median(self.samples)) if self.samples else None, "sm_max_mhz": self.max_mhz,
                 "reasons": sorted(self.reasons)}
 
 
@@ -193,11 +199,33 @@ def time_solver(solver, steps, warmup, flush, barrier, torch):
     return ts, last, solver.batch.launch_count() - l0, per
 
 
+DUMP_LIMIT = 64 * 1024 * 1024
+
+
+def dump_outputs(out_dir, out):
+    """The arrays `ShardedSolver.solve` returned in the last timed step, as float64 .npy files.  When the trajectories
+    would exceed DUMP_LIMIT, a fixed seeded subset of the sequences is written (its indices in `sequence_index.npy`)."""
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {"samples": out["samples"], "frames": out["frames"], "success": out["success"],
+              "stage_status": out["stage_status"], "stage_iters": out["stage_iters"]}
+    n = out["samples"].shape[0]
+    per_seq = sum(a.size // n for a in arrays.values()) * 8
+    if per_seq * n > DUMP_LIMIT:
+        idx = np.sort(np.random.default_rng(0).choice(n, DUMP_LIMIT // per_seq, replace=False))
+        arrays = {"samples": out["samples"][idx], "frames": out["frames"][idx], "success": out["success"][idx],
+                  "stage_status": out["stage_status"][:, idx], "stage_iters": out["stage_iters"][:, idx],
+                  "sequence_index": idx}
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), np.asarray(a, dtype=np.float64))
+
+
 def run_contact(args):
-    """BASELINE.json configs[2] (contact-net inference, 100k windows, 1 B200): scripts/bench_contact.py emits the line."""
+    """BASELINE.json configs[2] (contact-net inference, 100k windows, 1 H100): scripts/bench_contact.py emits the line."""
     cmd = [sys.executable, os.path.join(ROOT, "scripts", "bench_contact.py"), "--steps", str(args.steps), "--warmup", str(args.warmup)]
     if args.impl == "reference":
         cmd.append("--reference")
+    if args.dump_outputs:
+        cmd += ["--dump-outputs", args.dump_outputs]
     sys.exit(subprocess.call(cmd))
 
 
@@ -213,7 +241,10 @@ def main():
     ap.add_argument("--no-cpu", action="store_true")
     ap.add_argument("--no-named", action="store_true", help="skip the 1024-sequence pass at 8 GPUs")
     ap.add_argument("--named-world", type=int, default=8, help="world size at which the 128-per-GPU pass runs (8 = BASELINE configs[3])")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the outputs of the last timed step as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.dump_outputs and args.impl == "reference":
+        raise SystemExit("bench.py: --dump-outputs dumps the timed GPU path; the reference arm has none")
     rank, world, local = _env_int("RANK", 0), _env_int("WORLD_SIZE", 1), _env_int("LOCAL_RANK", 0)
     if args.workload == "contact":
         if rank == 0:
@@ -232,7 +263,7 @@ def main():
     torch.cuda.set_device(local)
     if world > 1:
         dist.init_process_group("nccl", device_id=torch.device("cuda", local))
-    flush = torch.empty(256 * 1024 * 1024 // 4, dtype=torch.float32, device="cuda")  # > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024 // 4, dtype=torch.float32, device="cuda")  # > 50 MB L2
 
     def barrier():
         torch.cuda.synchronize()
@@ -312,7 +343,7 @@ def main():
 
     named = None
     if world == args.named_world and args.workload == "phys" and per_gpu != 128 and not args.no_named:
-        # BASELINE.json configs[3]: 1024 sequences x 120 frames sharded across 8 B200 (128 per GPU)
+        # BASELINE.json configs[3]: 1024 sequences x 120 frames sharded across 8 H100 (128 per GPU)
         solver.close()
         Mn = measure(128, max(1, min(args.steps, 5)), 1, False)
         named = {"config": workload_config("phys", world, 128), "value": Mn["N"] * frames * max(1, min(args.steps, 5)) / Mn["t_total"],
@@ -333,7 +364,7 @@ def main():
             peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         except Exception:
             pass
-        hbm_peak, peak_src = (peaks.get("hbm_gbs"), "measured") if peaks.get("hbm_gbs") else (6650.0, "fallback")
+        hbm_peak, peak_src = (peaks.get("hbm_gbs"), "measured") if peaks.get("hbm_gbs") else (3350.0, "H100 SXM data sheet")
         last = M["last"]
         value = M["N"] * frames * args.steps / M["t_total"]
         kt = M["kt"]
@@ -349,14 +380,6 @@ def main():
         ach = launch_bytes / (kkt_ms / max(kkt_n, 1) * 1e-3) / 1e9 if kkt_n else 0.0
         eval_bytes = float((8 * (2 * sz[:, 0] + 2 * sz[:, 1] + sz[:, 2] + (18 + 3 * n_ee) * frames) * act).sum())
         eval_ach = eval_bytes / (eval_ms / max(eval_n, 1) * 1e-3) / 1e9 if eval_n else 0.0
-        traffic = None
-        for fn in ("r2_kkt_ncu.json", "r1_kkt_ncu.json"):
-            try:
-                prof = json.load(open(os.path.join(ROOT, "profiles", fn)))
-                traffic = prof["dram_bytes_per_sequence_per_launch"] * float(act.sum())   # ncu --set full capture, per launch
-                break
-            except Exception:
-                pass
         # band LDL^T flops of one factorisation: Na * (w + nb + 1)^2 (Golub & Van Loan); stage 3 works with the wider
         # band / border (switch times), the other stages with (w_fix, nb_fix)
         def fl(w, nb):
@@ -387,15 +410,15 @@ def main():
             # fp64 figure.  The HBM view of the same kernel (the north star asks for it) follows as `roofline_hbm`.
             "roofline": {"bound": "tensor", "kernel": "chd_k_kkt", "pipe": "fp64 tensor core (DMMA m8n8k4)",
                          "achieved": kkt_gflops / 1e3, "peak": (dmma_peak / 1e3) if dmma_peak else None, "unit": "TFLOP/s",
-                         "frac": (kkt_gflops / dmma_peak) if dmma_peak else None, "traffic": traffic,
+                         "frac": (kkt_gflops / dmma_peak) if dmma_peak else None,
                          "peak_source": "chd_measure_fp64_peak: DMMA loop on all SMs, measured in this run (no fp64 entry in MEASURED_PEAKS.json)",
                          "peak_dfma": (dfma_peak / 1e3) if dfma_peak else None,
                          "algorithmic_flops": kkt_flops, "ms_per_launch": kkt_ms / max(kkt_n, 1),
                          "active_sequences_per_launch": float(act.sum()),
                          "note": "band LDL^T flop count Na*(w+nb+1)^2 per active sequence and factorisation; one CTA per sequence, so at "
-                                 "most active_sequences_per_launch of the 148 SMs work"},
+                                 "most active_sequences_per_launch SMs work"},
             "roofline_hbm": {"bound": "hbm", "kernel": "chd_k_kkt", "achieved": ach, "peak": hbm_peak, "unit": "GB/s",
-                             "frac": ach / hbm_peak, "traffic": traffic, "algorithmic_bytes": launch_bytes, "peak_source": peak_src},
+                             "frac": ach / hbm_peak, "algorithmic_bytes": launch_bytes, "peak_source": peak_src},
             "kernels": {k: {"ms": v[0], "launches": v[1]} for k, v in kt.items()},
             "roofline_eval": {"bound": "hbm", "kernel": "chd_k_eval", "achieved": eval_ach, "peak": hbm_peak, "unit": "GB/s",
                               "frac": eval_ach / hbm_peak},
@@ -414,6 +437,8 @@ def main():
                                               "full staged solve, %.1f s wall" % (len(seeds), fr_, len(seeds) - 1, cores, wall),
                                     "residual": rc}
         print(json.dumps(line))
+        if args.dump_outputs:
+            dump_outputs(args.dump_outputs, last)
     if world > 1:
         dist.destroy_process_group()
 

@@ -223,7 +223,7 @@ int run_schedule(chd_phys_batch* b) {
 
 extern "C" {
 
-const char* chd_version(void) { return "libchd 0.1 (sm_100a)"; }
+const char* chd_version(void) { return "libchd 0.1 (sm_90a)"; }
 
 int chd_measure_fp64_peak(double* dfma_gflops, double* dmma_gflops) {
   int dev = 0, sms = 0;
@@ -331,7 +331,11 @@ static int batch_create_impl(const chd_phys_problem* problems, int32_t batch, co
   D.nbt = (hb.nb_max + 1 + 7) / 8;
   D.win_tiles = std::max(D.Q * (D.Q + 1) / 2, 2 * D.Q);
   D.kstride = (size_t)D.nbc_max * D.Q * 64 + (size_t)D.nbc_max * D.nbt * 64 + (size_t)64 * D.nbt * D.nbt;
-  b->kcopy_blocks = (int)std::min<size_t>(512, std::max<size_t>(std::max<size_t>(1, 592 / B), D.kstride * sizeof(double) / 131072));
+  int dev = 0, sms = 0, smem_max = 0;
+  CHD_CUDA(cudaGetDevice(&dev));
+  CHD_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  // CTAs per sequence: enough for four per SM over the whole batch, and at least one per 128 KB of band storage
+  b->kcopy_blocks = (int)std::min<size_t>(512, std::max<size_t>(std::max<size_t>(1, 4 * (size_t)sms / B), D.kstride * sizeof(double) / 131072));
   AL(cost, B * 2) AL(Kwork, B * D.kstride) AL(Kbase, B * D.kstride) AL(sol, B * (size_t)(hb.Na_max + hb.nb_max)) AL(ipm, B)
   AL(rhs0, B * (size_t)(hb.Na_max + hb.nb_max)) AL(rhs1, B * (size_t)(hb.Na_max + hb.nb_max))
 #undef AL
@@ -349,8 +353,6 @@ static int batch_create_impl(const chd_phys_problem* problems, int32_t batch, co
   // the per-unknown vectors alias the tail of the window region (chd_kkt_body)
   const size_t kkt_fixed = (CHD_KKT_THREADS + nbp8 * nbp8 + (size_t)D.pan_doubles + 16) * sizeof(double);
   const size_t kkt_win = ((size_t)D.win_tiles * 64 + (size_t)D.Q * D.nbt * 64) * sizeof(double);
-  int dev = 0, smem_max = 0;
-  CHD_CUDA(cudaGetDevice(&dev));
   CHD_CUDA(cudaDeviceGetAttribute(&smem_max, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
   const bool vectors_fit = (size_t)D.win_tiles * 64 + (size_t)D.Q * D.nbt * 64 >= n_even + xs_len + 2 * (size_t)D.Q * 64 + 3072;
   if (vectors_fit && kkt_fixed + kkt_win + kkt_static + 256 <= (size_t)smem_max) {
@@ -369,14 +371,11 @@ static int batch_create_impl(const chd_phys_problem* problems, int32_t batch, co
     }
   }
   {
-    int sms = 0;
-    CHD_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
     // Admission queue (continuous batching): CHD_SLOTS=n lets at most n sequences iterate at once, the others wait for a
-    // finished one to hand over (chd_stage_advance).  Off by default: measured on a 1024-sequence job (148 slots = one
-    // CTA per SM) 35.7 k frames/s against 39.4 k without the queue -- finished sequences already cost nothing but an
-    // early-exit CTA, the cost of a KKT launch grows with the number of live sequences either way (16 us per live
-    // sequence once their band storage exceeds the L2), and late admission only delays the slow sequences.
-    (void)sms;
+    // finished one to hand over (chd_stage_advance).  Off by default: on a 1024-sequence job with one slot per SM it was
+    // slower than no queue -- finished sequences already cost nothing but an early-exit CTA, the cost of a KKT launch
+    // grows with the number of live sequences either way (once their band storage exceeds the L2), and late admission
+    // only delays the slow sequences.
     b->slots = getenv("CHD_SLOTS") ? atoi(getenv("CHD_SLOTS")) : (1 << 30);
     if (b->slots < 1) b->slots = 1;
     if ((rc = dev_alloc(b, 2, &D.queue))) return rc;
@@ -394,7 +393,7 @@ static int batch_create_impl(const chd_phys_problem* problems, int32_t batch, co
   CHD_CUDA(cudaMallocAsync((void**)&b->d_frames, B * sizeof(int), b->stream));
   b->allocs.push_back(b->d_samples);
   b->allocs.push_back(b->d_frames);
-  b->h_ipm = (ChdIpm*)std::malloc(B * sizeof(ChdIpm));   // pageable: pinned allocation / release cost up to 0.3 s per batch
+  b->h_ipm = (ChdIpm*)std::malloc(B * sizeof(ChdIpm));   // pageable: pinned allocation / release is slow per batch
   if (!b->h_ipm) return -3;
   CHD_CUDA(cudaMallocAsync((void**)&b->d_stages, 6 * sizeof(ChdStageDev), b->stream));
   b->allocs.push_back(b->d_stages);
@@ -406,7 +405,7 @@ static int batch_create_impl(const chd_phys_problem* problems, int32_t batch, co
 void chd_phys_batch_destroy(chd_phys_batch* b) {
   if (!b) return;
   if (b->stream) {
-    for (void* p : b->allocs) cudaFreeAsync(p, b->stream);   // back to the pool, not to the driver (cudaFree cost up to 350 ms per batch)
+    for (void* p : b->allocs) cudaFreeAsync(p, b->stream);   // back to the pool, not to the driver (cudaFree synchronises the device)
     cudaStreamSynchronize(b->stream);
   }
   std::free(b->h_ipm);

@@ -1,4 +1,4 @@
-// Foot-contact classifier of contact-human-dynamics on sm_100a (product code).
+// Foot-contact classifier of contact-human-dynamics on sm_90a (product code).
 //
 // Replaces, for inference, src/contact_learning/test.py:51-152 (val_full_video) +
 // src/contact_learning/models/openpose_only.py:29-78 + the window construction of
@@ -9,10 +9,11 @@
 //                          8x8 outputs per thread, double-buffered shared-memory tiles (layers 351-1024-512-128)
 //   chd_k_contact_tail   : the two small layers 128-32-20
 //   chd_k_contact_vote   : sigmoid > 0.5, 5-vote aggregation, edge thresholds, 2-frame padding, int64 labels
-// Windows are processed in slabs of 16384 so that the activations of a slab (132 MB) stay in the 126 MB L2 / HBM
-// working set instead of shared memory; every output is one fp32 accumulator summed over k in ascending order
-// (fmaf), the same arithmetic as a plain loop.  fp32 FFMA, no tf32/bf16: the integer labels must match the
-// reference's fp32 forward away from the logit-0 boundary (SURVEY 8(a)-D note; tcgen05 has no fp32 kind).
+// Windows are processed in slabs of 16384 (activations of a slab: 132 MB, in HBM rather than shared memory; a slab
+// small enough for the 50 MB L2 would leave the 128-wide layer with fewer tiles than SMs); every output is one fp32
+// accumulator summed over k in ascending order (fmaf), the same arithmetic as a plain loop.  fp32 FFMA, no tf32/bf16:
+// the integer labels must match the reference's fp32 forward away from the logit-0 boundary (SURVEY 8(a)-D note;
+// wgmma has no fp32-input kind).
 #include <cuda_runtime.h>
 #include <cstdlib>
 
@@ -467,8 +468,8 @@ int chd_contact_detect(chd_contact_net* net, const double* raw, const int32_t* s
     return rc;
   // Videos are independent: the batch is cut into up to four chunks whose keypoints are uploaded on a copy stream while
   // the previous chunk is preprocessed, classified and voted on the compute stream (the 65 MB upload of the 100k-window
-  // configuration otherwise sits in front of 5 ms of compute); every chunk is padded to the global Fmax, so the labels
-  // do not depend on the cut.
+  // configuration otherwise sits in front of about 6 ms of compute on an H100); every chunk is padded to the global
+  // Fmax, so the labels do not depend on the cut.
   int nchunk = 1;
   if (const char* e = getenv("CHD_CONTACT_CHUNKS")) nchunk = std::max(1, std::min(4, atoi(e)));
   if (V < 16 * nchunk) nchunk = 1;

@@ -1,4 +1,4 @@
-// Shared host/device definitions for the batched phys-optim NLP (product code, sm_100a).
+// Shared host/device definitions for the batched phys-optim NLP (product code, sm_90a).
 //
 // What this replaces: the per-iteration evaluation the reference performs through ifopt's virtual
 // ConstraintSet/CostTerm interface (towr_phys_optim/src/constraints/*.cpp, src/costs/*.cpp,

@@ -1,4 +1,4 @@
-// sm_100a kernels of the batched interior-point trajectory optimiser (product code).
+// sm_90a kernels of the batched interior-point trajectory optimiser (product code).
 // One CTA owns one sequence in every kernel; sequences are independent NLPs (SURVEY.md 8(e)).
 //
 //   chd_k_stage_begin : row activity flags + IPM state reset for a stage

@@ -1,4 +1,4 @@
-// KKT kernels of the batched interior-point solver (product code, sm_100a).
+// KKT kernels of the batched interior-point solver (product code, sm_90a).
 //
 //   chd_k_hess_base : once per stage -- Gauss-Newton Hessian of the (quadratic, fixed-duration) cost terms
 //                     of data_cost.cpp / vel_smooth_cost.cpp, scaled by the objective scaling, in tile format (Kbase)
@@ -699,9 +699,9 @@ __device__ __forceinline__ void chd_kkt_body(const ChdDev& D) {
     // (c) stream in block row Kc + Q (its slots are dead now), trailing updates on the fp64 tensor core;
     //     warp 0 takes the pair that completes the next diagonal tile and factors it right away
     const int In = Kc + Q;
-    // Two stream-in variants (D.tma, environment CHD_TMA at batch creation; measured on the benchmark batch: 1.00 ms per
-    // launch with the per-thread cp.async chunks, 1.04 ms with the TMA producer warp, 1.21 ms when a lane of an updating
-    // warp issues the bulk copies, 1.11 ms with dynamically dealt update blocks):
+    // Two stream-in variants (D.tma, environment CHD_TMA at batch creation; benchmark batch on an H100 SXM at 400 W:
+    // 1.14 ms per launch with the per-thread cp.async chunks, 1.22 ms with the TMA producer warp; bulk copies issued by a
+    // lane of an updating warp and dynamically dealt update blocks were slower still when tried):
     if (WS && !use_tma && In < nbc) {
       // 16-byte cp.async chunks by the warps 1..15; warp 0 goes straight to the diagonal tile
       for (int idx = tid - 32; idx < Q * 32 + nbt_s * 32; idx += nt - 32) {
@@ -772,7 +772,7 @@ __device__ __forceinline__ void chd_kkt_body(const ChdDev& D) {
       if (!WS && !compact) {
         // more than 64 panel groups, window in global (L2) memory: each warp collects up to four target tiles, issues all their loads, and only
         // then runs the tensor-core updates and the stores.  (With the window in shared memory the simple loop below
-        // is faster: measured 707 vs 820 ms of KKT time per benchmark step.)
+        // was faster on the benchmark batch.)
         const int r8 = (lane >> 2) * 8 + 2 * (lane & 3);
         int p = warp - 1;
         while (p < np_loop) {

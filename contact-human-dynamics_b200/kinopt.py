@@ -6,7 +6,7 @@ Reference: `src/optimize/optimize_trajectory.py` -- residual vector `fun_anim_fo
 `optimize_trajectory` (:522-834: IK initialisation, two `scipy.least_squares(max_nfev=50, tr_solver='lsmr')` stages,
 Huber floor fit + contact pruning in between).
 
-What is different here, deliberately (B200-first):
+What is different here, deliberately (GPU-first):
 * The reference materialises a dense (terms x 84 F) Jacobian in Python loops (4 GB at 120 frames), multiplies it frame by
   frame with the IK Jacobian and hands a `lil_matrix` to LSMR.  Every residual is *linear* in the joint positions of at most
   three consecutive frames (only the projection term is not, and it touches one frame), so J = A * blockdiag(dP_f/dx_f) + E
@@ -285,8 +285,8 @@ def _banded_cholesky_solve(t, H, g, lam, dense=None):
     F, n = D.shape[0], D.shape[1]
     Dd = D + lam * t.diag_embed(t.diagonal(D, dim1=1, dim2=2).clamp_min(1e-12))
     if dense is None:
-        # on the GPU the sweep below is F dependent steps of a few tiny kernels each (launch bound: ~0.2 s per solve at 120
-        # frames); one dense fp64 Cholesky of the (87 F)^2 matrix is far faster there as long as it fits comfortably
+        # on the GPU the sweep below is F dependent steps of a few tiny kernels each (launch bound); one dense fp64
+        # Cholesky of the (87 F)^2 matrix is far faster there as long as it fits comfortably
         dense = D.is_cuda and F * n <= DENSE_MAX_UNKNOWNS
     if dense:
         A = t.zeros(F * n, F * n, dtype=D.dtype, device=D.device)

@@ -1,6 +1,6 @@
 """Host-side mirror of the reference's phys-optim operator for a batch of sequences.
 
-`PhysBatch` binds libchd.so (hand-written sm_100a kernels behind a C ABI, include/chd.h) through ctypes.
+`PhysBatch` binds libchd.so (hand-written sm_90a kernels behind a C ABI, include/chd.h) through ctypes.
 There is NO CPU fallback: if the CUDA library is missing or no GPU is visible, construction fails loudly
 (`host_only=True` builds only the host-side NLP layout tables, which is what the CPU tests exercise).
 

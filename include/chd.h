@@ -1,4 +1,4 @@
-/* libchd -- C ABI of the B200-native batched physics-based trajectory optimiser and foot-contact
+/* libchd -- C ABI of the H100-native batched physics-based trajectory optimiser and foot-contact
  * classifier (drop-in for the hot path of davrempe/contact-human-dynamics).
  *
  * Every entry point is plain C: pointers + sizes, int return (0 = ok, negative = error), no exceptions

@@ -1,4 +1,4 @@
-"""Contact-net inference benchmark (BASELINE.json configs[2]: 100k 9-frame OpenPose-25 windows, 1 B200); reached as
+"""Contact-net inference benchmark (BASELINE.json configs[2]: 100k 9-frame OpenPose-25 windows, 1 H100); reached as
 `python bench.py --workload contact [--impl reference]`.  Prints one JSON line in bench.py's schema:
 
 value : windows/s with the preprocessed keypoints already resident in HBM (`chd_contact_forward_device`)
@@ -6,6 +6,7 @@ e2e   : windows/s through the public host call `ContactNet.detect` (`chd_contact
         page-locked host memory -> H2D -> preprocessing kernel -> windows / MLP / votes -> D2H of the int64 labels
 --reference : the CPU arm -- the oracle restatement of the reference's dataset preprocessing + torch-CPU fp32 forward +
         vote aggregation on a bounded sample of the same videos, all host threads
+--dump-outputs DIR : labels and logits of the last timed device-resident step as DIR/<name>.npy (float32)
 """
 import argparse
 import ctypes as C
@@ -20,7 +21,7 @@ sys.path.insert(0, os.path.join(ROOT, "tests", "golden"))
 import numpy as np
 
 V, F = 1000, 108                      # 1000 videos x 100 windows
-CONFIG = {"workload": "contact-net inference: 100k 9-frame OpenPose-25 joint windows (%d synthetic videos x %d frames), 1 B200" % (V, F),
+CONFIG = {"workload": "contact-net inference: 100k 9-frame OpenPose-25 joint windows (%d synthetic videos x %d frames), 1 H100" % (V, F),
           "videos": V, "frames": F, "windows": V * (F - 8)}
 
 
@@ -48,6 +49,7 @@ def main():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--reference", action="store_true")
     ap.add_argument("--cpu-videos", type=int, default=100)
+    ap.add_argument("--dump-outputs", metavar="DIR")
     args = ap.parse_args()
     import torch
     from make_contact_golden import contact_weights
@@ -112,8 +114,13 @@ def main():
     ns = args.cpu_videos
     cpu_t, ref_lab = cpu_arm(raw[:ns], sd, cores)
     agree = float(np.mean([np.array_equal(ref_lab[i], labels[i]) for i in range(ns)]))
+    if args.dump_outputs:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "labels.npy"), lab_h.astype(np.float32))
+        np.save(os.path.join(args.dump_outputs, "logits.npy"), lg.cpu().numpy())
     flops = 2 * 953984 * nwin
-    peak = 148 * 128 * 2 * 1.965e9 / 1e12
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    peak = sms * 128 * 2 * 1.98e9 / 1e12
     print(json.dumps({"metric": "contact windows/s", "value": nwin / dev, "unit": "windows/s", "n_gpus": 1, "steps": args.steps, "warmup": args.warmup,
                       "ms_per_step": 1e3 * dev, "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f32", "data": "synthetic",
                       "config": CONFIG,
@@ -123,7 +130,7 @@ def main():
                       "gpu_launches": int(launches),
                       "roofline": {"bound": "tensor", "kernel": "chd_k_contact_gemm", "achieved": flops / dev / 1e12, "peak": peak, "unit": "TFLOP/s",
                                    "frac": flops / dev / 1e12 / peak, "traffic": None,
-                                   "note": "fp32 FFMA pipe (no tensor core: integer labels must match the reference's fp32 forward); peak = nominal 148 SMs x 128 FFMA x 1.965 GHz"},
+                                   "note": "fp32 FFMA pipe (no tensor core: integer labels must match the reference's fp32 forward); peak = nominal SMs x 128 FFMA x 1.98 GHz (H100 SXM boost clock)"},
                       "cpu_baseline": {"value": ns * (F - 8) / cpu_t, "unit": "windows/s", "cores": cores, "kind": "port",
                                        "sample": "%d of the %d videos (%d windows): numpy preprocessing + torch fp32 CPU forward + votes, %.1f s" % (ns, V, ns * (F - 8), cpu_t)},
                       "labels_equal_frac_vs_cpu": agree, "min_abs_logit": mabs}))

@@ -1,4 +1,4 @@
-import sys; sys.path.insert(0,'/root/repo')
+import os, sys; sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np, ctypes as C, chd
 from oracle.phys import OracleProblem
 p = chd.synth.make_problem(1, n_ee=2)

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Turns the CSV of `ncu --metrics gpu__time_duration.sum --clock-control none --csv --log-file X ...` into the
-per-kernel table kept under profiles/ (shares of the step; absolute times under ncu are cold-cache and serialised)."""
+per-kernel table (shares of the step; absolute times under ncu are cold-cache and serialised)."""
 import csv
 import sys
 from collections import defaultdict

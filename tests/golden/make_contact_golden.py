@@ -1,7 +1,7 @@
 """Generates the contact-classifier golden vectors by running the REFERENCE's own code
-(/root/reference/src/contact_learning: RealVideoDataset, OpenPoseModel, test.val_full_video) on small synthetic
-OpenPose directories with seeded weights.  Run once in the build container (the reference is not present on the
-GPU box); the outputs under tests/golden/contact/ are committed.
+(src/contact_learning of a checkout of the reference at $CHD_REFERENCE_DIR, default ../contact-human-dynamics next to
+this repository: RealVideoDataset, OpenPoseModel, test.val_full_video) on small synthetic OpenPose directories with
+seeded weights.  Run once; the outputs under tests/golden/contact/ are committed, so the tests need no reference.
 
     python tests/golden/make_contact_golden.py
 
@@ -19,7 +19,7 @@ import numpy as np
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
 sys.path.insert(0, ROOT)
-REF = "/root/reference/src"
+REF = os.path.join(os.environ.get("CHD_REFERENCE_DIR", os.path.join(ROOT, "..", "contact-human-dynamics")), "src")
 
 
 def contact_weights(seed=0):

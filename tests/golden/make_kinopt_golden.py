@@ -1,12 +1,12 @@
 """Golden vectors for the kinematic optimiser (`src/optimize/optimize_trajectory.py`), produced by the REFERENCE'S OWN code
-imported from /root/reference with the shims of make_towr_golden.py (numpy 2 aliases, plotting stubs).  Build container
-only.  Writes tests/golden/kinopt/:
+imported from the reference checkout of make_towr_golden.py, with its shims (numpy 2 aliases, plotting stubs).
+Writes tests/golden/kinopt/:
 
   inputs.npz      synthetic clip: 2D keypoints + confidences, root-relative 3D joints, root translation, initial joint
                   angles (axis-angle, SMPL-style), contact labels; the skeleton is tests/golden/kinopt/skeleton.bvh
   skeleton.npz    update_skeleton(...) of the reference: fitted offsets
   funjac.npz      fun_anim_for_projection / jac_anim_for_projection_sparse of the reference at two points x (stage weights
-                  with and without the floor term)
+                  with and without the floor term); the Jacobians shrunk by `jacobian_golden` to stay under 1 MB
   run.npz         the reference's full optimize_trajectory(...) output on the clip: final x is not exposed by the
                   reference, so: final joint positions, re-projected 2D points, floor normal / point, refined contact labels,
                   and the objective 0.5 |f|^2 of the returned animation under the final-stage weights
@@ -44,6 +44,20 @@ def synth_clip(chd, seed=0):
     T[:, 0] = 0.0
     gp, _ = prepare.forward_kinematics(np.array(parents), R, T)                 # root-relative positions, skeleton order
     return names, parents, off, e, root, gp
+
+
+def jacobian_golden(J, F, tag):
+    """The parts of the reference Jacobian J (terms x 87 F) that tests/test_kinopt_cpu.py compares, small enough to store:
+    the projection rows (F x 28 x 2) at a seeded set of columns, and the other rows in CSR form -- the even ones for point
+    "a", the odd ones for point "b", so that every row is checked at one of the two points."""
+    import scipy.sparse as sp
+    nproj = F * 28 * 2
+    cols = np.concatenate([np.random.default_rng(0).choice(F * 87, 10, replace=False), [0, 1, 2, 87, 89]])
+    rows = np.arange(nproj + (tag == "b"), J.shape[0], 2)
+    R = sp.csr_matrix(J[rows])
+    return {"Jshape_" + tag: np.array(J.shape), "Jproj_cols_" + tag: cols, "Jproj_" + tag: J[:nproj][:, cols],
+            "Jrows_" + tag: rows.astype(np.int32), "Jdata_" + tag: R.data, "Jindices_" + tag: R.indices.astype(np.int32),
+            "Jindptr_" + tag: R.indptr.astype(np.int32)}
 
 
 def main():
@@ -118,7 +132,7 @@ def main():
         args = (sk, poses3D, root_pos, j2n, normal, point, pw, dw, np.arange(J), np.arange(J), ot.SMOOTH_WEIGHTS, vel, 1000.0, 0.1, 0.5, 0.3, 10.0, fw)
         fj["x_" + tag] = x
         fj["f_" + tag] = ot.fun_anim_for_projection(x, *args)
-        fj["J_" + tag] = np.asarray(ot.jac_anim_for_projection_sparse(x, *args).todense())
+        fj.update(jacobian_golden(np.asarray(ot.jac_anim_for_projection_sparse(x, *args).todense()), F, tag))
     np.savez_compressed(os.path.join(OUT, "funjac.npz"), normal=normal, point=point, pw=pw, dw=dw, j2n=j2n, **fj)
 
     # the full run

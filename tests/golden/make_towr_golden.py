@@ -1,10 +1,10 @@
 """Golden vectors for the steps on either side of the phys-optim hot path, produced by the REFERENCE'S OWN code
 (`src/utils/towr_utils.py`: prepare_input :451-777, load_results :51-122, apply_results :779-857, and the BVH / Animation
-/ Quaternions / InverseKinematics library under `src/skeleton_fitting/ik`) imported from /root/reference.
+/ Quaternions / InverseKinematics library under `src/skeleton_fitting/ik`) imported from a checkout of the reference ($CHD_REFERENCE_DIR, default ../contact-human-dynamics).
 
 The reference modules do not import on numpy 2 as they are: this script installs shims for `numpy.core.umath_tests`,
 `np.float` / `np.int` and the plotting / image modules (none of which the three functions use) and then calls the
-unmodified functions.  Run in the build container only (the GPU box has no /root/reference):
+unmodified functions.  Run where that checkout exists (the committed outputs are all the tests need):
 
     python tests/golden/make_towr_golden.py
 
@@ -21,7 +21,7 @@ import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, ROOT)
 OUT = os.path.join(ROOT, "tests", "golden", "towr")
-REF = "/root/reference/src"
+REF = os.path.join(os.environ.get("CHD_REFERENCE_DIR", os.path.join(ROOT, "..", "contact-human-dynamics")), "src")
 
 
 def import_reference():

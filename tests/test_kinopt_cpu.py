@@ -4,6 +4,7 @@ import os
 
 import numpy as np
 import pytest
+import scipy.sparse
 
 G = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "kinopt")
 
@@ -46,22 +47,25 @@ def test_residual_and_jacobian_vs_reference(chd, data, tag, floor_w):
     assert f.shape == fj["f_" + tag].shape
     # the reference's quaternion path carries 1e-10 relative noise (axis / (|axis| + 1e-10)); projection weight 1000
     np.testing.assert_allclose(f, fj["f_" + tag], rtol=0, atol=2e-7)
-    Jm, Jr = m.dense_jacobian(x, w).numpy(), fj["J_" + tag]
-    assert Jm.shape == Jr.shape
+    Jm = m.dense_jacobian(x, w).numpy()
+    assert Jm.shape == tuple(fj["Jshape_" + tag])
     nproj = F * 28 * 2
-    np.testing.assert_allclose(Jm[nproj:], Jr[nproj:], rtol=0, atol=1e-6)          # every group but the projection term
+    # every group but the projection term; the golden holds every other row of them at each of the two points
+    rows = fj["Jrows_" + tag]
+    Jr = scipy.sparse.csr_matrix((fj["Jdata_" + tag], fj["Jindices_" + tag], fj["Jindptr_" + tag]), shape=(len(rows), Jm.shape[1]))
+    assert rows[0] in (nproj, nproj + 1) and (np.diff(rows) == 2).all() and rows[-1] >= Jm.shape[0] - 2
+    np.testing.assert_allclose(Jm[rows], Jr.toarray(), rtol=0, atol=1e-6)
     # projection rows: exact derivative here (central differences); the reference's analytic rows are not (see kinopt.py)
-    rng = np.random.default_rng(0)
-    cols = np.concatenate([rng.choice(F * 87, 10, replace=False), [0, 1, 2, 87, 89]])
+    cols = fj["Jproj_cols_" + tag]
     eps, worst_ref = 1e-6, 0.0
-    for c in cols:
+    for k, c in enumerate(cols):
         xp, xm = x.reshape(-1).clone(), x.reshape(-1).clone()
         xp[c] += eps
         xm[c] -= eps
         fd = (m.residual_vector(xp.reshape(F, -1), w) - m.residual_vector(xm.reshape(F, -1), w)).numpy() / (2 * eps)
         scale = max(1.0, np.abs(Jm[:, c]).max())
         assert np.abs(fd - Jm[:, c]).max() / scale < 1e-7
-        worst_ref = max(worst_ref, np.abs(fd[:nproj] - Jr[:nproj, c]).max() / scale)
+        worst_ref = max(worst_ref, np.abs(fd[:nproj] - fj["Jproj_" + tag][:, k]).max() / scale)
     assert worst_ref > 1e-3      # documents the reference's misplaced root-translation columns (optimize_trajectory.py:106-137)
 
 

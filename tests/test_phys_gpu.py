@@ -213,7 +213,7 @@ def test_phys_optim_cli_files(chd, tmp_path):
 
 def test_fp64_peak_probe(chd):
     """chd_measure_fp64_peak (roofline denominator of bench.py): DFMA and DMMA throughput of the device, both far above
-    anything a single SM could deliver and of the same order (B200: ~36-37 TFLOP/s each)."""
+    anything a single SM could deliver and of the same order (H100 SXM at a 400 W power limit: 32-33 TFLOP/s each)."""
     dfma, dmma = chd.phys.measure_fp64_peak()
     assert 5e3 < dfma < 2e5 and 5e3 < dmma < 2e5
     assert 0.3 < dfma / dmma < 3.0
