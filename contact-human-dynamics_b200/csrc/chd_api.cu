@@ -62,7 +62,6 @@ struct chd_phys_batch {
   int64_t h2d_bytes = 0;
   ChdStageDev* d_stages = nullptr;
   int sched_max_iter = 0;
-  int slots = 1 << 30;          // sequences iterating at once (CTAs that can be resident); the rest of a large batch queues up
   bool sched_has_dur = false;   // the running schedule contains stage 3 (its cost Hessian is rebuilt every iteration)
   // pristine copies of the tables stage 3 rewrites (chd_phys_reset)
   double *poly_T0 = nullptr, *poly_tend0 = nullptr, *phase_tend0 = nullptr;
@@ -139,10 +138,6 @@ int set_schedule(chd_phys_batch* b, const int* sched, int nsched, int override_s
   b->sched_max_iter = 0;
   b->sched_has_dur = false;
   for (int i = 0; i < nsched; ++i) b->sched_max_iter += tab[sched[i]].max_iter + 2, b->sched_has_dur |= sched[i] == CHD_STAGE_3;
-  {
-    int q[2] = {0, b->slots};
-    CHD_CUDA(cudaMemcpyAsync(b->D.queue, q, sizeof(q), cudaMemcpyHostToDevice, b->stream));
-  }
   chd_k_sched_reset<<<(b->hb.B + 127) / 128, 128, 0, b->stream>>>(b->D);
   b->launches++;
   return 0;
@@ -326,8 +321,7 @@ static int batch_create_impl(const chd_phys_problem* problems, int32_t batch, co
   AL(sc, mm) AL(dL, mm) AL(dU, mm) AL(s, mm) AL(y, mm) AL(zL, mm) AL(zU, mm) AL(ds, mm) AL(dy, mm) AL(dzL, mm) AL(dzU, mm)
   D.nbc_max = (hb.Na_max + 7) / 8;
   D.Q = (hb.w_max + 7) / 8 + 1;
-  D.Qfix = (hb.w_fix_max + 7) / 8 + 1;
-  D.tma = getenv("CHD_TMA") ? atoi(getenv("CHD_TMA")) : 0;   // band tiles the fixed-duration stages work with (storage strides follow Q)
+  D.Qfix = (hb.w_fix_max + 7) / 8 + 1;   // band tiles the fixed-duration stages work with (storage strides follow Q)
   D.nbt = (hb.nb_max + 1 + 7) / 8;
   D.win_tiles = std::max(D.Q * (D.Q + 1) / 2, 2 * D.Q);
   D.kstride = (size_t)D.nbc_max * D.Q * 64 + (size_t)D.nbc_max * D.nbt * 64 + (size_t)64 * D.nbt * D.nbt;
@@ -358,6 +352,12 @@ static int batch_create_impl(const chd_phys_problem* problems, int32_t batch, co
   if (vectors_fit && kkt_fixed + kkt_win + kkt_static + 256 <= (size_t)smem_max) {
     D.win_smem = 1;
     b->smem_kkt = kkt_fixed + kkt_win;
+    // chd_k_kkt compacts at most 64 panel groups (band + border tiles) for its trailing updates and has no other update
+    // loop for the shared-memory window; any window that fits is well below that (Q + nbt <= 30 at 227 KB)
+    if (D.Q - 1 + D.nbt > 64) {
+      fprintf(stderr, "libchd: band + border too wide for the compacted update loop (Q=%d nbt=%d)\n", D.Q, D.nbt);
+      return -5;
+    }
   } else {
     // long horizons / wide bands: vectors and window in a global scratch area (chd_k_kkt_gwin)
     D.win_smem = 0;
@@ -369,16 +369,6 @@ static int batch_create_impl(const chd_phys_problem* problems, int32_t batch, co
       fprintf(stderr, "libchd: band + border too wide for the pair tables (Q=%d nbt=%d)\n", D.Q, D.nbt);
       return -5;
     }
-  }
-  {
-    // Admission queue (continuous batching): CHD_SLOTS=n lets at most n sequences iterate at once, the others wait for a
-    // finished one to hand over (chd_stage_advance).  Off by default: on a 1024-sequence job with one slot per SM it was
-    // slower than no queue -- finished sequences already cost nothing but an early-exit CTA, the cost of a KKT launch
-    // grows with the number of live sequences either way (once their band storage exceeds the L2), and late admission
-    // only delays the slow sequences.
-    b->slots = getenv("CHD_SLOTS") ? atoi(getenv("CHD_SLOTS")) : (1 << 30);
-    if (b->slots < 1) b->slots = 1;
-    if ((rc = dev_alloc(b, 2, &D.queue))) return rc;
   }
   if (b->smem_eval + 1024 > (size_t)smem_max || b->smem_kkt + kkt_static + 256 > (size_t)smem_max) {
     fprintf(stderr, "libchd: problem too large for the shared-memory staged kernels (n_max=%d)\n", hb.n_max);
@@ -463,10 +453,7 @@ int chd_phys_eval(chd_phys_batch* b, int32_t stage, double* cost, double* grad, 
   if (!b || stage < 0 || stage > 5 || b->host_only) return -1;
   const ChdHostBatch& hb = b->hb;
   int sched[1] = {stage};
-  const int slots_keep = b->slots;
-  b->slots = 1 << 30;                       // a function evaluation touches every sequence of the batch at once (no queue)
   int rc = set_schedule(b, sched, 1, -1, 0);
-  b->slots = slots_keep;
   if (rc) return rc;
   {
     Timer t(b, KT_INIT);
@@ -571,7 +558,6 @@ int chd_phys_solve_stage(chd_phys_batch* b, int32_t stage, int32_t max_iter, int
       double* s = stats + 8 * i;
       s[0] = I.f, s[1] = I.E0, s[2] = I.viol_u, s[3] = I.dual_u, s[4] = I.compl_u, s[5] = I.mu, s[6] = I.delta_w, s[7] = I.ls_fail;
     }
-    if (i == 0 && getenv("CHD_PROF")) fprintf(stderr, "chd prof factor loop (Mcycles, accumulated since batch creation) warp1: panel+barrier %.2f updates %.2f wait+barrier %.2f | warp0: panel+barrier %.2f diagonal %.2f wait+barrier %.2f\n", I.dbg[0]/1e6, I.dbg[1]/1e6, I.dbg[2]/1e6, I.dbg[3]/1e6, I.dbg[4]/1e6, I.dbg[5]/1e6);
     if (i == 0 && getenv("CHD_PROF")) fprintf(stderr, "chd prof (Mcycles) seq0 stage %d: err %.2f jasm %.2f hasm %.2f factor %.2f border %.2f back %.2f rec %.2f\n", stage, I.prof[0]/1e6, I.prof[1]/1e6, I.prof[2]/1e6, I.prof[3]/1e6, I.prof[4]/1e6, I.prof[5]/1e6, I.prof[6]/1e6);
   }
   return 0;

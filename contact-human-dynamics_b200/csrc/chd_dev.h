@@ -23,7 +23,6 @@
 #define CHD_PH_BEGIN 0
 #define CHD_PH_RUN 1
 #define CHD_PH_FINISHED 2
-#define CHD_PH_WAITING 3    /* not admitted yet: more sequences than resident CTAs (continuous batching, chd_stage_advance) */
 struct ChdIpm {
   int status;    // of the current stage: 1 running, 0 converged, -1 iteration cap, -2 numerical failure
   int iter, nfilt, ls_fail, max_iter, n_bounds, m_act, pad0;
@@ -60,8 +59,7 @@ struct ChdStageDev {
 
 struct ChdDev {
   int B, S, Pmax, n_max, m_max, slots_max, sets_max, tab_max, F_max, Kd_max, Kr_max, Na_max, nb_max, w_max, par_stride,
-      n_ee_max, fo_max, Ph_max, win_smem, nbc_max, Q, Qfix, nbt, win_tiles, pan_doubles,
-      tma;   // 1: the elimination window is streamed with TMA bulk copies by a producer warp (CHD_TMA=1), 0: cp.async chunks by all warps
+      n_ee_max, fo_max, Ph_max, win_smem, nbc_max, Q, Qfix, nbt, win_tiles, pan_doubles;
   size_t kstride;                             // doubles per sequence of a tile-format KKT buffer (band | bord | corn)
   // ---- static layout ----
   const ChdSeq* seq;
@@ -91,7 +89,6 @@ struct ChdDev {
   double *rhs0, *rhs1;                        // right-hand side of the KKT system as rhs0 + mu * rhs1 (chd_k_asm), [B][Na_max + nb_max]
   size_t scratch_stride;                      // doubles per sequence in `scratch`
   ChdIpm* ipm;                                // B
-  int* queue;                                 // [0] next sequence to admit when a running one finishes, [1] slots (sequences iterating at once)
   const ChdStageDev* stages;                  // 6 stage configurations (device)
   int sched[8], nsched;                       // stage ids of the running schedule
   double* snapshots;                          // 3 x B x fo_max x (6 + 7 n_ee_max)
@@ -144,14 +141,7 @@ __device__ __forceinline__ void chd_stage_advance(const ChdDev& D, ChdIpm& I, in
   if (I.stage == CHD_STAGE_3 && status == 0 && I.pos < D.nsched && D.sched[I.pos] == CHD_STAGE_4) I.pos += 1;
   else if (I.stage == CHD_STAGE_3 && status != 0 && I.pos < D.nsched && D.sched[I.pos] == CHD_STAGE_4) snap_after = -1;  // SaveSolution comes after stage 4 (:758)
   I.snap = snap_after;
-  if (I.pos < D.nsched) {
-    I.stage = D.sched[I.pos], I.phase = CHD_PH_BEGIN;
-  } else {
-    I.phase = CHD_PH_FINISHED;
-    // continuous batching: the finished sequence hands its CTA slot to the next waiting one, which starts its first
-    // stage at the next iteration (every kernel skips sequences that are not in the phase it works on)
-    const int nxt = atomicAdd(D.queue, 1);
-    if (nxt < D.B) D.ipm[nxt].phase = CHD_PH_BEGIN;
-  }
+  if (I.pos < D.nsched) I.stage = D.sched[I.pos], I.phase = CHD_PH_BEGIN;
+  else I.phase = CHD_PH_FINISHED;
 }
 #endif

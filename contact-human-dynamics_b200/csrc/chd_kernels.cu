@@ -257,10 +257,8 @@ __global__ void __launch_bounds__(CHD_THREADS) chd_k_linesearch(ChdDev D) {
       bool ok = isfinite(phit) && isfinite(theta_t) && theta_t <= I.theta_max;
       // nonlinearity guard of stage 3: the linearised constraints predict theta(alpha) = (1 - alpha) theta; the trial
       // point is refused while the second-order error exceeds the predicted decrease (or a small absolute level)
-#ifndef CHD_PROFILE
       if (ls == 0) I.dbg[4] = 0.0, I.dbg[5] = 0.0;
       I.dbg[0] = alpha, I.dbg[1] = ls, I.dbg[2] = theta_t, I.dbg[3] = phit;
-#endif
       if (sg.opt_dur && s_trust) ok = false;
       if (sg.opt_dur && ok && theta_t - (1.0 - alpha) * theta > CHD_NL_GUARD * fmax(alpha * theta, CHD_NL_FLOOR * fmax(1.0, theta_ref))) ok = false;
       for (int q = 0; ok && q < I.nfilt; ++q)
@@ -438,9 +436,6 @@ __global__ void chd_k_sched_reset(ChdDev D) {
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b >= D.B) return;
   ChdIpm& I = D.ipm[b];
-  // the first `slots` sequences start, the others wait for a slot (one CTA per SM can be resident: more running
-  // sequences than that would only add waves of mostly finished CTAs to every launch)
-  I.pos = 0, I.stage = D.sched[0], I.phase = b < D.queue[1] ? CHD_PH_BEGIN : CHD_PH_WAITING, I.snap = -1, I.step_ready = 0, I.kw_req = 0, I.status = 1;
-  if (b == 0) D.queue[0] = D.queue[1] < D.B ? D.queue[1] : D.B;
+  I.pos = 0, I.stage = D.sched[0], I.phase = CHD_PH_BEGIN, I.snap = -1, I.step_ready = 0, I.kw_req = 0, I.status = 1;
   for (int q = 0; q < 6; ++q) I.st_status[q] = -9, I.st_iters[q] = 0;
 }

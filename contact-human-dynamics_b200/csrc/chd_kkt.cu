@@ -379,70 +379,100 @@ __device__ __forceinline__ void chd_assemble(const ChdDev& D, int b, const ChdKT
   }
 }
 
-// dynamic shared memory layout of chd_k_kkt (doubles):
-//   red[CHD_KKT_THREADS] | vecn[n_max] | xs[Np_max + nbp8] | cc[nbp8*nbp8] | ypan[(Q+nbt)*64] | xpan[(Q+nbt)*64] | xs2[Np_max] | dinv[16]
-//   | win[Q(Q+1)/2 * 64] | bwin[Q*nbt*64]            (the last two in global scratch when they do not fit)
-template <bool WS>
-__device__ __forceinline__ void chd_kkt_body(const ChdDev& D) {
-  extern __shared__ double sm[];
-  __shared__ int s_fail;
-  const int b = blockIdx.x;
-  ChdIpm& I = D.ipm[b];
-  if (I.phase != CHD_PH_RUN) return;
-  const int pre_refreshed = I.kw_req;   // Kwork = Kbase + distance-row curvature already prepared on the side stream
-  const ChdStageDev sg = D.stages[I.stage];
-  const ChdSeq* h = D.seq + b;
-  const int n = h->n, m = h->m, tid = threadIdx.x, nt = blockDim.x;
-  const int lane = tid & 31, warp = tid >> 5, nwarp = nt >> 5;
-  const size_t ro = (size_t)b * D.m_max, vo = (size_t)b * D.n_max;
-  const int* rf = D.rflag + ro;
-  const int* vk = D.var_kkt + vo;
-  const int* rk = D.row_kkt + ro;
-  const int* ep = D.ent_ptr + (size_t)b * (D.m_max + 1);
-  const int* ec = D.ent_col + (size_t)b * D.slots_max;
-  const double* Jv = D.Jv + (size_t)b * D.slots_max;
-  const double* grad = D.grad + vo;
+// Kwork <- Kbase of sequence b: double2 elements i, i + nt, ... below hi (four independent 16-byte loads in flight per
+// thread).  Whole matrix inside chd_k_kkt on the first iteration of a stage, one slice per CTA in chd_k_kcopy.
+__device__ __forceinline__ void chd_kwork_copy(const ChdDev& D, int b, size_t i, size_t hi, size_t nt) {
+  const double2* src = reinterpret_cast<const double2*>(D.Kbase + (size_t)b * D.kstride);
+  double2* dst = reinterpret_cast<double2*>(D.Kwork + (size_t)b * D.kstride);
+  for (; i + 3 * nt < hi; i += 4 * nt) {
+    const double2 v0 = src[i], v1 = src[i + nt], v2 = src[i + 2 * nt], v3 = src[i + 3 * nt];
+    dst[i] = v0, dst[i + nt] = v1, dst[i + 2 * nt] = v2, dst[i + 3 * nt] = v3;
+  }
+  for (; i < hi; i += nt) dst[i] = src[i];
+}
+
+// What every phase of chd_k_kkt sees of its sequence: the thread's place in the CTA, the sequence's arrays and KKT
+// storage, the sizes of the current stage, the carve-up of the dynamic shared memory (doubles)
+//   red[CHD_KKT_THREADS] | cc[nbp8*nbp8] | ypan[(Q+nbt)*64] | xpan[(Q+nbt)*64] ... (pan_doubles from ypan) | dinv[16]
+//   | win[win_tiles * 64] | bwin[Q*nbt*64]            (the last two in global scratch when they do not fit)
+// and the barrier parameter / step rules decided by the error measures.  (The solution vector D.sol is addressed by
+// each phase that uses it: a pointer held across the factorisation costs spills.)
+struct ChdKktCtx {
+  int b, tid, nt, lane, warp, nwarp;
+  ChdIpm* I;
+  int pre_refreshed;   // Kwork = Kbase + distance-row curvature already prepared on the side stream
+  ChdStageDev sg;
+  const ChdSeq* h;
+  int n, m, n_act, Qs, Q, nbt, nbp8, nbl, nbc, NBR, nbt_s;
+  size_t ro, vo, n_even, xs_len, win_region;
+  const int *rf, *vk, *rk, *ep, *ec;
+  const double *Jv, *grad;
   ChdKT K;
-  double* kw = D.Kwork + (size_t)b * D.kstride;
-  chd_kt_init(D, h, kw, K);
+  double *red, *cc, *ypan, *xpan, *dinv, *win, *bwin, *vecn, *xs, *xs2;
+  double sf, mu, tau, delta_w;
+  bool polish;
+};
+
+template <bool WS>
+__device__ __forceinline__ void chd_kkt_ctx_init(const ChdDev& D, ChdIpm& I, ChdKktCtx& c) {
+  extern __shared__ double sm[];
+  const int b = blockIdx.x;
+  c.b = b, c.I = &I;
+  c.pre_refreshed = I.kw_req;
+  c.sg = D.stages[I.stage];
+  const ChdSeq* h = c.h = D.seq + b;
+  c.n = h->n, c.m = h->m, c.tid = threadIdx.x, c.nt = blockDim.x;
+  c.lane = c.tid & 31, c.warp = c.tid >> 5, c.nwarp = c.nt >> 5;
+  c.ro = (size_t)b * D.m_max, c.vo = (size_t)b * D.n_max;
+  c.rf = D.rflag + c.ro;
+  c.vk = D.var_kkt + c.vo;
+  c.rk = D.row_kkt + c.ro;
+  c.ep = D.ent_ptr + (size_t)b * (D.m_max + 1);
+  c.ec = D.ent_col + (size_t)b * D.slots_max;
+  c.Jv = D.Jv + (size_t)b * D.slots_max;
+  c.grad = D.grad + c.vo;
+  ChdKT& K = c.K;
+  chd_kt_init(D, h, D.Kwork + (size_t)b * D.kstride, K);
   K.ovf = &I.band_ovf;
-  if (!sg.opt_dur) K.q = D.Qfix - 1;   // fixed-duration stages: the static pattern needs fewer band tiles than stage 3 may
-  // (below, Q is the number of block rows of the elimination window of this stage, Qs the storage stride of a block column)
-  const int n_act = sg.opt_dur ? n : n - h->n_dur;          // the durations (last n_dur entries of x) are unknowns in stage 3 only
-  const int Qs = K.Q, Q = sg.opt_dur ? K.Q : D.Qfix, nbt = K.nbt, nbp8 = K.nbp8, nbl = sg.opt_dur ? h->nb : h->nb_fix, nbc = K.nbc;
+  if (!c.sg.opt_dur) K.q = D.Qfix - 1;   // fixed-duration stages: the static pattern needs fewer band tiles than stage 3 may
+  // (Q is the number of block rows of the elimination window of this stage, Qs the storage stride of a block column)
+  c.n_act = c.sg.opt_dur ? c.n : c.n - h->n_dur;          // the durations (last n_dur entries of x) are unknowns in stage 3 only
+  c.Qs = K.Q, c.Q = c.sg.opt_dur ? K.Q : D.Qfix, c.nbt = K.nbt, c.nbp8 = K.nbp8, c.nbl = c.sg.opt_dur ? h->nb : h->nb_fix, c.nbc = K.nbc;
   // the right-hand side rides along as border row NBR, directly behind the border unknowns of this stage; nbt_s = border
   // tiles in use (the switch-time columns of stage 3 are all zero in the fixed-duration stages: not even looked at)
-  const int NBR = nbl, nbt_s = (nbl + 1 + 7) >> 3;
+  c.NBR = c.nbl, c.nbt_s = (c.nbl + 1 + 7) >> 3;
   // WS: everything in shared memory.  !WS (long horizons / very wide bands): only the reduction buffer, the
   // corner and the panel buffers stay in shared memory; the per-unknown vectors and the window live in a global
   // (L2 resident) scratch area  vecn | xs | xs2 | win | bwin.
-  const size_t n_even = (size_t)((D.n_max + 1) & ~1), xs_len = (size_t)(8 * D.nbc_max + nbp8);
+  c.n_even = (size_t)((D.n_max + 1) & ~1), c.xs_len = (size_t)(8 * D.nbc_max + c.nbp8);
   double* gs = WS ? nullptr : D.scratch + (size_t)b * D.scratch_stride;
-  double* red = sm;
-  double* cc = red + CHD_KKT_THREADS;
-  double* ypan = cc + nbp8 * nbp8;
-  double* xpan = ypan + (Q + nbt) * 64;
-  double* dinv = ypan + D.pan_doubles;
+  c.red = sm;
+  c.cc = c.red + CHD_KKT_THREADS;
+  c.ypan = c.cc + c.nbp8 * c.nbp8;
+  c.xpan = c.ypan + (c.Q + c.nbt) * 64;
+  c.dinv = c.ypan + D.pan_doubles;
   // WS: the per-unknown vectors vecn (step recovery) and xs (right-hand side before, solution after the factorisation)
   // alias the tail of the window region, which is dead whenever they are live (the right-hand side moves into the border
   // storage before the window is loaded; the back-substitution stages its tiles in the front part only)
-  const size_t win_region = (size_t)D.win_tiles * 64 + (size_t)Qs * nbt * 64;
-  double* win = WS ? dinv + 16 : gs + n_even + xs_len + 8 * (size_t)D.nbc_max;
-  double* bwin = win + (size_t)D.win_tiles * 64;
-  double* vecn = WS ? win + win_region - n_even : gs;
-  double* xs = WS ? vecn - xs_len : vecn + n_even;
-  double* xs2 = WS ? ypan : xs + xs_len;      // back-substitution accumulator (WS: aliases the then idle panel buffers)
-  const double sf = I.sf;
-  double mu = I.mu;
-  // per-phase cycle counters (scripts/prof_stage.py): compiled in only with -DCHD_PROFILE (extra barriers + clock reads)
-#ifdef CHD_PROFILE
-  long long tk0 = clock64();
-#define CHD_PROF(slot) do { __syncthreads(); if (tid == 0) { long long t_ = clock64(); I.prof[slot] += (double)(t_ - tk0); tk0 = t_; } } while (0)
-#else
-#define CHD_PROF(slot) do { } while (0)
-#endif
+  c.win_region = (size_t)D.win_tiles * 64 + (size_t)c.Qs * c.nbt * 64;
+  c.win = WS ? c.dinv + 16 : gs + c.n_even + c.xs_len + 8 * (size_t)D.nbc_max;
+  c.bwin = c.win + (size_t)D.win_tiles * 64;
+  c.vecn = WS ? c.win + c.win_region - c.n_even : gs;
+  c.xs = WS ? c.vecn - c.xs_len : c.vecn + c.n_even;
+  c.xs2 = WS ? c.ypan : c.xs + c.xs_len;      // back-substitution accumulator (WS: aliases the then idle panel buffers)
+  c.sf = I.sf;
+}
 
-  // ---------------- A. error measures, convergence, barrier update ----------------
+// A. error measures, convergence test, barrier update.  Returns true when the sequence has finished its stage (it has
+// moved on in the schedule); otherwise decides mu, tau and delta_w of this iteration.
+__device__ __forceinline__ bool chd_kkt_errors(const ChdDev& D, ChdKktCtx& c, int& s_fail) {
+  ChdIpm& I = *c.I;
+  const int b = c.b, tid = c.tid, nt = c.nt, n = c.n, m = c.m, n_act = c.n_act;
+  const size_t ro = c.ro, vo = c.vo;
+  const int *rf = c.rf, *vk = c.vk, *ep = c.ep, *ec = c.ec;
+  const double *Jv = c.Jv, *grad = c.grad, sf = c.sf;
+  double* red = c.red;
+  double mu = I.mu;
   // J^T y is gathered per variable from a column-oriented index of the Jacobian slots (no shared-memory fp64
   // atomics, which are compare-and-swap loops): per-row multipliers first, into the (idle) dy array
   const int* erow = D.ent_row + (size_t)b * D.slots_max;
@@ -532,7 +562,7 @@ __device__ __forceinline__ void chd_kkt_body(const ChdDev& D) {
     I.E0 = E0, I.viol_u = violu, I.dual_u = dual_u, I.compl_u = compl_u;
     I.status = new_status;
     s_fail = 0;
-    if (done) chd_stage_advance(D, I, new_status, sg.snap_after);
+    if (done) chd_stage_advance(D, I, new_status, c.sg.snap_after);
     if (!done) {
       I.mu = mu;
       I.tau = fmax(CHD_TAU_MIN, 1.0 - mu);
@@ -541,65 +571,197 @@ __device__ __forceinline__ void chd_kkt_body(const ChdDev& D) {
       I.theta0 = theta;
     }
   }
-  if (done) return;
-  const double tau = fmax(CHD_TAU_MIN, 1.0 - mu);
+  if (done) return true;
+  c.mu = mu;
+  c.tau = fmax(CHD_TAU_MIN, 1.0 - mu);
   // feasibility polish: every test but the unscaled constraint violation passes -> this step only restores feasibility
   // (a large Levenberg-Marquardt weight makes it the least-norm Newton correction of the constraints; the adaptive
   // weight itself is left alone)
-  const bool polish = E0 <= CHD_TOL && dual_u <= CHD_DUAL_INF_TOL && compl_u <= CHD_COMPL_INF_TOL && violu > CHD_CONSTR_VIOL_TOL &&
-                      I.delta_w < CHD_DW_POLISH;
-  const double delta_w = polish ? CHD_DW_POLISH : I.delta_w;
-  CHD_PROF(0);
+  c.polish = E0 <= CHD_TOL && dual_u <= CHD_DUAL_INF_TOL && compl_u <= CHD_COMPL_INF_TOL && violu > CHD_CONSTR_VIOL_TOL &&
+             I.delta_w < CHD_DW_POLISH;
+  c.delta_w = c.polish ? CHD_DW_POLISH : I.delta_w;
+  return false;
+}
 
-  // ---------------- B. assemble the KKT system ----------------
-  // Narrow inequality rows (<= 12 slots: terrain, friction pyramid, height) are condensed into the primal block
-  // (J^T Sigma J); wide ones (leg length) keep their multiplier as an unknown with diagonal
-  // -1/Sigma, which needs 36 instead of 666 matrix updates per row.  The right-hand side is accumulated in
-  // shared memory (xs) and written out once.
-  if (!pre_refreshed) {   // first iteration of a stage; afterwards chd_k_kcopy refreshes Kwork on the side stream
-    const double* base = D.Kbase + (size_t)b * D.kstride;
-    const double2* src = reinterpret_cast<const double2*>(base);
-    double2* dst = reinterpret_cast<double2*>(kw);
-    const size_t cnt2 = D.kstride / 2;
-    size_t i = tid;
-    for (; i + 3 * (size_t)nt < cnt2; i += 4 * (size_t)nt) {   // four independent 16-byte loads in flight per thread
-      const double2 v0 = src[i], v1 = src[i + nt], v2 = src[i + 2 * (size_t)nt], v3 = src[i + 3 * (size_t)nt];
-      dst[i] = v0, dst[i + nt] = v1, dst[i + 2 * (size_t)nt] = v2, dst[i + 3 * (size_t)nt] = v3;
-    }
-    for (; i < cnt2; i += nt) dst[i] = src[i];
-  }
+// B. assembly of the KKT system (the distance-row curvature terms follow separately, see chd_kkt_body).
+// Narrow inequality rows (<= 12 slots: terrain, friction pyramid, height) are condensed into the primal block
+// (J^T Sigma J); wide ones (leg length) keep their multiplier as an unknown with diagonal
+// -1/Sigma, which needs 36 instead of 666 matrix updates per row.  The right-hand side is accumulated in
+// shared memory (xs) and written out once.
+__device__ __forceinline__ void chd_kkt_assemble(const ChdDev& D, const ChdKktCtx& c) {
+  const ChdIpm& I = *c.I;
+  const ChdKT& K = c.K;
+  const int b = c.b, tid = c.tid, nt = c.nt, n_act = c.n_act, nbl = c.nbl, nbt = c.nbt, nbp8 = c.nbp8, NBR = c.NBR;
+  const int* vk = c.vk;
+  const double mu = c.mu;
+  if (!c.pre_refreshed) chd_kwork_copy(D, b, tid, D.kstride / 2, nt);   // first iteration of a stage; afterwards chd_k_kcopy refreshes Kwork on the side stream
   const int Na = K.Na;
-  double* rhs_s = xs;   // [0, Np) band unknowns, [8*nbc_max, +nb) border unknowns
+  double* rhs_s = c.xs;   // [0, Np) band unknowns, [8*nbc_max, +nb) border unknowns
   for (int i = tid; i < 8 * D.nbc_max + nbp8; i += nt) rhs_s[i] = 0.0;
   __syncthreads();
   // matrix entries do not depend on the barrier parameter: for sequences that continue in their stage they were
   // added by chd_k_asm (8 CTAs per sequence) before this kernel; the right-hand side (shared-memory atomics) is
   // always assembled here
-  if (pre_refreshed && polish) {   // chd_k_asm put the adaptive weight on the diagonal: top it up
-    const double extra = delta_w - I.delta_w;
+  if (c.pre_refreshed && c.polish) {   // chd_k_asm put the adaptive weight on the diagonal: top it up
+    const double extra = c.delta_w - I.delta_w;
     for (int i = tid; i < n_act; i += nt)
       if (vk[i] >= 0) chd_kadd(K, vk[i], vk[i], extra);
   }
-  if (pre_refreshed) {
+  if (c.pre_refreshed) {
     const double* r0 = D.rhs0 + (size_t)b * (D.Na_max + D.nb_max);
     const double* r1 = D.rhs1 + (size_t)b * (D.Na_max + D.nb_max);
     for (int i = tid; i < Na; i += nt) rhs_s[i] = r0[i] + mu * r1[i];
     for (int i = tid; i < nbl; i += nt) rhs_s[8 * D.nbc_max + i] = r0[D.Na_max + i] + mu * r1[D.Na_max + i];
   } else {
-    chd_assemble(D, b, K, delta_w, mu, sf, rhs_s, true, tid, nt);
+    chd_assemble(D, b, K, c.delta_w, mu, c.sf, rhs_s, true, tid, nt);
   }
   __syncthreads();
   for (int i = tid; i < K.Np; i += nt) K.bord[((size_t)(i >> 3) * nbt + (NBR >> 3)) * 64 + (NBR & 7) * 8 + (i & 7)] = i < Na ? rhs_s[i] : 0.0;
   for (int i = tid; i < nbl; i += nt) K.corn[(size_t)NBR * nbp8 + i] = rhs_s[8 * D.nbc_max + i];
-  CHD_PROF(1);
-  // y^+ * Jd^T Jd of the squared-distance rows: in-kernel only on the first iteration of a stage, afterwards
-  // chd_k_curv has already added them on the side stream (many CTAs per sequence: the atomics are the cost)
-  if (!pre_refreshed) chd_curv_rows(D, b, K, sg, warp, nwarp, lane, win + warp * 192);
-  __threadfence_block();
-  __syncthreads();
-  CHD_PROF(2);
+}
 
-  // ---------------- C. tiled band LDL^T with dense border ----------------
+// Trailing updates C -= X Y^T of one block column by the warps 1 .. nwarp-1, for at most 64 panel groups (every
+// shared-memory window; global windows of narrower bands).  2 x 2 register blocking over the compacted list of the groups
+// with a non-zero X tile: one trip loads the operand fragments of two panel rows (X) and two panel columns (Y) once and
+// updates up to four target tiles with them -- the loop is shared-memory bandwidth bound, this cuts the bytes per tile
+// update from 2 KB to 1.5 KB and the index work 4x.  cmp: this warp's rank -> group table.
+template <class BandTile, class BordTile>
+__device__ __forceinline__ void chd_kkt_update_compact(const ChdKktCtx& c, const unsigned short* s_pairs, unsigned char* cmp, const int* gnz,
+                                                       int GB, int Gm, int tq, const BandTile& band_tile, const BordTile& bord_tile) {
+  const int lane = c.lane, warp = c.warp, nbp8 = c.nbp8;
+  const double *xpan = c.xpan, *ypan = c.ypan;
+  // compact list of the groups with a non-zero X tile (every warp builds it redundantly: no extra barrier).
+  // the pair table enumerates (i >= j) row by row, so its first na(na+1)/2 entries pair the first na entries.
+  int na;
+  {
+    // up to 64 groups, two per lane; scatter by rank through a per-warp table (__fns is slow)
+    const int g1 = lane + 32;
+    const bool act0 = lane < Gm && (lane >= GB || lane < tq) && gnz[lane];
+    const bool act1 = g1 < Gm && (g1 >= GB || g1 < tq) && gnz[g1 < 96 ? g1 : 0];
+    const unsigned m0 = __ballot_sync(0xffffffffu, act0), m1 = __ballot_sync(0xffffffffu, act1);
+    const unsigned below = (1u << lane) - 1u;
+    const int n0 = __popc(m0);
+    na = n0 + __popc(m1);
+    if (act0) cmp[__popc(m0 & below)] = (unsigned char)lane;
+    if (act1) cmp[n0 + __popc(m1 & below)] = (unsigned char)g1;
+    __syncwarp();
+  }
+  auto corner = [&](const double* X, const double* Y, int bi, int bj) {   // corner block: same tensor-core update, row stride nbp8
+    double* Cc = c.cc + (size_t)(bi * 8 + (lane >> 2)) * nbp8 + bj * 8 + 2 * (lane & 3);
+    double c0 = Cc[0], c1 = Cc[1];
+    chd_tile_mma(c0, c1, X, Y, lane);
+    Cc[0] = c0, Cc[1] = c1;
+  };
+  const int step = c.nwarp - 1, r8 = (lane >> 2) * 8 + 2 * (lane & 3);
+  const int nb2 = (na + 1) >> 1, nblk = nb2 * (nb2 + 1) / 2;
+  for (int p = warp - 1; p < nblk; p += step) {
+    const int bi = s_pairs[p] >> 8, bj = s_pairs[p] & 255;
+    const int i1 = 2 * bi + 1, j1 = 2 * bj + 1;
+    const bool vi1 = i1 < na, vj1 = j1 < na;
+    int gi[2], gj[2];
+    gi[0] = cmp[2 * bi], gi[1] = cmp[i1 & 63];
+    gj[0] = cmp[2 * bj], gj[1] = cmp[j1 & 63];
+    double2 xf[2], yf[2];
+    xf[0] = *reinterpret_cast<const double2*>(xpan + gi[0] * 64 + 2 * lane);
+    yf[0] = *reinterpret_cast<const double2*>(ypan + gj[0] * 64 + 2 * lane);
+    xf[1] = vi1 ? *reinterpret_cast<const double2*>(xpan + gi[1] * 64 + 2 * lane) : make_double2(0.0, 0.0);
+    yf[1] = vj1 ? *reinterpret_cast<const double2*>(ypan + gj[1] * 64 + 2 * lane) : make_double2(0.0, 0.0);
+    double* Cp[4];
+    double2 cv[4];
+#pragma unroll
+    for (int t = 0; t < 4; ++t) {
+      const int a = t & 1, cl = t >> 1;          // tile (row a, column cl) of the block
+      bool ok = (a == 0 || vi1) && (cl == 0 || vj1) && !(bi == bj && a == 0 && cl == 1);
+      const int g_i = gi[a], g_j = gj[cl];
+      ok = ok && !(g_i == 0 && g_j == 0);       // the next diagonal tile is updated by warp 0
+      Cp[t] = nullptr;
+      if (ok) {
+        if (g_i < GB) Cp[t] = band_tile(g_i, g_j);
+        else if (g_j < GB) Cp[t] = bord_tile(g_i - GB, g_j);
+        else corner(xpan + g_i * 64, ypan + g_j * 64, g_i - GB, g_j - GB);
+      }
+      if (Cp[t]) cv[t] = *reinterpret_cast<const double2*>(Cp[t] + r8);
+    }
+#pragma unroll
+    for (int t = 0; t < 4; ++t)
+      if (Cp[t]) {
+        const double2 xa = xf[t & 1], yb = yf[t >> 1];
+        asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};"
+                     : "+d"(cv[t].x), "+d"(cv[t].y)
+                     : "d"(-xa.x), "d"(yb.x));
+      }
+#pragma unroll
+    for (int t = 0; t < 4; ++t)
+      if (Cp[t]) {
+        const double2 xa = xf[t & 1], yb = yf[t >> 1];
+        asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};"
+                     : "+d"(cv[t].x), "+d"(cv[t].y)
+                     : "d"(-xa.y), "d"(yb.y));
+        *reinterpret_cast<double2*>(Cp[t] + r8) = cv[t];
+      }
+  }
+}
+
+// Trailing updates of one block column by the warps 1 .. nwarp-1 with more than 64 panel groups (window in global (L2)
+// memory): each warp collects up to four target tiles from the full pair table, issues all their loads, and only then
+// runs the tensor-core updates and the stores.  (With the window in shared memory the simple loop was faster on the
+// benchmark batch.)
+template <class BandTile, class BordTile>
+__device__ __forceinline__ void chd_kkt_update_wide(const ChdKktCtx& c, const unsigned short* s_pairs, const int* gnz, int GB, int npairs,
+                                                    int tq, const BandTile& band_tile, const BordTile& bord_tile) {
+  const int lane = c.lane, nwarp = c.nwarp, nbp8 = c.nbp8;
+  const double *xpan = c.xpan, *ypan = c.ypan;
+  double* cc = c.cc;
+  const int r8 = (lane >> 2) * 8 + 2 * (lane & 3);
+  int p = c.warp - 1;
+  while (p < npairs) {
+    // target tiles and their operands; one array of structs, not three pointer arrays: an array of the compact loop's
+    // type double*[4] gets merged with its Cp when both loops are inlined, which puts that one in local memory as well
+    struct { double* C; const double *X, *Y; } tl[4];
+    int nq = 0;
+    while (nq < 4 && p < npairs) {
+      const int gi = s_pairs[p] >> 8, gj = s_pairs[p] & 255;
+      p += nwarp - 1;
+      if ((gi < GB && gi >= tq) || (gj < GB && gj >= tq) || !gnz[gi] || !gnz[gj]) continue;
+      if (gi == 0 && gj == 0) continue;
+      const double* X = xpan + gi * 64;
+      const double* Y = ypan + gj * 64;
+      if (gi < GB) {
+        tl[nq].C = band_tile(gi, gj), tl[nq].X = X, tl[nq].Y = Y, ++nq;
+      } else if (gj < GB) {
+        tl[nq].C = bord_tile(gi - GB, gj), tl[nq].X = X, tl[nq].Y = Y, ++nq;
+      } else {
+        const int bi = gi - GB, bj = gj - GB;
+        for (int e = lane; e < 64; e += 32) {
+          const int r = e >> 3, cq = e & 7;
+          double acc = 0.0;
+#pragma unroll
+          for (int kk = 0; kk < 8; ++kk) acc += X[r * 8 + kk] * Y[cq * 8 + kk];
+          cc[(bi * 8 + r) * nbp8 + bj * 8 + cq] -= acc;
+        }
+      }
+    }
+    double c0[4], c1[4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+      if (i < nq) c0[i] = tl[i].C[r8], c1[i] = tl[i].C[r8 + 1];
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+      if (i < nq) {
+        chd_tile_mma(c0[i], c1[i], tl[i].X, tl[i].Y, lane);
+        tl[i].C[r8] = c0[i], tl[i].C[r8 + 1] = c1[i];
+      }
+  }
+}
+
+// C. tiled band LDL^T with dense border, block column by block column: panel, stream-in of the next block row, trailing
+// updates.  Sets s_fail on a bad pivot of a diagonal tile.
+template <bool WS>
+__device__ __forceinline__ void chd_kkt_factor(const ChdKktCtx& c, int& s_fail) {
+  const ChdKT& K = c.K;
+  const int tid = c.tid, nt = c.nt, lane = c.lane, warp = c.warp, nwarp = c.nwarp;
+  const int Qs = c.Qs, Q = c.Q, nbt = c.nbt, nbp8 = c.nbp8, nbc = c.nbc, nbt_s = c.nbt_s;
+  double *cc = c.cc, *ypan = c.ypan, *xpan = c.xpan, *dinv = c.dinv, *win = c.win, *bwin = c.bwin;
   // corner (incl. rhs row) to shared memory; initial window: band tiles (I, J), 0 <= J <= I <= q and border columns 0..q
   for (int i = tid; i < nbp8 * nbp8; i += nt) cc[i] = K.corn[i];
   // (without the shared-memory window the factorisation runs in place on Kwork: no window copy, no stream-in)
@@ -621,10 +783,6 @@ __device__ __forceinline__ void chd_kkt_body(const ChdDev& D) {
   __shared__ unsigned short s_pairs[3000];
   __shared__ unsigned char s_cmp[CHD_KKT_THREADS / 32][64];   // per warp: rank -> id of the non-zero panel groups
   __shared__ __align__(16) double s_winv[2][64];   // inverse of the current / next diagonal tile factor, fragment order
-  __shared__ __align__(8) unsigned long long s_mbar;   // completion of the TMA bulk stream-in of one block row
-  unsigned mbar_phase = 0;
-  const bool use_tma = WS && D.tma;
-  if (use_tma && tid == 0) chd_mbar_init(&s_mbar, 1);
   const int GB = K.q, Gm = K.q + nbt_s, npairs = Gm * (Gm + 1) / 2;
   for (int p = tid; p < npairs && p < 3000; p += nt) {
     int gi = (int)((sqrt(8.0 * p + 1.0) - 1.0) * 0.5);
@@ -641,13 +799,7 @@ __device__ __forceinline__ void chd_kkt_body(const ChdDev& D) {
   }
   __syncthreads();
   int kslot = 0, cur = 0;  // kslot = Kc % Q
-#ifdef CHD_PROFILE
-  long long pf_a = 0, pf_b = 0, pf_c = 0, pf_acc[3] = {0, 0, 0};
-#endif
   for (int Kc = 0; Kc < nbc; ++Kc, cur ^= 1) {
-#ifdef CHD_PROFILE
-    pf_a = clock64();
-#endif
     const int tq = min(K.q, nbc - 1 - Kc);          // band tiles below the diagonal tile
     const int* rs = s_rs[cur];
     // tile addresses: circular triangular window in shared memory, or in place in the global band / border storage
@@ -693,17 +845,12 @@ __device__ __forceinline__ void chd_kkt_body(const ChdDev& D) {
     if (WS)
       for (int e = tid; e < 64; e += nt) K.band[(size_t)Kc * Qs * 64 + e] = Tkk[e];
     __syncthreads();
-#ifdef CHD_PROFILE
-    pf_b = clock64();
-#endif
     // (c) stream in block row Kc + Q (its slots are dead now), trailing updates on the fp64 tensor core;
     //     warp 0 takes the pair that completes the next diagonal tile and factors it right away
     const int In = Kc + Q;
-    // Two stream-in variants (D.tma, environment CHD_TMA at batch creation; benchmark batch on an H100 SXM at 400 W:
-    // 1.14 ms per launch with the per-thread cp.async chunks, 1.22 ms with the TMA producer warp; bulk copies issued by a
-    // lane of an updating warp and dynamically dealt update blocks were slower still when tried):
-    if (WS && !use_tma && In < nbc) {
-      // 16-byte cp.async chunks by the warps 1..15; warp 0 goes straight to the diagonal tile
+    if (WS && In < nbc) {
+      // 16-byte cp.async chunks by the warps 1..15; warp 0 goes straight to the diagonal tile.  (A TMA producer warp, bulk
+      // copies issued by a lane of an updating warp and dynamically dealt update blocks were slower: DESIGN.md section 9)
       for (int idx = tid - 32; idx < Q * 32 + nbt_s * 32; idx += nt - 32) {
         if (idx < 0) break;
         const int tile = idx >> 5, off = (idx & 31) * 2;
@@ -716,22 +863,6 @@ __device__ __forceinline__ void chd_kkt_body(const ChdDev& D) {
         }
       }
     }
-    // TMA variant: the last warp is the producer of the shared-memory window -- it only streams (the trailing updates
-    // are dealt to the warps 1 .. nwarp-2), so no warp of the update loop is held up by the serial issue of the copies
-    const bool producer = use_tma && warp == nwarp - 1;
-    if (producer && In < nbc && lane == 0) {
-      // TMA bulk copies (cp.async.bulk + mbarrier): one thread streams the Q band tiles of block row In (512 contiguous
-      // bytes each in the block-column storage) and its border tiles (one contiguous piece) into the slots the pivot
-      // block row just vacated; the slots were last touched through the generic proxy (panel phase, before the barrier)
-      chd_fence_async_smem();
-      chd_mbar_expect(&s_mbar, (unsigned)((Q + nbt_s) * 512));
-      for (int tile = 0; tile < Q; ++tile) {
-        const int J = tile < GB ? Kc + 1 + tile : In;
-        double* dst = tile < GB ? win + (size_t)tri(kslot, rs[tile]) * 64 : Tkk;
-        chd_bulk_g2s(dst, K.band + ((size_t)J * Qs + (In - J)) * 64, 512u, &s_mbar);
-      }
-      chd_bulk_g2s(Bk, K.bord + (size_t)In * nbt * 64, (unsigned)(nbt_s * 512), &s_mbar);
-    }
     if (warp == 0) {
       if (tq >= 1) {
         double* Tn = band_tile(0, 0);
@@ -740,7 +871,7 @@ __device__ __forceinline__ void chd_kkt_body(const ChdDev& D) {
         const bool ok = chd_tile_ldl(Tn, dinv + 8 * (cur ^ 1), s_winv[cur ^ 1], lane);
         if (!ok && lane == 0) s_fail = 1;
       }
-    } else if (!producer) {
+    } else {
       if (warp == 1) {
         for (int g = lane; g < GB; g += 32) {   // slot table of the next block column
           int v = kslot + 2 + g;
@@ -749,209 +880,21 @@ __device__ __forceinline__ void chd_kkt_body(const ChdDev& D) {
         }
         for (int g = lane; g < Gm; g += 32) s_gnz[cur ^ 1][g] = 0;
       }
-      // compact list of the groups with a non-zero X tile (every warp builds it redundantly: no extra barrier).
-      // the pair table enumerates (i >= j) row by row, so its first na(na+1)/2 entries pair the first na entries.
-      const int* gnz = s_gnz[cur];
-      int na;
-      const unsigned char* cmp = s_cmp[warp];
-      {
-        // up to 64 groups, two per lane; scatter by rank through a per-warp table (__fns is slow)
-        const int g1 = lane + 32;
-        const bool act0 = lane < Gm && (lane >= GB || lane < tq) && gnz[lane];
-        const bool act1 = g1 < Gm && (g1 >= GB || g1 < tq) && gnz[g1 < 96 ? g1 : 0];
-        const unsigned m0 = __ballot_sync(0xffffffffu, act0), m1 = __ballot_sync(0xffffffffu, act1);
-        const unsigned below = (1u << lane) - 1u;
-        const int n0 = __popc(m0);
-        na = n0 + __popc(m1);
-        if (act0) s_cmp[warp][__popc(m0 & below)] = (unsigned char)lane;
-        if (act1) s_cmp[warp][n0 + __popc(m1 & below)] = (unsigned char)g1;
-        __syncwarp();
-      }
-      const bool compact = Gm <= 64;
-      const int np_loop = compact ? na * (na + 1) / 2 : npairs;
-      if (!WS && !compact) {
-        // more than 64 panel groups, window in global (L2) memory: each warp collects up to four target tiles, issues all their loads, and only
-        // then runs the tensor-core updates and the stores.  (With the window in shared memory the simple loop below
-        // was faster on the benchmark batch.)
-        const int r8 = (lane >> 2) * 8 + 2 * (lane & 3);
-        int p = warp - 1;
-        while (p < np_loop) {
-          double* Cp[4];
-          const double *Xp[4], *Yp[4];
-          int nq = 0;
-          while (nq < 4 && p < np_loop) {
-            const int ai = s_pairs[p] >> 8, aj = s_pairs[p] & 255;
-            p += nwarp - 1;
-            int gi, gj;
-            if (compact) {
-              gi = cmp[ai], gj = cmp[aj];
-            } else {
-              gi = ai, gj = aj;
-              if ((gi < GB && gi >= tq) || (gj < GB && gj >= tq) || !gnz[gi] || !gnz[gj]) continue;
-            }
-            if (gi == 0 && gj == 0) continue;
-            const double* X = xpan + gi * 64;
-            const double* Y = ypan + gj * 64;
-            if (gi < GB) {
-              Cp[nq] = band_tile(gi, gj), Xp[nq] = X, Yp[nq] = Y, ++nq;
-            } else if (gj < GB) {
-              Cp[nq] = bord_tile(gi - GB, gj), Xp[nq] = X, Yp[nq] = Y, ++nq;
-            } else {
-              const int bi = gi - GB, bj = gj - GB;
-              for (int e = lane; e < 64; e += 32) {
-                const int r = e >> 3, cq = e & 7;
-                double acc = 0.0;
-#pragma unroll
-                for (int kk = 0; kk < 8; ++kk) acc += X[r * 8 + kk] * Y[cq * 8 + kk];
-                cc[(bi * 8 + r) * nbp8 + bj * 8 + cq] -= acc;
-              }
-            }
-          }
-          double c0[4], c1[4];
-#pragma unroll
-          for (int i = 0; i < 4; ++i)
-            if (i < nq) c0[i] = Cp[i][r8], c1[i] = Cp[i][r8 + 1];
-#pragma unroll
-          for (int i = 0; i < 4; ++i)
-            if (i < nq) {
-              chd_tile_mma(c0[i], c1[i], Xp[i], Yp[i], lane);
-              Cp[i][r8] = c0[i], Cp[i][r8 + 1] = c1[i];
-            }
-        }
-      } else {
-        // window in shared memory: two target tiles per loop trip with interleaved tensor-core updates (the dependent
-        // chain index -> tile address -> load -> 2 x DMMA -> store of a single tile leaves the pipe idle most of the time)
-        auto decode = [&](int p, double*& C, const double*& X, const double*& Y, int& bi, int& bj) -> int {
-          const int ai = s_pairs[p] >> 8, aj = s_pairs[p] & 255;
-          int gi, gj;
-          if (compact) {
-            gi = cmp[ai], gj = cmp[aj];
-          } else {
-            gi = ai, gj = aj;
-            if ((gi < GB && gi >= tq) || (gj < GB && gj >= tq) || !gnz[gi] || !gnz[gj]) return 0;
-          }
-          if (gi == 0 && gj == 0) return 0;   // the next diagonal tile is updated by warp 0
-          X = xpan + gi * 64;
-          Y = ypan + gj * 64;
-          if (gi < GB) {
-            C = band_tile(gi, gj);
-            return 1;
-          }
-          if (gj < GB) {
-            C = bord_tile(gi - GB, gj);
-            return 1;
-          }
-          bi = gi - GB, bj = gj - GB;
-          return 2;
-        };
-        auto corner = [&](const double* X, const double* Y, int bi, int bj) {   // corner block: same tensor-core update, row stride nbp8
-          double* Cc = cc + (size_t)(bi * 8 + (lane >> 2)) * nbp8 + bj * 8 + 2 * (lane & 3);
-          double c0 = Cc[0], c1 = Cc[1];
-          chd_tile_mma(c0, c1, X, Y, lane);
-          Cc[0] = c0, Cc[1] = c1;
-        };
-        const int step = use_tma ? nwarp - 2 : nwarp - 1, r8 = (lane >> 2) * 8 + 2 * (lane & 3);
-        if (compact) {
-          // 2 x 2 register blocking over the compacted group list: one trip loads the operand fragments of two panel
-          // rows (X) and two panel columns (Y) once and updates up to four target tiles with them -- the loop is
-          // shared-memory bandwidth bound, this cuts the bytes per tile update from 2 KB to 1.5 KB and the index work 4x
-          const int nb2 = (na + 1) >> 1, nblk = nb2 * (nb2 + 1) / 2;
-          for (int p = warp - 1; p < nblk; p += step) {
-            const int bi = s_pairs[p] >> 8, bj = s_pairs[p] & 255;
-            const int i1 = 2 * bi + 1, j1 = 2 * bj + 1;
-            const bool vi1 = i1 < na, vj1 = j1 < na;
-            int gi[2], gj[2];
-            gi[0] = cmp[2 * bi], gi[1] = cmp[i1 & 63];
-            gj[0] = cmp[2 * bj], gj[1] = cmp[j1 & 63];
-            double2 xf[2], yf[2];
-            xf[0] = *reinterpret_cast<const double2*>(xpan + gi[0] * 64 + 2 * lane);
-            yf[0] = *reinterpret_cast<const double2*>(ypan + gj[0] * 64 + 2 * lane);
-            xf[1] = vi1 ? *reinterpret_cast<const double2*>(xpan + gi[1] * 64 + 2 * lane) : make_double2(0.0, 0.0);
-            yf[1] = vj1 ? *reinterpret_cast<const double2*>(ypan + gj[1] * 64 + 2 * lane) : make_double2(0.0, 0.0);
-            double* Cp[4];
-            double2 cv[4];
-#pragma unroll
-            for (int t = 0; t < 4; ++t) {
-              const int a = t & 1, c = t >> 1;          // tile (row a, column c) of the block
-              bool ok = (a == 0 || vi1) && (c == 0 || vj1) && !(bi == bj && a == 0 && c == 1);
-              const int g_i = gi[a], g_j = gj[c];
-              ok = ok && !(g_i == 0 && g_j == 0);       // the next diagonal tile is updated by warp 0
-              Cp[t] = nullptr;
-              if (ok) {
-                if (g_i < GB) Cp[t] = band_tile(g_i, g_j);
-                else if (g_j < GB) Cp[t] = bord_tile(g_i - GB, g_j);
-                else corner(xpan + g_i * 64, ypan + g_j * 64, g_i - GB, g_j - GB);
-              }
-              if (Cp[t]) cv[t] = *reinterpret_cast<const double2*>(Cp[t] + r8);
-            }
-#pragma unroll
-            for (int t = 0; t < 4; ++t)
-              if (Cp[t]) {
-                const double2 xa = xf[t & 1], yb = yf[t >> 1];
-                asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};"
-                             : "+d"(cv[t].x), "+d"(cv[t].y)
-                             : "d"(-xa.x), "d"(yb.x));
-              }
-#pragma unroll
-            for (int t = 0; t < 4; ++t)
-              if (Cp[t]) {
-                const double2 xa = xf[t & 1], yb = yf[t >> 1];
-                asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};"
-                             : "+d"(cv[t].x), "+d"(cv[t].y)
-                             : "d"(-xa.y), "d"(yb.y));
-                *reinterpret_cast<double2*>(Cp[t] + r8) = cv[t];
-              }
-          }
-        } else
-        for (int p = warp - 1; p < np_loop; p += 2 * step) {
-          double *C1 = nullptr, *C2 = nullptr;
-          const double *X1 = nullptr, *Y1 = nullptr, *X2 = nullptr, *Y2 = nullptr;
-          int b1i = 0, b1j = 0, b2i = 0, b2j = 0;
-          const int k1 = decode(p, C1, X1, Y1, b1i, b1j);
-          const int k2 = p + step < np_loop ? decode(p + step, C2, X2, Y2, b2i, b2j) : 0;
-          if (k1 == 1 && k2 == 1) {
-            double2 c1 = *reinterpret_cast<const double2*>(C1 + r8), c2 = *reinterpret_cast<const double2*>(C2 + r8);
-            const double2 xa1 = *reinterpret_cast<const double2*>(X1 + 2 * lane), yb1 = *reinterpret_cast<const double2*>(Y1 + 2 * lane);
-            const double2 xa2 = *reinterpret_cast<const double2*>(X2 + 2 * lane), yb2 = *reinterpret_cast<const double2*>(Y2 + 2 * lane);
-            asm volatile(
-                "mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%4}, {%5}, {%0,%1};\n\t"
-                "mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%2,%3}, {%6}, {%7}, {%2,%3};\n\t"
-                "mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%8}, {%9}, {%0,%1};\n\t"
-                "mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%2,%3}, {%10}, {%11}, {%2,%3};"
-                : "+d"(c1.x), "+d"(c1.y), "+d"(c2.x), "+d"(c2.y)
-                : "d"(-xa1.x), "d"(yb1.x), "d"(-xa2.x), "d"(yb2.x), "d"(-xa1.y), "d"(yb1.y), "d"(-xa2.y), "d"(yb2.y));
-            *reinterpret_cast<double2*>(C1 + r8) = c1;
-            *reinterpret_cast<double2*>(C2 + r8) = c2;
-          } else {
-            if (k1 == 1) chd_tile_sub_xyT(C1, X1, Y1, lane);
-            if (k2 == 1) chd_tile_sub_xyT(C2, X2, Y2, lane);
-          }
-          if (k1 == 2) corner(X1, Y1, b1i, b1j);
-          if (k2 == 2) corner(X2, Y2, b2i, b2j);
-        }
-      }
+      // every shared-memory window has Gm <= 64 (batch creation checks Q - 1 + nbt <= 64)
+      if (!WS && Gm > 64) chd_kkt_update_wide(c, s_pairs, s_gnz[cur], GB, npairs, tq, band_tile, bord_tile);
+      else chd_kkt_update_compact(c, s_pairs, s_cmp[warp], s_gnz[cur], GB, Gm, tq, band_tile, bord_tile);
     }
-#ifdef CHD_PROFILE
-    pf_c = clock64();
-#endif
-    if (use_tma && In < nbc) {
-      chd_mbar_wait(&s_mbar, mbar_phase);
-      mbar_phase ^= 1u;
-    } else {
-      chd_copy_wait(WS);
-    }
+    chd_copy_wait(WS);
     __syncthreads();
     kslot = kslot + 1 == Q ? 0 : kslot + 1;
-#ifdef CHD_PROFILE
-    { const long long t_ = clock64(); pf_acc[0] += pf_b - pf_a, pf_acc[1] += pf_c - pf_b, pf_acc[2] += t_ - pf_c; }
-#endif
   }
-#ifdef CHD_PROFILE
-  if (tid == 32) I.dbg[0] += (double)pf_acc[0], I.dbg[1] += (double)pf_acc[1], I.dbg[2] += (double)pf_acc[2];   // warp 1: panel+barrier | own updates | wait+barrier
-  if (tid == 0) I.dbg[3] += (double)pf_acc[0], I.dbg[4] += (double)pf_acc[1], I.dbg[5] += (double)pf_acc[2];    // warp 0: panel+barrier | diagonal tile | wait+barrier
-#endif
-  CHD_PROF(3);
-  // dense LDL^T of the border Schur complement S = cc[0..nbl)^2 and solve S xb = rb (rb = row NBR of cc)
+}
+
+// dense LDL^T of the border Schur complement S = cc[0..nbl)^2 and solve S xb = rb (rb = row NBR of cc); xb goes to
+// xs[8*nbc_max ..) and to the solution vector.  Sets s_fail on a bad pivot.
+__device__ __forceinline__ void chd_kkt_border(const ChdDev& D, const ChdKktCtx& c, int& s_fail) {
+  const int tid = c.tid, nt = c.nt, lane = c.lane, warp = c.warp, nbl = c.nbl, nbp8 = c.nbp8, NBR = c.NBR, Na = c.K.Na;
+  double* cc = c.cc;
   for (int k = 0; k < nbl; ++k) {
     const double dk = cc[k * nbp8 + k];
     if (tid == 0 && !(dk > 0.0 && isfinite(dk))) s_fail = 1;
@@ -965,7 +908,7 @@ __device__ __forceinline__ void chd_kkt_body(const ChdDev& D) {
     for (int j = k + 1 + tid; j < nbl; j += nt) cc[NBR * nbp8 + j] -= cc[j * nbp8 + k] * ik * cc[NBR * nbp8 + k];
     __syncthreads();
   }
-  double* xb = xs + 8 * D.nbc_max;  // border solution
+  double* xb = c.xs + 8 * D.nbc_max;  // border solution
   if (warp == 0) {
     // column-oriented back-substitution by one warp: x_k = acc_k / d_k, then acc_j -= (L d)[k][j] x_k for j < k
     // (row k of cc holds the unscaled column entries; one division per unknown instead of one per matrix entry)
@@ -980,88 +923,100 @@ __device__ __forceinline__ void chd_kkt_body(const ChdDev& D) {
     }
   }
   __syncthreads();
-  double* sol = D.sol + (size_t)b * (D.Na_max + D.nb_max);
-  for (int i = tid; i < nbl; i += nt) sol[Na + i] = xb[i];
-  CHD_PROF(4);
-  // backward substitution, column oriented: acc = u - Lb^T xb; for K descending: x_K = L0^-T acc_K (warp 0),
-  // then acc_J -= L(K,J)^T x_K for the block row K (all threads).  Tiles are staged two block rows ahead.
-  {
-    double* accv = xpan;                  // panel buffers are free now; accv needs 8*nbc doubles <= (Q+nbt)*64? no -> use xs2
-    accv = xs2;
-    for (int i = tid; i < K.Np; i += nt) {
-      const double* bt = K.bord + (size_t)(i >> 3) * nbt * 64 + (i & 7);
-      double v = bt[NBR * 8];
-      for (int q2 = 0; q2 < nbl; ++q2) v -= bt[q2 * 8] * xb[q2];
-      accv[i] = v;
+  for (int i = tid; i < nbl; i += nt) D.sol[(size_t)c.b * (D.Na_max + D.nb_max) + Na + i] = xb[i];
+}
+
+// backward substitution of the band, column oriented: acc = u - Lb^T xb; for K descending: x_K = L0^-T acc_K (warp 0),
+// then acc_J -= L(K,J)^T x_K for the block row K (all threads).  Tiles are staged two block rows ahead.  The band
+// solution goes to xs and to the solution vector.
+template <bool WS>
+__device__ __forceinline__ void chd_kkt_backsub(const ChdDev& D, const ChdKktCtx& c) {
+  const ChdKT& K = c.K;
+  const int tid = c.tid, nt = c.nt, lane = c.lane, warp = c.warp, Q = c.Q, Qs = c.Qs, nbt = c.nbt, nbl = c.nbl, nbc = c.nbc;
+  const int NBR = c.NBR, Na = K.Na;
+  double *xs = c.xs, *sol = D.sol + (size_t)c.b * (D.Na_max + D.nb_max);
+  const double* xb = xs + 8 * D.nbc_max;
+  double* accv = c.xs2;
+  for (int i = tid; i < K.Np; i += nt) {
+    const double* bt = K.bord + (size_t)(i >> 3) * nbt * 64 + (i & 7);
+    double v = bt[NBR * 8];
+    for (int q2 = 0; q2 < nbl; ++q2) v -= bt[q2 * 8] * xb[q2];
+    accv[i] = v;
+  }
+  // staging buffers in the (now free) window + border window: two chunks of R block rows each,
+  // row slot = diag tile | tiles (K, K-1-g), g = 0..q-1.  Warp 0 alone walks through a chunk (the recursion is
+  // sequential anyway; without block barriers a block row costs ~0.5 k cycles instead of 1.4 k) while the other
+  // warps prefetch the next chunk; one barrier per chunk.
+  const int per = Q * 64;
+  const int R = max(1, (int)((c.win_region - (WS ? c.n_even + c.xs_len : 0)) / 64) / (2 * Q));
+  double* stg = c.win;
+  auto stage_chunk = [&](int Ktop, int buf, int t0, int tstep) {   // block rows Ktop, Ktop-1, ... (R of them)
+    for (int idx = t0; idx < R * Q * 32; idx += tstep) {
+      const int rr = idx / (Q * 32), rem = idx - rr * (Q * 32);
+      const int Kr = Ktop - rr;
+      if (Kr < 0) break;
+      const int tile = rem >> 5, off = (rem & 31) * 2;
+      const int J = tile == 0 ? Kr : Kr - tile;     // tile 0: diagonal; tile g+1: (Kr, Kr-1-g)
+      if (J < 0) continue;
+      chd_copy16(stg + ((size_t)buf * R + rr) * per + tile * 64 + off, K.band + ((size_t)J * Qs + (Kr - J)) * 64 + off, WS);
     }
-    // staging buffers in the (now free) window + border window: two chunks of R block rows each,
-    // row slot = diag tile | tiles (K, K-1-g), g = 0..q-1.  Warp 0 alone walks through a chunk (the recursion is
-    // sequential anyway; without block barriers a block row costs ~0.5 k cycles instead of 1.4 k) while the other
-    // warps prefetch the next chunk; one barrier per chunk.
-    const int per = Q * 64;
-    const int R = max(1, (int)((win_region - (WS ? n_even + xs_len : 0)) / 64) / (2 * Q));
-    double* stg = win;
-    auto stage_chunk = [&](int Ktop, int buf, int t0, int tstep) {   // block rows Ktop, Ktop-1, ... (R of them)
-      for (int idx = t0; idx < R * Q * 32; idx += tstep) {
-        const int rr = idx / (Q * 32), rem = idx - rr * (Q * 32);
-        const int Kr = Ktop - rr;
-        if (Kr < 0) break;
-        const int tile = rem >> 5, off = (rem & 31) * 2;
-        const int J = tile == 0 ? Kr : Kr - tile;     // tile 0: diagonal; tile g+1: (Kr, Kr-1-g)
-        if (J < 0) continue;
-        chd_copy16(stg + ((size_t)buf * R + rr) * per + tile * 64 + off, K.band + ((size_t)J * Qs + (Kr - J)) * 64 + off, WS);
+  };
+  stage_chunk(nbc - 1, 0, tid, nt);
+  chd_copy_wait(WS);
+  __syncthreads();
+  int buf = 0;
+  for (int Ktop = nbc - 1; Ktop >= 0; Ktop -= R, buf ^= 1) {
+    if (warp != 0) {
+      stage_chunk(Ktop - R, buf ^ 1, tid - 32, nt - 32);
+    } else {
+      for (int rr = 0; rr < R && Ktop - rr >= 0; ++rr) {
+        const int Kc = Ktop - rr;
+        const double* T0 = stg + ((size_t)buf * R + rr) * per;
+        double xk[8];
+#pragma unroll
+        for (int cl = 7; cl >= 0; --cl) {
+          double v = accv[Kc * 8 + cl];
+#pragma unroll
+          for (int p = 7; p > cl; --p) v -= T0[p * 8 + cl] * xk[p];   // oldest unknown first: only the last link waits for xk[cl+1]
+          xk[cl] = v;
+        }
+        if (lane < 8) {
+          const int gi = Kc * 8 + lane;
+          double v = xk[0];
+#pragma unroll
+          for (int cl = 1; cl < 8; ++cl) v = lane == cl ? xk[cl] : v;
+          xs[gi] = v;
+          if (gi < Na) sol[gi] = v;
+        }
+        const int nrow = min(K.q, Kc);   // tiles (Kc, Kc-1-g), g < nrow
+        for (int idx = lane; idx < nrow * 8; idx += 32) {
+          const int g = idx >> 3, cl = idx & 7;
+          const double* T = T0 + (g + 1) * 64;
+          double v = 0.0;
+#pragma unroll
+          for (int r = 0; r < 8; ++r) v += T[r * 8 + cl] * xk[r];
+          accv[(Kc - 1 - g) * 8 + cl] -= v;
+        }
+        __syncwarp();
       }
-    };
-    stage_chunk(nbc - 1, 0, tid, nt);
+    }
     chd_copy_wait(WS);
     __syncthreads();
-    int buf = 0;
-    for (int Ktop = nbc - 1; Ktop >= 0; Ktop -= R, buf ^= 1) {
-      if (warp != 0) {
-        stage_chunk(Ktop - R, buf ^ 1, tid - 32, nt - 32);
-      } else {
-        for (int rr = 0; rr < R && Ktop - rr >= 0; ++rr) {
-          const int Kc = Ktop - rr;
-          const double* T0 = stg + ((size_t)buf * R + rr) * per;
-          double xk[8];
-#pragma unroll
-          for (int c = 7; c >= 0; --c) {
-            double v = accv[Kc * 8 + c];
-#pragma unroll
-            for (int p = 7; p > c; --p) v -= T0[p * 8 + c] * xk[p];   // oldest unknown first: only the last link waits for xk[c+1]
-            xk[c] = v;
-          }
-          if (lane < 8) {
-            const int gi = Kc * 8 + lane;
-            double v = xk[0];
-#pragma unroll
-            for (int c = 1; c < 8; ++c) v = lane == c ? xk[c] : v;
-            xs[gi] = v;
-            if (gi < Na) sol[gi] = v;
-          }
-          const int nrow = min(K.q, Kc);   // tiles (Kc, Kc-1-g), g < nrow
-          for (int idx = lane; idx < nrow * 8; idx += 32) {
-            const int g = idx >> 3, c = idx & 7;
-            const double* T = T0 + (g + 1) * 64;
-            double v = 0.0;
-#pragma unroll
-            for (int r = 0; r < 8; ++r) v += T[r * 8 + c] * xk[r];
-            accv[(Kc - 1 - g) * 8 + c] -= v;
-          }
-          __syncwarp();
-        }
-      }
-      chd_copy_wait(WS);
-      __syncthreads();
-    }
   }
-  CHD_PROF(5);
+}
+
+// No step from this factorisation: a coupling left the band (the stage fails) or a pivot broke down (the regularisation
+// goes up and the iteration is repeated).  Returns true in either case.
+__device__ __forceinline__ bool chd_kkt_no_step(const ChdDev& D, const ChdKktCtx& c, const int& s_fail) {
+  ChdIpm& I = *c.I;
+  const int tid = c.tid, nt = c.nt, n = c.n, m = c.m;
+  const size_t ro = c.ro, vo = c.vo;
   if (I.band_ovf) {
     // a coupling left the band (stage 3 moved a polynomial boundary further than the layout allows): the stage fails and
     // the schedule goes on with the fixed-duration stage 4, as the reference does after a failed stage 3
     __syncthreads();
-    if (tid == 0) I.status = -2, chd_stage_advance(D, I, -2, sg.snap_after);
-    return;
+    if (tid == 0) I.status = -2, chd_stage_advance(D, I, -2, c.sg.snap_after);
+    return true;
   }
   if (s_fail) {
     // numerical breakdown: raise the primal regularisation and retry next iteration (no step is taken)
@@ -1071,15 +1026,24 @@ __device__ __forceinline__ void chd_kkt_body(const ChdDev& D) {
       I.ls_fail += 1;
       I.step_ready = 1;
       I.kw_req = 1;
-      if (I.delta_w > CHD_DW_MAX) I.status = -2, chd_stage_advance(D, I, -2, sg.snap_after);
+      if (I.delta_w > CHD_DW_MAX) I.status = -2, chd_stage_advance(D, I, -2, c.sg.snap_after);
     }
     for (int i = tid; i < n; i += nt) D.dx[vo + i] = 0.0;
     for (int r = tid; r < m; r += nt) D.ds[ro + r] = 0.0, D.dy[ro + r] = 0.0, D.dzL[ro + r] = 0.0, D.dzU[ro + r] = 0.0;
-    return;
+    return true;
   }
-  __syncthreads();
+  return false;
+}
 
-  // ---------------- D. recover the full step, fraction-to-the-boundary, line-search inputs ----------------
+// D. recover the full step, fraction-to-the-boundary, line-search inputs
+__device__ __forceinline__ void chd_kkt_recover(const ChdDev& D, const ChdKktCtx& c) {
+  ChdIpm& I = *c.I;
+  const ChdSeq* h = c.h;
+  const int b = c.b, tid = c.tid, nt = c.nt, n = c.n, m = c.m, n_act = c.n_act;
+  const size_t ro = c.ro, vo = c.vo;
+  const int *rf = c.rf, *vk = c.vk, *rk = c.rk, *ep = c.ep, *ec = c.ec;
+  const double *Jv = c.Jv, *grad = c.grad, *sol = D.sol + (size_t)c.b * (D.Na_max + D.nb_max), sf = c.sf, mu = c.mu, tau = c.tau;
+  double *vecn = c.vecn, *red = c.red;
   double* dx = D.dx + vo;
   for (int i = tid; i < n; i += nt) {
     const int k = vk[i];
@@ -1088,7 +1052,7 @@ __device__ __forceinline__ void chd_kkt_body(const ChdDev& D) {
     vecn[i] = v;   // step in the unknowns (switch times for the durations): what the Jacobian columns refer to
   }
   __syncthreads();
-  if (sg.opt_dur) {   // the line search moves x, i.e. phase durations: dd_k = dtau_k - dtau_{k-1}
+  if (c.sg.opt_dur) {   // the line search moves x, i.e. phase durations: dd_k = dtau_k - dtau_{k-1}
     for (int ee = 0; ee < h->n_ee; ++ee)
       for (int k = 1 + tid; k < h->n_phases[ee] - 1; k += nt) dx[h->dur_xoff[ee] + k] = vecn[h->dur_xoff[ee] + k] - vecn[h->dur_xoff[ee] + k - 1];
   }
@@ -1136,8 +1100,45 @@ __device__ __forceinline__ void chd_kkt_body(const ChdDev& D) {
     I.step_ready = 1;
     I.kw_req = 1;
   }
+}
+
+// One interior-point iteration of the sequence of this CTA: the phases above in order, each ending on a block barrier.
+template <bool WS>
+__device__ __forceinline__ void chd_kkt_body(const ChdDev& D) {
+  __shared__ int s_fail;
+  ChdIpm& I = D.ipm[blockIdx.x];
+  if (I.phase != CHD_PH_RUN) return;
+  ChdKktCtx c;
+  chd_kkt_ctx_init<WS>(D, I, c);
+  // per-phase cycle counters (scripts/prof_stage.py): compiled in only with -DCHD_PROFILE (extra barriers + clock reads)
+#ifdef CHD_PROFILE
+  long long tk0 = clock64();
+#define CHD_PROF(slot) do { __syncthreads(); if (c.tid == 0) { long long t_ = clock64(); I.prof[slot] += (double)(t_ - tk0); tk0 = t_; } } while (0)
+#else
+#define CHD_PROF(slot) do { } while (0)
+#endif
+  if (chd_kkt_errors(D, c, s_fail)) return;
+  CHD_PROF(0);
+  chd_kkt_assemble(D, c);
+  CHD_PROF(1);
+  // y^+ * Jd^T Jd of the squared-distance rows: in-kernel only on the first iteration of a stage, afterwards
+  // chd_k_curv has already added them on the side stream (many CTAs per sequence: the atomics are the cost)
+  if (!c.pre_refreshed) chd_curv_rows(D, c.b, c.K, c.sg, c.warp, c.nwarp, c.lane, c.win + c.warp * 192);
+  __threadfence_block();
+  __syncthreads();
+  CHD_PROF(2);
+  chd_kkt_factor<WS>(c, s_fail);
+  CHD_PROF(3);
+  chd_kkt_border(D, c, s_fail);
+  CHD_PROF(4);
+  chd_kkt_backsub<WS>(D, c);
+  CHD_PROF(5);
+  if (chd_kkt_no_step(D, c, s_fail)) return;
+  __syncthreads();
+  chd_kkt_recover(D, c);
   CHD_PROF(6);
 }
+#undef CHD_PROF
 
 // Kwork <- Kbase for the sequences whose KKT kernel asked for it; runs on a side stream, overlapped with the line
 // search / evaluation kernels of the next iteration, on the SMs the one-CTA-per-sequence kernels leave idle
@@ -1155,15 +1156,7 @@ __global__ void __launch_bounds__(256) chd_k_kcopy(ChdDev D) {
   }
   const size_t cnt2 = D.kstride / 2, per = (cnt2 + gridDim.x - 1) / gridDim.x;
   const size_t lo = (size_t)blockIdx.x * per, hi = lo + per < cnt2 ? lo + per : cnt2;
-  const double2* src = reinterpret_cast<const double2*>(D.Kbase + (size_t)b * D.kstride);
-  double2* dst = reinterpret_cast<double2*>(D.Kwork + (size_t)b * D.kstride);
-  const size_t nt = blockDim.x;
-  size_t i = lo + threadIdx.x;
-  for (; i + 3 * nt < hi; i += 4 * nt) {
-    const double2 v0 = src[i], v1 = src[i + nt], v2 = src[i + 2 * nt], v3 = src[i + 3 * nt];
-    dst[i] = v0, dst[i + nt] = v1, dst[i + 2 * nt] = v2, dst[i + 3 * nt] = v3;
-  }
-  for (; i < hi; i += nt) dst[i] = src[i];
+  chd_kwork_copy(D, b, lo + threadIdx.x, hi, blockDim.x);
 }
 
 // distance-row curvature terms of the next iteration (needs the iterate the line search just accepted); side stream,

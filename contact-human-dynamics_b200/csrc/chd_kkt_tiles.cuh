@@ -7,15 +7,17 @@
 // Global layout per sequence (doubles):  band | bord | corn
 //   band : block column J (8 columns) holds Q = q+1 tiles (I = J .. J+q), tile = 8x8 row major
 //   bord : block column J holds nbt tiles of border rows (row b -> tile b>>3, r = b&7)
-//   corn : nbp8 x nbp8 dense, row major (nbp8 = 8*nbt); row `nbr` carries the border part of the rhs
+//   corn : nbp8 x nbp8 dense, row major (nbp8 = 8*nbt)
+// The right-hand side is stored as the border row right behind the border unknowns of the stage (chd_k_kkt).
 // The factorisation is an unpivoted block LDL^T (the matrix is quasi-definite by construction, DESIGN.md):
-// per block column: 8x8 diagonal LDL^T (warp shuffles), row-wise triangular solves of the panel, and
-// FP64 tensor-core (mma.sync m8n8k4) rank-8 trailing updates of the shared-memory window.
+// per block column: 8x8 diagonal LDL^T (warp shuffles) that also yields the inverse of its unit factor, the panel as one
+// FP64 tensor-core (mma.sync m8n8k4) product per tile, and rank-8 tensor-core trailing updates of the elimination window
+// (shared memory, or in place in global memory for wide bands).
 #pragma once
 #include "chd_dev.h"
 
 struct ChdKT {
-  int Na, Np, nbc, q, Q, nbt, nbp8, nbr;
+  int Na, Np, nbc, q, Q, nbt, nbp8;
   double *band, *bord, *corn;
   int* ovf;   // set when a coupling falls outside the band (run-time patterns of stage 3), nullptr: not checked
 };
@@ -28,7 +30,6 @@ __device__ __forceinline__ void chd_kt_init(const ChdDev& D, const ChdSeq* h, do
   K.q = D.Q - 1;
   K.nbt = D.nbt;
   K.nbp8 = 8 * D.nbt;
-  K.nbr = D.nb_max;
   K.ovf = nullptr;
   K.band = base;
   K.bord = base + (size_t)D.nbc_max * D.Q * 64;
@@ -51,10 +52,6 @@ __device__ __forceinline__ void chd_kadd(const ChdKT& K, int i, int j, double v)
   } else {
     atomicAdd(K.corn + (size_t)(i - K.Na) * K.nbp8 + (j - K.Na), v);
   }
-}
-__device__ __forceinline__ void chd_radd(const ChdKT& K, int i, double v) {  // right-hand side
-  if (i < K.Na) atomicAdd(K.bord + ((size_t)(i >> 3) * K.nbt + (K.nbr >> 3)) * 64 + (K.nbr & 7) * 8 + (i & 7), v);
-  else atomicAdd(K.corn + (size_t)K.nbr * K.nbp8 + (i - K.Na), v);
 }
 
 // D(8x8) = C - X * Y^T for row-major 8x8 tiles X, Y (fp64 tensor core, two k-steps of m8n8k4).
@@ -166,38 +163,6 @@ __device__ __forceinline__ void chd_copy16(double* dst, const double* src, int s
 __device__ __forceinline__ void chd_copy_wait(int smem) {
   if (smem) asm volatile("cp.async.wait_all;" ::: "memory");
 }
-
-// TMA 1-D bulk copies global -> shared memory with mbarrier completion (cp.async.bulk, SASS UBLKCP / SYNCS): one elected
-// thread streams a whole block row of the elimination window, the other warps keep their issue slots for the tensor-core
-// updates instead of spending them on address arithmetic for 16-byte cp.async chunks.
-__device__ __forceinline__ void chd_mbar_init(unsigned long long* bar, int count) {
-  const unsigned a = (unsigned)__cvta_generic_to_shared(bar);
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(a), "r"(count) : "memory");
-  asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-}
-__device__ __forceinline__ void chd_mbar_expect(unsigned long long* bar, unsigned bytes) {
-  const unsigned a = (unsigned)__cvta_generic_to_shared(bar);
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(a), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void chd_bulk_g2s(double* dst, const double* src, unsigned bytes, unsigned long long* bar) {
-  const unsigned d = (unsigned)__cvta_generic_to_shared(dst), a = (unsigned)__cvta_generic_to_shared(bar);
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(d), "l"(src), "r"(bytes), "r"(a)
-               : "memory");
-}
-__device__ __forceinline__ void chd_mbar_wait(unsigned long long* bar, unsigned parity) {
-  const unsigned a = (unsigned)__cvta_generic_to_shared(bar);
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "WAIT_%=:\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
-      "@p bra DONE_%=;\n\t"
-      "bra WAIT_%=;\n\t"
-      "DONE_%=:\n\t"
-      "}" ::"r"(a), "r"(parity)
-      : "memory");
-}
-__device__ __forceinline__ void chd_fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 // window slot of band tile (I, J), I >= J, both inside a sliding window of Q block rows/columns
 __device__ __forceinline__ int chd_win_slot(int I, int J, int Q) {
