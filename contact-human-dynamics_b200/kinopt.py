@@ -124,6 +124,20 @@ class _Model:
         self.is_root = torch.zeros(NJ, **f64)
         self.is_root[ROOT_IDX] = 1.0
 
+    # ---- what differs between one clip and several clips on one frame axis (_BatchModel) ----
+    def _bone(self, gRq, j):
+        """Offset of joint j rotated by its parent's global rotation."""
+        return gRq @ self.off[j]
+
+    def _rows(self, span, r, G):
+        """A residual group whose row of base frame f couples frames f .. f+span -> (base frames, r, G); 0 = all from 0."""
+        return 0, r, G
+
+    def _floor(self, cf, ab, dab, jac):
+        r = cf * ((ab - self.pt) @ self.n)
+        G = {0: cf[..., None] * self.t.einsum("c,fjcv->fjv", self.n, dab)} if jac else None
+        return r, G
+
     # ---- forward kinematics: y (F, 28, 3) in body-25 order (root entry = root translation, others root-relative) ----
     def points(self, x, jac=False):
         t = self.t
@@ -139,7 +153,7 @@ class _Model:
                 gR[j], gP[j] = Rl[:, j], t.zeros(F, 3, **self.f64)
             else:
                 gR[j] = gR[q] @ Rl[:, j]
-                gP[j] = gP[q] + gR[q] @ self.off[j]
+                gP[j] = gP[q] + self._bone(gR[q], j)
         gR, gP = t.stack(gR, 1), t.stack(gP, 1)                                       # skeleton order, root at the origin
         y = gP[:, self.back].clone()
         y[:, ROOT_IDX] = x[:, :3]
@@ -162,7 +176,7 @@ class _Model:
 
     # ---- residual groups; each returns (r, [(frame offset d, dr/dy_{f+d} as (F', rows, 84))]) ----
     def residuals(self, x, w: StageWeights, jac=False):
-        """List of (base frames F', r (F', rows), blocks {d: G (F', rows, 87)} = dr/dx_{f+d})."""
+        """List of (base frames, r (F', rows), blocks {d: G (F', rows, 87)} = dr/dx_{f+d}); base frames 0: 0 .. F'-1."""
         t = self.t
         F = self.F
         y, dP = self.points(x, jac)
@@ -196,7 +210,7 @@ class _Model:
                 g0 = (ws[None, :, :, None] * dP[:-1]).reshape(F - 1, -1, NV)
                 g1 = (-ws[None, :, :, None] * dP[1:]).reshape(F - 1, -1, NV)
                 G = {0: g0, 1: g1}
-            out.append((0, r, G))
+            out.append(self._rows(1, r, G))
         # 3. acceleration smoothness (frames f, f+1, f+2)
         if F > 2:
             r = (w.smooth_acc * (y[2:] - 2.0 * y[1:-1] + y[:-2])).reshape(F - 2, -1)
@@ -204,7 +218,7 @@ class _Model:
             if jac:
                 G = {0: (w.smooth_acc * dP[:-2]).reshape(F - 2, -1, NV), 1: (-2.0 * w.smooth_acc * dP[1:-1]).reshape(F - 2, -1, NV),
                      2: (w.smooth_acc * dP[2:]).reshape(F - 2, -1, NV)}
-            out.append((0, r, G))
+            out.append(self._rows(2, r, G))
         # 4. data
         tgt = self.poses3D * nr[None, :, None] + self.root_trans[:, None, :] * self.is_root[None, :, None]
         wd = w.data * self.dw
@@ -218,11 +232,9 @@ class _Model:
             G = None
             if jac:
                 G = {0: (c[..., None, None] * dab[:-1]).reshape(F - 1, -1, NV), 1: (-c[..., None, None] * dab[1:]).reshape(F - 1, -1, NV)}
-            out.append((0, r, G))
+            out.append(self._rows(1, r, G))
         # 6. floor
-        cf = w.floor * self.con
-        r = cf * ((ab - self.pt) @ self.n)
-        G = {0: cf[..., None] * t.einsum("c,fjcv->fjv", self.n, dab)} if jac else None
+        r, G = self._floor(w.floor * self.con, ab, dab, jac)
         out.append((0, r, G))
         # 7. smoothness of the unknowns themselves (root translation and Euler angles)
         if F > 1:
@@ -232,7 +244,7 @@ class _Model:
             if jac:
                 I = (we * t.eye(NV, **self.f64)).expand(F - 1, NV, NV)
                 G = {0: I, 1: -I}
-            out.append((0, r, G))
+            out.append(self._rows(1, r, G))
         return out
 
     def residual_vector(self, x, w):
@@ -372,6 +384,242 @@ def levenberg_marquardt(model: _Model, x0, w: StageWeights, max_nfev: int = 50, 
     return x, cost, nfev
 
 
+# ---------------------------------------------------------------------------------------------------------------------
+# Several clips at once: one concatenated frame axis, one block-banded solve launch per Levenberg-Marquardt round
+# ---------------------------------------------------------------------------------------------------------------------
+class _BatchModel(_Model):
+    """`_Model` over the concatenated frames of K clips of the same skeleton.  Offsets and floor are per frame (each clip
+    keeps its own), and the rows that would couple the last frames of one clip with the next clip (velocity,
+    acceleration, contact velocity, Euler smoothness) are dropped, so H has no block coupling two clips.  The per-frame
+    arithmetic is the single-clip one; cost and normal equations return per-clip costs (numpy, K)."""
+
+    def __init__(self, probs, device=None):
+        if not probs:
+            raise ValueError("no clips")
+        parents = np.asarray(probs[0].parents)
+        if any(not np.array_equal(np.asarray(p.parents), parents) for p in probs):
+            raise ValueError("all clips of a batch must use the same skeleton hierarchy")
+        self.lens = np.array([p.poses3D.shape[0] for p in probs], dtype=np.int64)
+        if (self.lens < 1).any():
+            raise ValueError("every clip needs at least one frame")
+        self.K = len(probs)
+        self.seg = np.concatenate([[0], np.cumsum(self.lens)]).astype(np.int64)
+        cat = lambda a: np.concatenate([np.asarray(getattr(p, a), np.float64) for p in probs], 0)
+        rep = lambda a: np.repeat(np.stack([np.asarray(getattr(p, a), np.float64) for p in probs]), self.lens, axis=0)
+        super().__init__(Problem(parents, rep("offsets"), cat("poses3D"), cat("root_trans"), cat("joints2d"), cat("proj_w"),
+                                 cat("data_w"), cat("contacts"), rep("floor_normal"), rep("floor_point")), device)
+        t, F = self.t, self.F
+        self.clip = t.as_tensor(np.repeat(np.arange(self.K), self.lens), device=self.dev)      # clip of every frame
+        end = np.repeat(self.seg[1:], self.lens)
+        self.keep = {k: t.as_tensor(np.nonzero(np.arange(max(F - k, 0)) + k < end[:max(F - k, 0)])[0], device=self.dev)
+                     for k in (1, 2)}
+        self.all = t.arange(F, device=self.dev)
+        # On the CPU the products with a clip's offsets and floor are taken clip by clip, as the matrix-vector products of
+        # the single-clip model: a per-frame batched product rounds differently in the last bit, and Levenberg-Marquardt
+        # amplifies that along weakly determined directions.  On a GPU one batched product serves all clips.
+        self.by_clip = self.dev.type == "cpu"
+        as_t = lambda a: t.as_tensor(np.stack([np.asarray(getattr(p, a), np.float64) for p in probs]), **self.f64)
+        self.off_k, self.n_k, self.pt_k = as_t("offsets"), as_t("floor_normal"), as_t("floor_point")
+        self.spans = [(int(a), int(b)) for a, b in zip(self.seg[:-1], self.seg[1:])]
+
+    def _bone(self, gRq, j):
+        if self.by_clip:
+            return self.t.cat([gRq[a:b] @ self.off_k[k, j] for k, (a, b) in enumerate(self.spans)], 0)
+        return (gRq @ self.off[:, j, :, None])[..., 0]
+
+    def _rows(self, span, r, G):
+        idx = self.keep[span]
+        return idx, r[idx], ({d: g[idx] for d, g in G.items()} if G is not None else None)
+
+    def _floor(self, cf, ab, dab, jac):
+        t = self.t
+        if self.by_clip:
+            r = t.cat([cf[a:b] * ((ab[a:b] - self.pt_k[k]) @ self.n_k[k]) for k, (a, b) in enumerate(self.spans)], 0)
+            G = {0: t.cat([cf[a:b, :, None] * t.einsum("c,fjcv->fjv", self.n_k[k], dab[a:b]) for k, (a, b) in enumerate(self.spans)], 0)} if jac else None
+            return r, G
+        r = cf * t.einsum("fjc,fc->fj", ab - self.pt[:, None, :], self.n)
+        G = {0: cf[..., None] * t.einsum("fc,fjcv->fjv", self.n, dab)} if jac else None
+        return r, G
+
+    def _base(self, base, Fp):
+        return self.all[:Fp] if isinstance(base, int) else base
+
+    def per_clip(self, v):
+        """Segment sums of a per-frame numpy vector."""
+        return np.add.reduceat(np.asarray(v, dtype=np.float64), self.seg[:-1])
+
+    def _costs(self, groups, each):
+        """0.5 * sum of squares per clip of the residual groups [(base, r)]; `each`: halve every group's sum (as
+        `_Model.normal_equations`) instead of the total (as `_Model.cost`).  By clip: one reduction per clip and group, in
+        the single-clip model's order.  Otherwise per frame on the device (a row counts for its first frame), then
+        per clip on the host."""
+        t = self.t
+        if self.by_clip:
+            c = np.zeros(self.K)
+            for base, r in groups:
+                rr = r.reshape(r.shape[0], -1)
+                cuts = self.seg if isinstance(base, int) else np.searchsorted(base.cpu().numpy(), self.seg)
+                for k in range(self.K):
+                    v = rr[cuts[k]:cuts[k + 1]]
+                    if v.shape[0]:
+                        c[k] += 0.5 * float((v * v).sum()) if each else float((v * v).sum())
+            return c if each else 0.5 * c
+        return 0.5 * self.per_clip(self.frame_costs(groups).cpu().numpy())
+
+    def frame_costs(self, groups):
+        cf = self.t.zeros(self.F, **self.f64)
+        for base, r in groups:
+            rr = r.reshape(r.shape[0], -1)
+            cf.index_add_(0, self._base(base, rr.shape[0]), (rr * rr).sum(1))
+        return cf
+
+    def cost(self, x, w):
+        return self._costs([(b, r) for b, r, _ in self.residuals(x, w, jac=False)], each=False)
+
+    def trial(self, xn, w, step, lam, H, g, status):
+        """(cost at xn, predicted decrease 0.5 step^T (lam diag(H) step - g), solve status) per clip, numpy; one device to
+        host copy."""
+        t = self.t
+        dg = t.diagonal(H[0], dim1=1, dim2=2).clamp_min(1e-12)
+        if self.by_clip:
+            pred = np.array([0.5 * float((step[a:b] * (float(lam[k]) * dg[a:b] * step[a:b] - g[a:b])).sum()) for k, (a, b) in enumerate(self.spans)])
+            return self.cost(xn, w), pred, status.cpu().numpy()
+        lamf = t.as_tensor(np.repeat(lam, self.lens), **self.f64)
+        pf = (step * (lamf[:, None] * dg * step - g)).sum(1)
+        cf = self.frame_costs([(b, r) for b, r, _ in self.residuals(xn, w, jac=False)])
+        host = t.cat([cf, pf, status.to(t.float64)]).cpu().numpy()
+        F = self.F
+        return 0.5 * self.per_clip(host[:F]), 0.5 * self.per_clip(host[F:2 * F]), host[2 * F:]
+
+    def dense_jacobian(self, x, w):
+        """(terms, 87 F) -- tests only (small F)."""
+        t = self.t
+        rows = []
+        for base, r, G in self.residuals(x, w, jac=True):
+            Fp, nr_ = r.shape[0], r.reshape(r.shape[0], -1).shape[1]
+            bf = self._base(base, Fp).tolist()
+            blk = t.zeros(Fp, nr_, self.F * NV, **self.f64)
+            for d, g in G.items():
+                for i, f in enumerate(bf):
+                    blk[i, :, (f + d) * NV:(f + d + 1) * NV] = g[i]
+            rows.append(blk.reshape(-1, self.F * NV))
+        return t.cat(rows, 0)
+
+    def normal_equations(self, x, w):
+        t = self.t
+        F = self.F
+        H = [t.zeros(F, NV, NV, **self.f64), t.zeros(max(F - 1, 0), NV, NV, **self.f64), t.zeros(max(F - 2, 0), NV, NV, **self.f64)]
+        g = t.zeros(F, NV, **self.f64)
+        groups = []
+        for base, r, G in self.residuals(x, w, jac=True):
+            Fp = r.shape[0]
+            rr = r.reshape(Fp, -1)
+            bf = self._base(base, Fp)
+            groups.append((base, r))
+            for d, gd in G.items():
+                g.index_add_(0, bf + d, t.einsum("frv,fr->fv", gd, rr))
+                for e_, ge in G.items():
+                    if e_ < d:
+                        continue
+                    H[e_ - d].index_add_(0, bf + d, gd.transpose(1, 2) @ ge if e_ == d else ge.transpose(1, 2) @ gd)
+        return self._costs(groups, each=True), H, g
+
+
+class _KinSolver:
+    """The damped block-banded solves of all live clips of a `_BatchModel` in one step: one `chd_kin_solve` launch on a
+    CUDA device (libchd is required there), `_banded_cholesky_solve` per clip segment on the CPU."""
+
+    def __init__(self, model: _BatchModel):
+        t = model.t
+        self.m = model
+        self.cuda = model.dev.type == "cuda"
+        self.s = t.zeros(model.F, NV, **model.f64)
+        self.status = t.zeros(model.K, dtype=t.int32, device=model.dev)
+        if self.cuda:
+            from .phys import load_lib
+            self.L = load_lib()
+            nb = self.L.chd_kin_work_bytes(int(model.F))
+            self.work = t.empty(max(nb // 8, 1), **model.f64)
+            self.seg = t.as_tensor(model.seg, dtype=t.int32, device=model.dev)
+
+    def __call__(self, H, g, lam, live):
+        """Solves (H + lam_k diag H) s = g for the clips `live`.  Returns (s, status) on the model's device; status is 0
+        for a solved clip, nonzero for a failed factorisation or a clip not in `live`, and s is only defined where 0."""
+        t, m = self.m.t, self.m
+        self.status.fill_(-2)
+        if not self.cuda:
+            st = np.full(m.K, -2, dtype=np.int32)
+            for k in live:
+                a, b = int(m.seg[k]), int(m.seg[k + 1])
+                try:
+                    self.s[a:b] = _banded_cholesky_solve(t, (H[0][a:b], H[1][a:b - 1], H[2][a:b - 2]), g[a:b], float(lam[k]))
+                    st[k] = 0
+                except Exception:         # not positive definite at this damping
+                    st[k] = 1
+            self.status.copy_(t.as_tensor(st))
+            return self.s, self.status
+        ptr = lambda a: a.data_ptr() if a.numel() else None
+        lam_d = t.as_tensor(np.asarray(lam, np.float64), **m.f64)
+        sel = t.as_tensor(np.asarray(live, np.int32), device=m.dev)
+        D, B1, B2, gc = (a.contiguous() for a in (H[0], H[1], H[2], g))
+        with t.cuda.device(m.dev):
+            rc = self.L.chd_kin_solve(ptr(D), ptr(B1), ptr(B2), ptr(gc), self.seg.data_ptr(), lam_d.data_ptr(), sel.data_ptr(),
+                                      len(live), m.K, m.F, self.work.data_ptr(), self.s.data_ptr(), self.status.data_ptr(),
+                                      t.cuda.current_stream(m.dev).cuda_stream)
+        if rc != 0:
+            raise RuntimeError("chd_kin_solve failed with code %d" % rc)
+        return self.s, self.status
+
+
+def levenberg_marquardt_batch(model: _BatchModel, x0s, w: StageWeights, max_nfev: int = 50, rtol: float = 1e-10, verbose: bool = False):
+    """`levenberg_marquardt` for every clip of `model` at once, from x0s (one (F_k, 87) array per clip).  Each clip keeps
+    its own state (damping, cost, evaluation count) and follows exactly the single-clip state machine; a round solves all
+    live clips in one step and synchronises the host once for the accept decisions.  Returns (xs, costs, nfevs), lists."""
+    t = model.t
+    K, seg = model.K, model.seg
+    x = t.as_tensor(np.concatenate([np.asarray(a, np.float64).reshape(-1, NV) for a in x0s], 0), **model.f64).clone()
+    if x.shape[0] != model.F:
+        raise ValueError("x0s do not match the model's frames")
+    solve = _KinSolver(model)
+    cost, H, g = model.normal_equations(x, w)
+    nfev = np.ones(K, dtype=np.int64)
+    lam = np.full(K, 1e-3)
+    done = nfev >= max_nfev
+    rnd = 0
+    while not done.all():
+        live = np.nonzero(~done)[0]
+        s, status = solve(H, g, lam, live)
+        okf = (status == 0)[model.clip]                                           # frames of the clips that got a step
+        step = -t.where(okf[:, None], s, t.zeros_like(s))
+        xn = x + step
+        cn, pred, st = model.trial(xn, w, step, lam, H, g, status)
+        acc = np.zeros(K, dtype=bool)
+        for k in live:
+            if st[k] != 0:                # not positive definite at this damping
+                lam[k] *= 10.0
+                done[k] = lam[k] > 1e12
+                continue
+            nfev[k] += 1
+            rho = (cost[k] - cn[k]) / pred[k] if pred[k] > 0 else -1.0
+            if cn[k] < cost[k]:
+                acc[k] = True
+                done[k] = (cost[k] - cn[k]) <= rtol * cost[k]
+                lam[k] = max(lam[k] * max(1.0 / 3.0, 1.0 - (2.0 * rho - 1.0) ** 3), 1e-9) if rho > 0 else lam[k]
+            else:
+                lam[k] *= 4.0
+                done[k] = lam[k] > 1e12
+            done[k] = done[k] or nfev[k] >= max_nfev
+        if verbose:
+            rnd += 1
+            print("  round %3d  live %d  accepted %d  cost %.6e" % (rnd, len(live), int(acc.sum()), float(np.sum(cost))))
+        if acc.any():
+            x = t.where(t.as_tensor(acc, device=model.dev)[model.clip][:, None], xn, x)
+            cnew, H, g = model.normal_equations(x, w)
+            cost = np.where(acc, cnew, cost)
+    xs = [x[seg[k]:seg[k + 1]] for k in range(K)]
+    return xs, [float(c) for c in cost], [int(n) for n in nfev]
+
+
 def huber_fit(X, y, epsilon: float, alpha: float = 1e-4, max_iter: int = 100, tol: float = 1e-5):
     """Linear fit with the Huber loss and a concomitant scale (the estimator `sklearn.linear_model.HuberRegressor`
     implements; optimize_trajectory.py:719-750 uses it with epsilon 1.5 / 2.2):
@@ -487,6 +735,87 @@ def _global_positions(parents, off, x):
     return forward_kinematics(np.asarray(parents), rot_zyx(x[:, 3:].reshape(F, NJ, 3)), T)[0]
 
 
+def optimize_trajectory_batch(poses2D, joint_conf_2d, poses3D, root_pos, joint_angles, parents, offsets, ppx, ppy, cam_focal, vel_constraints,
+                              plane_normal=None, plane_point=None, device=None, ik_iterations: int = 200, max_nfev: int = 50, verbose: bool = False):
+    """`optimize_trajectory` for K clips at once: every per-clip argument is a list with one entry per clip (plane_normal /
+    plane_point: None, or a list whose None entries mean "fit the floor" for that clip).  The IK initialisation is one
+    call over all frames, each Levenberg-Marquardt stage runs all clips together (`levenberg_marquardt_batch`); the
+    skeleton fit, the floor fit and the contact pruning stay per clip.  Returns the list of `optimize_trajectory`'s tuples."""
+    from .prepare import euler_zyx_from_matrix
+    K = len(poses3D)
+    pn_in = plane_normal if plane_normal is not None else [None] * K
+    pp_in = plane_point if plane_point is not None else [None] * K
+    clips = []
+    for k in range(K):
+        p2, p3, rp = np.asarray(poses2D[k], np.float64), np.asarray(poses3D[k], np.float64), np.asarray(root_pos[k], np.float64)
+        F, J = p3.shape[:2]
+        if p2.shape[1] != J:
+            raise ValueError("clip %d: 2D and 3D data must have the same number of joints" % k)
+        targets = p3[:, FORWARD] + rp[:, None, :]
+        off = update_skeleton(parents[k], offsets[k], targets)
+        j2n, pw, dw = make_weights(p2, np.asarray(joint_conf_2d[k], np.float64), (ppx[k], ppy[k]), cam_focal[k])
+        given = pn_in[k] is not None and pp_in[k] is not None
+        clips.append(dict(F=F, p3=p3, rp=rp, targets=targets, off=off, j2n=j2n, pw=pw, dw=dw, given=given,
+                          vel=np.asarray(vel_constraints[k], dtype=np.float64).copy(), parents=np.asarray(parents[k]),
+                          pn=np.asarray(pn_in[k], np.float64) if given else None, pp=np.asarray(pp_in[k], np.float64) if given else None))
+    J = clips[0]["p3"].shape[1]
+    # IK initialisation of every frame of every clip in one call (smoothness 0: the frames are independent)
+    R0, P0 = [], []
+    for k, c in enumerate(clips):
+        aa = -np.asarray(joint_angles[k], np.float64)
+        ang = np.linalg.norm(aa, axis=2)
+        axis = aa / (ang + 1e-10)[..., None]
+        Km = np.zeros(aa.shape[:2] + (3, 3))
+        Km[..., 0, 1], Km[..., 0, 2], Km[..., 1, 0], Km[..., 1, 2], Km[..., 2, 0], Km[..., 2, 1] = -axis[..., 2], axis[..., 1], axis[..., 2], -axis[..., 0], -axis[..., 1], axis[..., 0]
+        R0.append(np.eye(3) + np.sin(ang)[..., None, None] * Km + (1.0 - np.cos(ang))[..., None, None] * (Km @ Km))
+        P = np.tile(c["off"][None], (c["F"], 1, 1))
+        P[:, 0] = c["rp"]
+        P0.append(P)
+    names = ["joint_%d" % i for i in range(J)]
+    anim = SkelAnim(names, clips[0]["parents"], clips[0]["off"], np.concatenate(R0), np.concatenate(P0))
+    tm = {j: np.concatenate([c["targets"][:, j] for c in clips]) for j in range(J) if j not in SPINE_IDX}
+    anim = ik_solve(anim, tm, iterations=ik_iterations, smoothness=0.0, damping=7.0, translate=False, device=device)
+    xall = np.concatenate([anim.positions[:, 0], euler_zyx_from_matrix(anim.rotations).reshape(anim.rotations.shape[0], -1)], axis=1)
+    seg = np.concatenate([[0], np.cumsum([c["F"] for c in clips])])
+    xs = [xall[seg[k]:seg[k + 1]] for k in range(K)]
+    zero = np.zeros(3)
+    probs = [Problem(c["parents"], c["off"], c["p3"], c["rp"], c["j2n"], c["pw"], c["dw"], c["vel"], c["pn"] if c["given"] else zero,
+                     c["pp"] if c["given"] else zero) for c in clips]
+    # stage 1: no floor term
+    out1, c1, n1 = levenberg_marquardt_batch(_BatchModel(probs, device), xs, StageWeights(floor=0.0), max_nfev, verbose=verbose)
+    xs = [v.cpu().numpy() for v in out1]
+    # floor fit on the contact feet, contact pruning (per clip)
+    feet_lab = np.array([FORWARD[k] for k in FEET_IDX])
+    for k, c in enumerate(clips):
+        vel = c["vel"]
+        gp = _global_positions(c["parents"], c["off"], xs[k])
+        sel = vel[:, feet_lab] == 1
+        feet_pos = gp[:, FEET_IDX][sel]
+        if not c["given"]:
+            c["pn"], c["pp"], _ = fit_floor(feet_pos, 1.5)
+            _, _, _, outl = huber_fit(feet_pos[:, [0, 2]], feet_pos[:, 1], 2.2)
+            fv = vel[:, feet_lab]
+            fv[sel] = np.where(outl, 0.0, 1.0)
+            vel[:, feet_lab] = fv
+        probs[k].contacts, probs[k].floor_normal, probs[k].floor_point = vel, np.asarray(c["pn"], np.float64), np.asarray(c["pp"], np.float64)
+    # stage 2: feet on the floor
+    out2, c2, n2 = levenberg_marquardt_batch(_BatchModel(probs, device), xs, StageWeights(floor=10.0), max_nfev, verbose=verbose)
+    res = []
+    for k, c in enumerate(clips):
+        x = out2[k].cpu().numpy()
+        F, off = c["F"], c["off"]
+        info = dict(stage1=dict(cost=c1[k], nfev=n1[k]), stage2=dict(cost=c2[k], nfev=n2[k]), x=x)
+        gp = _global_positions(c["parents"], off, x)
+        new3d = gp[:, BACKWARD]
+        fo = cam_focal[k]
+        proj = np.stack([fo[0] * new3d[..., 0] / new3d[..., 2] + ppx[k], fo[1] * new3d[..., 1] / new3d[..., 2] + ppy[k]], -1)
+        Pl = np.tile(off[None], (F, 1, 1))
+        Pl[:, 0] = x[:, :3]
+        a = SkelAnim(names, c["parents"], off, rot_zyx(x[:, 3:].reshape(F, J, 3)), Pl)
+        res.append((a, new3d, proj, np.asarray(c["pn"]), np.asarray(c["pp"]), c["vel"], info))
+    return res
+
+
 # ---------------------------------------------------------------------------------------------------------------------
 # File-level driver (src/optimize/kinematic_optimizer.py:30-224 optimize_2d_3d) and the Monocular-Total-Capture reader
 # ---------------------------------------------------------------------------------------------------------------------
@@ -586,3 +915,63 @@ def optimize_2d_3d(input_path: str, skel_path: str, output_path: str, min_idx: i
     save_bvh(os.path.join(output_path, "final_test.bvh"), anim, b.names, frametime)
     print("Finished kinematic optimization!")
     return res
+
+
+def optimize_2d_3d_batch(jobs, device=None, frametime: float = 1.0 / 24.0):
+    """`optimize_2d_3d` for several videos with one `optimize_trajectory_batch` call.  `jobs`: list of (input_path,
+    skel_path, output_path, min_idx, max_idx, use_gt_floor); every video gets the three files `optimize_2d_3d` writes.
+    Returns one result per job (None for a video whose inputs are missing, as `optimize_2d_3d`)."""
+    import os
+    from . import contact
+    from .prepare import load_bvh
+    from .results import save_bvh
+    loaded = []
+    for input_path, skel_path, output_path, min_idx, max_idx, use_gt_floor in jobs:
+        os.makedirs(output_path, exist_ok=True)
+        d = os.path.dirname(input_path)
+        op_dir, tc_path, fc_path = os.path.join(d, "openpose_result"), os.path.join(d, "tracked_results.json"), os.path.join(d, "foot_contacts.npy")
+        missing = [m for ok, m in ((os.path.isdir(op_dir), "Could not find openpose results in " + op_dir + "!"),
+                                   (os.path.isfile(tc_path), "Could not find total capture results!"),
+                                   (os.path.isfile(fc_path), "Could not find foot contact labels!")) if not ok]
+        if missing:
+            print(missing[0])
+            loaded.append(None)
+            continue
+        kp = contact.load_keypoint_dir(op_dir)
+        poses3D, root_pos, ang = combined_inputs(load_totalcap_results(tc_path))
+        sl = slice(min_idx, max_idx)
+        n = len(range(*sl.indices(kp.shape[0])))
+        normal = point = None
+        if use_gt_floor:
+            with open(os.path.join(d, "floor_gt.txt")) as f:
+                normal = np.array([float(v) for v in f.readline().split()])
+                point = np.array([float(v) for v in f.readline().split()]) * 100.0
+        loaded.append(dict(out=output_path, bvh=load_bvh(skel_path), normal=normal, point=point,
+                           poses2D=np.concatenate([kp[sl, :, :2], np.zeros((n, 3, 2))], axis=1),
+                           conf=np.concatenate([kp[sl, :, 2], np.zeros((n, 3))], axis=1), poses3D=poses3D[sl], root_pos=root_pos[sl],
+                           ang=ang[sl], vel=contacts_to_constraints(np.load(fc_path)[sl])))
+    vids = [v for v in loaded if v is not None]
+    results = []
+    if vids:
+        col = lambda key: [v[key] for v in vids]
+        K = len(vids)
+        results = optimize_trajectory_batch(col("poses2D"), col("conf"), col("poses3D"), col("root_pos"), col("ang"), [v["bvh"].parents for v in vids],
+                                            [v["bvh"].offsets for v in vids], [MTC_SIZE[0] / 2] * K, [MTC_SIZE[1] / 2] * K, [np.array(MTC_FOCAL)] * K,
+                                            col("vel"), plane_normal=col("normal"), plane_point=col("point"), device=device)
+    it = iter(results)
+    out = []
+    for v in loaded:
+        if v is None:
+            out.append(None)
+            continue
+        res = next(it)
+        anim, new3d, proj, pn, pp, newvel, info = res
+        anim.names = list(v["bvh"].names)
+        np.save(os.path.join(v["out"], "foot_contacts"), constraints_to_contacts(newvel))
+        with open(os.path.join(v["out"], "floor_out.txt"), "w") as f:
+            f.write("%s %s %s\n%s %s %s" % tuple(str(float(q)) for q in list(pn) + list(pp)))
+        save_bvh(os.path.join(v["out"], "final_test.bvh"), anim, v["bvh"].names, frametime)
+        out.append(res)
+    if vids:
+        print("Finished kinematic optimization!")
+    return out

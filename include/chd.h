@@ -186,6 +186,26 @@ int64_t chd_contact_launch_count(const chd_contact_net* net);
  * Returns 0, -1 bad argument, -2 unreadable file, -3 malformed file / keypoint count != 3 * num_joints. */
 int chd_openpose_load(const char* const* paths, int32_t n_files, int32_t num_joints, double* out, int32_t n_threads);
 
+/* ---------------------------------------------------------------------------------------------------------
+ * Kinematic initialisation: the linear solves inside least_squares(tr_solver='lsmr') of optimize_trajectory.py:660-670
+ * and :779-789, for K clips in one launch.  Clip k owns frames seg[k] .. seg[k+1]-1 of the concatenated frame axis;
+ * every system is the damped Gauss-Newton system of the clip,
+ *     (H + lam[k] * diag(max(diag H, 1e-12))) s = g,
+ * with H symmetric block-pentadiagonal in 87 x 87 blocks: D [device] (F_total x 87 x 87) diagonal blocks,
+ * B1 [device] ((F_total-1) x 87 x 87) with B1[f] = block (f+1, f), B2 [device] ((F_total-2) x 87 x 87) with
+ * B2[f] = block (f+2, f), all row major; blocks that would couple two clips are not read.  g, s [device] F_total x 87.
+ * seg [device] K+1 frame offsets, lam [device] K.  sel [device, may be NULL]: the n_sel clips to solve (NULL: all K);
+ * the others' s and status are not touched.  work [device]: chd_kin_work_bytes(F_total) bytes.
+ * status [device] K: 0 solved, f + 1 when block f of the clip (clip-local frame) has a pivot that is not positive and
+ * finite (s of that clip unspecified), -1 when the clip's frame range is not inside [0, F_total).  Each clip's s is
+ * bitwise the same whatever else is in the launch.  Asynchronous on `stream` (cudaStream_t as void*).
+ * Returns 0, -1 bad argument, <= -100 CUDA error. */
+int chd_kin_solve(const double* D, const double* B1, const double* B2, const double* g, const int32_t* seg,
+                  const double* lam, const int32_t* sel, int32_t n_sel, int32_t K, int32_t F_total, double* work,
+                  double* s, int32_t* status, void* stream);
+/* Bytes of `work` chd_kin_solve needs for F_total frames (three padded 88 x 88 fp64 blocks per frame); -1 if F_total < 0. */
+int64_t chd_kin_work_bytes(int32_t F_total);
+
 const char* chd_version(void);
 
 /* Measurement helper (no reference counterpart): sustained fp64 throughput of the current device in GFLOP/s, for the
