@@ -86,8 +86,22 @@ def load_weights(path: str) -> Dict[str, np.ndarray]:
     return {k: v.numpy() for k, v in sd.items()}
 
 
+PRECISIONS = {"fp32": 0, "tf32x3": 1}       # CHD_CONTACT_FP32, CHD_CONTACT_TF32X3 (include/chd.h)
+
+
+def precision_code(precision: str) -> int:
+    if precision not in PRECISIONS:
+        raise ValueError("unknown contact precision %r: expected one of %s" % (precision, ", ".join(sorted(PRECISIONS))))
+    return PRECISIONS[precision]
+
+
 class ContactNet:
-    def __init__(self, state_dict: Dict[str, np.ndarray], device: int = -1, bn_eps: float = 1e-5):
+    """The classifier on one GPU.  `precision="fp32"` (default) is the FFMA path whose labels match the reference's
+    fp32 forward; `"tf32x3"` runs the three large layers on the tensor core with split TF32 operands
+    (`chd_contact_set_precision`), logits within a few 1e-5 of the fp32 mode."""
+
+    def __init__(self, state_dict: Dict[str, np.ndarray], device: int = -1, bn_eps: float = 1e-5, precision: str = "fp32"):
+        code = precision_code(precision)
         self.L = load_lib()
         L = self.L
         L.chd_contact_create.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_float, C.c_int32, C.POINTER(C.c_void_p)]
@@ -98,6 +112,7 @@ class ContactNet:
         L.chd_contact_detect.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]
         L.chd_contact_launch_count.argtypes = [C.c_void_p]
         L.chd_contact_launch_count.restype = C.c_int64
+        L.chd_contact_set_precision.argtypes = [C.c_void_p, C.c_int32]
         w, b, bn = pack_state_dict(state_dict)
         assert w.size == sum(i * o for i, o in zip(DIMS[:-1], DIMS[1:])) and b.size == sum(DIMS[1:])
         h = C.c_void_p()
@@ -105,6 +120,16 @@ class ContactNet:
         if rc != 0:
             raise RuntimeError("chd_contact_create failed with code %d (no CUDA device? no CPU fallback exists)" % rc)
         self.h = h
+        self.precision = "fp32"
+        if code != PRECISIONS["fp32"]:
+            self.set_precision(precision)
+
+    def set_precision(self, precision: str):
+        """Numerical mode of every later forward / detect call: "fp32" or "tf32x3"."""
+        rc = self.L.chd_contact_set_precision(self.h, precision_code(precision))
+        if rc != 0:
+            raise RuntimeError("chd_contact_set_precision failed with code %d" % rc)
+        self.precision = precision
 
     def close(self):
         if getattr(self, "h", None):
@@ -161,12 +186,14 @@ class ContactNet:
         return int(self.L.chd_contact_launch_count(self.h))
 
 
-def detect_contacts(data_root: str, out_root: str, state_dict, dimensions=(1920, 1080)) -> List[str]:
+def detect_contacts(data_root: str, out_root: str, state_dict, dimensions=(1920, 1080), precision: str = "fp32") -> List[str]:
     """`test.py --data D --out O --full-video --save-contacts --real-data`: for every video directory of D with an
-    `openpose_result/` writes O/contact_results/<video>/foot_contacts.npy (int64, F x 4), test.py:143-152."""
+    `openpose_result/` writes O/contact_results/<video>/foot_contacts.npy (int64, F x 4), test.py:143-152.
+    `precision`: numerical mode of the network (see `ContactNet`)."""
+    precision_code(precision)
     vids = sorted(d for d in os.listdir(data_root) if os.path.isdir(os.path.join(data_root, d)) and d[0] != ".")
     raw = load_keypoint_dirs([os.path.join(data_root, v, "openpose_result") for v in vids])
-    net = ContactNet(state_dict)
+    net = ContactNet(state_dict, precision=precision)
     labels, _ = net.detect(raw, dimensions)
     written = []
     for i, v in enumerate(vids):

@@ -13,7 +13,8 @@
 // small enough for the 50 MB L2 would leave the 128-wide layer with fewer tiles than SMs); every output is one fp32
 // accumulator summed over k in ascending order (fmaf), the same arithmetic as a plain loop.  fp32 FFMA, no tf32/bf16:
 // the integer labels must match the reference's fp32 forward away from the logit-0 boundary (SURVEY 8(a)-D note;
-// wgmma has no fp32-input kind).
+// wgmma has no fp32-input kind).  The opt-in 3xTF32 tensor-core mode of the three large layers (CHD_CONTACT_TF32X3)
+// is in chd_contact_tc.cu; this file's kernels are the default FP32 mode.
 #include <cuda_runtime.h>
 #include <cstdlib>
 
@@ -23,6 +24,7 @@
 #include <vector>
 
 #include "../../include/chd.h"
+#include "chd_contact_tc.h"
 
 #define CT_WIN 9
 #define CT_PRED 5
@@ -218,6 +220,12 @@ struct chd_contact_net {
   cudaEvent_t ev_up[4] = {nullptr, nullptr, nullptr, nullptr};
   void* io[8] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
   size_t io_bytes[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+  // CHD_CONTACT_TF32X3: split weight planes (one allocation) and the slab workspace of the tensor-core layers
+  int precision = CHD_CONTACT_FP32;
+  ChdContactTcNet tc = {};
+  float* tc_w = nullptr;
+  float* tc_ws = nullptr;
+  int tc_ws_rows = 0;
 };
 enum { IO_FRAMES = 0, IO_LENS = 1, IO_LABELS = 2, IO_LOGITS = 3, IO_MIN = 4, IO_RAW = 5, IO_OFFS = 6, IO_PACKED = 7 };
 
@@ -347,6 +355,8 @@ void chd_contact_destroy(chd_contact_net* net) {
   if (!net) return;
   for (void* p : net->allocs) cudaFree(p);
   if (net->ws) cudaFree(net->ws);
+  if (net->tc_w) cudaFree(net->tc_w);
+  if (net->tc_ws) cudaFree(net->tc_ws);
   for (int q = 0; q < 8; ++q)
     if (net->io[q]) cudaFree(net->io[q]);
   for (int q = 0; q < 4; ++q)
@@ -364,25 +374,44 @@ int chd_contact_forward_device(chd_contact_net* net, const double* frames_dev, i
   const float big = 3.4e38f;
   CT_CUDA(cudaMemcpyAsync(min_abs_dev, &big, sizeof(float), cudaMemcpyHostToDevice, s));
   const int rows = std::min(CT_SLAB, (total + GM - 1) / GM * GM);
-  if (rows > net->ws_rows) {
-    if (net->ws) cudaFree(net->ws);
-    net->ws = nullptr, net->ws_rows = 0;
-    CT_CUDA(cudaMalloc((void**)&net->ws, (size_t)rows * (CT_K0 + 1024 + 512 + 128) * sizeof(float)));
-    net->ws_rows = rows;
-  }
-  float* A0 = net->ws;
-  float* A1 = A0 + (size_t)net->ws_rows * CT_K0;
-  float* A2 = A1 + (size_t)net->ws_rows * 1024;
-  float* A3 = A2 + (size_t)net->ws_rows * 512;
   const ContactDev& d = net->dev;
-  for (int g0 = 0; g0 < total; g0 += CT_SLAB) {
-    const int Mp = (std::min(CT_SLAB, total - g0) + GM - 1) / GM * GM;
-    chd_k_contact_gather<<<(unsigned)(((size_t)Mp * CT_K0 + 255) / 256), 256, 0, s>>>(frames_dev, V, Fmax, g0, Mp, A0);
-    chd_k_contact_gemm<<<dim3(1024 / GN, Mp / GM), 256, 0, s>>>(A0, d.W[0], CT_K0, 1024, d.b[0], d.bn_scale[0], d.bn_mean[0], d.bn_beta[0], A1);
-    chd_k_contact_gemm<<<dim3(512 / GN, Mp / GM), 256, 0, s>>>(A1, d.W[1], 1024, 512, d.b[1], d.bn_scale[1], d.bn_mean[1], d.bn_beta[1], A2);
-    chd_k_contact_gemm<<<dim3(128 / GN, Mp / GM), 256, 0, s>>>(A2, d.W[2], 512, 128, d.b[2], d.bn_scale[2], d.bn_mean[2], d.bn_beta[2], A3);
-    chd_k_contact_tail<<<Mp / 32, 256, 0, s>>>(d, A3, g0, total, logits_dev);
-    net->launches += 5;
+  if (net->precision == CHD_CONTACT_TF32X3) {
+    // per slab: split gather, three tensor-core layers, FFMA tail (chd_contact_tc.cu)
+    if (rows > net->tc_ws_rows) {
+      if (net->tc_ws) cudaFree(net->tc_ws);
+      net->tc_ws = nullptr, net->tc_ws_rows = 0;
+      CT_CUDA(cudaMalloc((void**)&net->tc_ws, chd_contact_tc_ws_floats(rows) * sizeof(float)));
+      net->tc_ws_rows = rows;
+    }
+    ChdContactTcPlan plan;
+    int rc = chd_contact_tc_plan(&net->tc, net->tc_ws, net->tc_ws_rows, &plan);
+    if (rc) return rc;
+    for (int g0 = 0; g0 < total; g0 += CT_SLAB) {
+      const int Mp = (std::min(CT_SLAB, total - g0) + GM - 1) / GM * GM;
+      if ((rc = chd_contact_tc_layers(plan, frames_dev, V, Fmax, g0, Mp, s))) return rc;
+      chd_k_contact_tail<<<Mp / 32, 256, 0, s>>>(d, plan.a3, g0, total, logits_dev);
+      net->launches += 5;
+    }
+  } else {
+    if (rows > net->ws_rows) {
+      if (net->ws) cudaFree(net->ws);
+      net->ws = nullptr, net->ws_rows = 0;
+      CT_CUDA(cudaMalloc((void**)&net->ws, (size_t)rows * (CT_K0 + 1024 + 512 + 128) * sizeof(float)));
+      net->ws_rows = rows;
+    }
+    float* A0 = net->ws;
+    float* A1 = A0 + (size_t)net->ws_rows * CT_K0;
+    float* A2 = A1 + (size_t)net->ws_rows * 1024;
+    float* A3 = A2 + (size_t)net->ws_rows * 512;
+    for (int g0 = 0; g0 < total; g0 += CT_SLAB) {
+      const int Mp = (std::min(CT_SLAB, total - g0) + GM - 1) / GM * GM;
+      chd_k_contact_gather<<<(unsigned)(((size_t)Mp * CT_K0 + 255) / 256), 256, 0, s>>>(frames_dev, V, Fmax, g0, Mp, A0);
+      chd_k_contact_gemm<<<dim3(1024 / GN, Mp / GM), 256, 0, s>>>(A0, d.W[0], CT_K0, 1024, d.b[0], d.bn_scale[0], d.bn_mean[0], d.bn_beta[0], A1);
+      chd_k_contact_gemm<<<dim3(512 / GN, Mp / GM), 256, 0, s>>>(A1, d.W[1], 1024, 512, d.b[1], d.bn_scale[1], d.bn_mean[1], d.bn_beta[1], A2);
+      chd_k_contact_gemm<<<dim3(128 / GN, Mp / GM), 256, 0, s>>>(A2, d.W[2], 512, 128, d.b[2], d.bn_scale[2], d.bn_mean[2], d.bn_beta[2], A3);
+      chd_k_contact_tail<<<Mp / 32, 256, 0, s>>>(d, A3, g0, total, logits_dev);
+      net->launches += 5;
+    }
   }
   chd_k_contact_vote<<<(V * Fmax * 4 + 255) / 256, 256, 0, s>>>(logits_dev, V, Fmax, seq_lens_dev, (long long*)labels_dev, min_abs_dev);
   net->launches += 1;
@@ -512,5 +541,42 @@ int chd_contact_detect(chd_contact_net* net, const double* raw, const int32_t* s
 }
 
 int64_t chd_contact_launch_count(const chd_contact_net* net) { return net ? net->launches : 0; }
+
+int chd_contact_set_precision(chd_contact_net* net, int32_t precision) {
+  if (!net || (precision != CHD_CONTACT_FP32 && precision != CHD_CONTACT_TF32X3)) return -1;
+  if (precision == CHD_CONTACT_FP32) {             // the FP32 kernels never read the fast mode's buffers
+    if (net->tc_w) cudaFree(net->tc_w);
+    if (net->tc_ws) cudaFree(net->tc_ws);
+    net->tc_w = nullptr, net->tc_ws = nullptr, net->tc_ws_rows = 0, net->tc = ChdContactTcNet{};
+  } else if (!net->tc_w) {                         // split the weights of the three large layers once
+    const int K[3] = {CT_K0, 1024, 512}, N[3] = {1024, 512, 128};
+    size_t n = 0;
+    for (int l = 0; l < 3; ++l) n += 2 * (size_t)K[l] * N[l];
+    float* w = nullptr;
+    CT_CUDA(cudaMalloc((void**)&w, n * sizeof(float)));
+    ChdContactTcNet tc = {};
+    float* p = w;
+    int rc = 0;
+    for (int l = 0; l < 3 && !rc; ++l) {
+      float *hi = p, *lo = p + (size_t)K[l] * N[l];
+      p = lo + (size_t)K[l] * N[l];
+      tc.w_hi[l] = hi, tc.w_lo[l] = lo;
+      tc.bias[l] = net->dev.b[l], tc.scale[l] = net->dev.bn_scale[l], tc.mean[l] = net->dev.bn_mean[l], tc.beta[l] = net->dev.bn_beta[l];
+      rc = chd_contact_tc_split(net->dev.W[l], K[l], N[l], hi, lo, net->stream);
+      net->launches += 1;
+    }
+    if (!rc) {
+      const cudaError_t e = cudaStreamSynchronize(net->stream);
+      if (e != cudaSuccess) rc = -100 - (int)e;
+    }
+    if (rc) {
+      cudaFree(w);
+      return rc;
+    }
+    net->tc_w = w, net->tc = tc;
+  }
+  net->precision = precision;
+  return 0;
+}
 
 }  // extern "C"

@@ -194,10 +194,11 @@ def solve_sharded(problems, weights=(0.4, 1.7, 0.3, 0.1, 0.1), device: int = 0, 
 # Contact classifier: videos are independent too (SURVEY.md 8(e)): shard by frame count, one gather of the int64 labels.
 # ---------------------------------------------------------------------------------------------------------------------
 def detect_contacts_sharded(raw, state_dict=None, device: int = 0, rank: int = 0, world: int = 1, group=None, detect_fn=None,
-                            gather_device=None):
+                            gather_device=None, precision: str = "fp32"):
     """`raw`: list of (F_i, 25, 3) OpenPose keypoint arrays, identical on every rank.  Every rank runs
     `ContactNet.detect` (`chd_contact_detect`: preprocessing, windows, network, votes on its GPU) on its shard, the
     (slots, F_max, 4) int64 label blocks are gathered once and put back in input order.  Returns the list of (F_i, 4) labels.
+    `precision`: numerical mode of every rank's `ContactNet` ("fp32" or "tf32x3").
     `detect_fn(list_of_raw) -> list of (F_i, 4)` replaces the CUDA path in the CPU tests."""
     import torch
     n = len(raw)
@@ -213,7 +214,7 @@ def detect_contacts_sharded(raw, state_dict=None, device: int = 0, rank: int = 0
     batch = [raw[i] for i in mine] + ([raw[longest]] if mine and longest not in mine else [])
     if detect_fn is None:
         from .contact import ContactNet
-        net = ContactNet(state_dict, device=device)
+        net = ContactNet(state_dict, device=device, precision=precision)
         labels = net.detect(batch)[0][:len(mine)] if mine else []
         net.close()
     else:

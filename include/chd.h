@@ -178,6 +178,17 @@ int chd_contact_preprocess(chd_contact_net* net, const double* raw, const int32_
 int chd_contact_detect(chd_contact_net* net, const double* raw, const int32_t* seq_offsets, int32_t V, int32_t dim_w,
                        int64_t* labels_out, float* min_abs_logit);
 int64_t chd_contact_launch_count(const chd_contact_net* net);
+/* Numerical mode of every later chd_contact_forward / _forward_device / _detect call on this net.
+ * FP32 (default): FFMA, labels match the reference's fp32 forward.  TF32X3: the 352-1024-512-128 layers on the
+ * tensor core (wgmma) with every operand split into two TF32 parts, three products per term; logits within 5e-5
+ * absolute of an fp64 forward (measured on an H100: 8.3e-6 on the golden clips, fp32 mode 8.5e-7; at most 1.1e-5 from
+ * the fp32 mode over 100k windows), so labels can differ from FP32 only where a logit is within about 1e-5 of zero.
+ * The slab workspace grows from 7.9 KB to 15.3 KB per window (132 MB -> 256 MB for a full slab of 16384 windows) and
+ * the split weights take 7.6 MB.  Switching back to FP32 frees the fast mode's buffers; results are then bitwise
+ * those of a net that never left FP32.
+ * Returns 0, -1 bad argument, <= -100 CUDA error. */
+enum { CHD_CONTACT_FP32 = 0, CHD_CONTACT_TF32X3 = 1 };
+int chd_contact_set_precision(chd_contact_net* net, int32_t precision);
 
 /* OpenPose keypoint ingestion on the host threads (replaces the serial per-file json.load of
  * src/utils/openpose_utils.py:48-76 load_keypoint_file / load_keypoint_dir): n_files `*_keypoints.json` files ->

@@ -23,10 +23,13 @@ def main(argv=None):
     ap.add_argument("--viz", action="store_true")
     ap.add_argument("--classify-thresh", type=float, default=0.5)
     ap.add_argument("--copy-into-data", action="store_true")
+    ap.add_argument("--precision", choices=["fp32", "tf32x3"], default="fp32",
+                    help="fp32: labels match the reference's fp32 forward; tf32x3: the large layers on the tensor core "
+                         "with split TF32 operands")
     args = ap.parse_args(argv)
     import chd
     sd = chd.contact.load_weights(args.weights)
-    written = chd.contact.detect_contacts(args.data, args.out, sd)
+    written = chd.contact.detect_contacts(args.data, args.out, sd, precision=args.precision)
     for w in written:
         print("wrote", w)
         if args.copy_into_data:
