@@ -251,14 +251,22 @@ int chd_measure_fp64_peak(double* dfma_gflops, double* dmma_gflops) {
 }
 
 static int batch_create_impl(const chd_phys_problem* problems, int32_t batch, const chd_phys_weights* weights, int32_t device,
-                             chd_phys_batch* b);
+                             const chd_phys_options& opt, chd_phys_batch* b);
 
 int chd_phys_batch_create(const chd_phys_problem* problems, int32_t batch, const chd_phys_weights* weights, int32_t device,
                           chd_phys_batch** out) {
+  return chd_phys_batch_create_ex(problems, batch, weights, device, nullptr, out);
+}
+
+int chd_phys_batch_create_ex(const chd_phys_problem* problems, int32_t batch, const chd_phys_weights* weights, int32_t device,
+                             const chd_phys_options* opt, chd_phys_batch** out) {
   if (!problems || batch <= 0 || !out) return -1;
+  chd_phys_options o = {-1};
+  if (opt) o = *opt;
+  if (o.stage3_band_above < -1 || o.stage3_band_above > CHD_MAX_DUR) return -1;
   chd_phys_batch* b = new chd_phys_batch();
   std::memset(&b->D, 0, sizeof(b->D));
-  const int rc = batch_create_impl(problems, batch, weights, device, b);
+  const int rc = batch_create_impl(problems, batch, weights, device, o, b);
   if (rc) {
     chd_phys_batch_destroy(b);   // single cleanup path: streams, events, pooled allocations, host buffers
     return rc;
@@ -268,12 +276,12 @@ int chd_phys_batch_create(const chd_phys_problem* problems, int32_t batch, const
 }
 
 static int batch_create_impl(const chd_phys_problem* problems, int32_t batch, const chd_phys_weights* weights, int32_t device,
-                             chd_phys_batch* b) {
+                             const chd_phys_options& opt, chd_phys_batch* b) {
   const bool host_only = device == -2;  // layout tables only, no CUDA call (CPU-side tests of the host logic)
   if (device >= 0) CHD_CUDA(cudaSetDevice(device));
   chd_phys_weights w = {0.4, 1.7, 0.3, 0.1, 0.1};  // phys_optim.cpp:27-31
   if (weights) w = *weights;
-  int rc = chd_build_layout(problems, batch, w, b->hb);
+  int rc = chd_build_layout(problems, batch, w, b->hb, opt.stage3_band_above);
   if (rc) return rc;
   ChdHostBatch& hb = b->hb;
   ChdDev& D = b->D;
@@ -362,21 +370,23 @@ static int batch_create_impl(const chd_phys_problem* problems, int32_t batch, co
     // long horizons / wide bands: vectors and window in a global scratch area (chd_k_kkt_gwin)
     D.win_smem = 0;
     D.pan_doubles = 2 * (D.Q + D.nbt) * 64;
-    b->smem_kkt = (CHD_KKT_THREADS + nbp8 * nbp8 + (size_t)D.pan_doubles + 16) * sizeof(double);
+    b->smem_kkt = chd_kkt_gwin_smem(D.Q, D.nbt);
     D.scratch_stride = n_even + xs_len + 8 * (size_t)D.nbc_max + (size_t)D.win_tiles * 64 + (size_t)D.Q * D.nbt * 64;
     if ((rc = dev_alloc(b, B * D.scratch_stride, &D.scratch))) return rc;
-    if (D.Q - 1 + D.nbt > 76) {
+    if (D.Q - 1 + D.nbt > CHD_KKT_GROUPS_MAX) {
       fprintf(stderr, "libchd: band + border too wide for the pair tables (Q=%d nbt=%d)\n", D.Q, D.nbt);
       return -5;
     }
   }
-  if (b->smem_eval + 1024 > (size_t)smem_max || b->smem_kkt + kkt_static + 256 > (size_t)smem_max) {
+  // (the global-window kernel has more static shared memory than chd_k_kkt: its pair table holds up to 96 panel groups)
+  CHD_CUDA(cudaFuncGetAttributes(&fa, chd_k_kkt_gwin));
+  const size_t kkt_static_used = D.win_smem ? kkt_static : fa.sharedSizeBytes;
+  if (b->smem_eval + 1024 > (size_t)smem_max || b->smem_kkt + kkt_static_used + 256 > (size_t)smem_max) {
     fprintf(stderr, "libchd: problem too large for the shared-memory staged kernels (n_max=%d)\n", hb.n_max);
     return -5;
   }
   CHD_CUDA(cudaFuncSetAttribute(chd_k_eval, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)b->smem_eval));
-  CHD_CUDA(cudaFuncSetAttribute(chd_k_kkt, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)b->smem_kkt));
-  CHD_CUDA(cudaFuncSetAttribute(chd_k_kkt_gwin, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)b->smem_kkt));
+  CHD_CUDA(cudaFuncSetAttribute(D.win_smem ? chd_k_kkt : chd_k_kkt_gwin, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)b->smem_kkt));
   CHD_CUDA(cudaFuncSetAttribute(chd_k_linesearch, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)b->smem_ls));
   const size_t stride = 6 + 7 * (size_t)hb.n_ee_max;
   CHD_CUDA(cudaMallocAsync((void**)&b->d_samples, B * hb.fo_max * stride * sizeof(double), b->stream));
@@ -600,7 +610,7 @@ int chd_phys_sample(chd_phys_batch* b, double* out, int32_t* frames_out) {
 // Staged schedule of phys_optim.cpp:554-749.  Every sequence walks through 1.1, 1.2, 2.1, 2.2, 3 and -- only when its
 // stage 3 did not succeed (:713-749) -- 4 at its own pace (converged sequences do not wait for the slowest one of
 // their stage).  Stage status -9 = stage not run (stage 4 after a successful stage 3), -3 = stage 3 not attempted
-// (more phase durations than CHD_MAX_DUR).
+// (more phase durations than CHD_MAX_DUR with the switch times in the border, or a banded layout too wide).
 int chd_phys_solve(chd_phys_batch* b, double* samples, int32_t* frames_out, int32_t* success, int32_t* stage_status,
                    int32_t* stage_iters) {
   if (!b || b->host_only) return -1;

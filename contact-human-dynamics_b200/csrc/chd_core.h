@@ -33,7 +33,8 @@ enum ChdSetType : int {
 };
 #define CHD_TAU_TRUST 0.04   /* [s] stage 3 keeps every switch time within this distance of its input value: the layout sizes the
                                 band for the polynomials that can move onto a sample time within it (line-search trials beyond are refused) */
-#define CHD_MAX_DUR 96   /* most phase-duration variables (sum over feet of P-1) stage 3 handles as dense border unknowns */
+#define CHD_MAX_DUR 96   /* most phase-duration variables (sum over feet of P-1) stage 3 handles as dense border unknowns
+                            (more need banded switch times: chd_phys_options) */
 // stage bit masks over set types (phys_optim.cpp:554-749, SURVEY Appendix B)
 #define CHD_MASK(t) (1u << (t))
 enum ChdStage : int { CHD_STAGE_11 = 0, CHD_STAGE_12 = 1, CHD_STAGE_21 = 2, CHD_STAGE_22 = 3, CHD_STAGE_3 = 4, CHD_STAGE_4 = 5 };
@@ -71,9 +72,11 @@ struct ChdSeq {
   int n_dyn, n_rom, n_smooth;
   int Na, nb, w;  // KKT: banded unknowns, border unknowns (stance positions, then the switch times), half bandwidth
   int n_dur;      // phase-duration variables (0: stage 3 not available for this sequence), the last n_dur entries of x
-  int nb_fix;     // border unknowns of the fixed-duration stages (= nb - n_dur)
+  int nb_fix;     // border unknowns of the fixed-duration stages (= nb - n_dur, or nb when dur_band)
   int w_fix;      // half bandwidth of the fixed-duration stages (static pattern); w additionally covers the polynomials
                   // stage 3 may move onto a sample time
+  int dur_band;   // 1: the switch times are band unknowns (time ordered) instead of the last n_dur border unknowns; the
+                  // fixed-duration stages give them a unit diagonal and no couplings
   int dur_xoff[CHD_MAX_EE];   // first duration variable of every foot (P - 1 of them)
   double dt, T, mass, grav, mu, max_leg, max_heel, heel_dist, force_limit;
   double normal[3], point[3], gvec[3], nrm[3], tan1[3], tan2[3], dhdx, dhdy;

@@ -21,7 +21,8 @@ __global__ void chd_k_stage_begin(ChdDev D) {
   const int max_iter = sg.max_iter;
   const ChdSeq* h = D.seq + b;
   if (sg.opt_dur && h->n_dur == 0) {
-    // more phase durations than the dense border holds (CHD_MAX_DUR): stage 3 is not attempted; like the reference
+    // more phase durations than the dense border holds (CHD_MAX_DUR) and no banded switch times: stage 3 is not
+    // attempted; like the reference
     // after a failed stage 3 the schedule continues with the fixed-duration stage 4 (phys_optim.cpp:713-749)
     __syncthreads();
     if (threadIdx.x == 0) {

@@ -96,6 +96,11 @@ __device__ void chd_hess_build(const ChdDev& D, int b, const ChdStageDev& sg, do
   }
   if (part == 0)
     for (int i = K.Na + tid; i < K.Np; i += nt) K.band[((size_t)(i >> 3) * K.Q) * 64 + (i & 7) * 9] = 1.0;  // identity padding of the band
+  if (part == 0 && !sg.opt_dur && h->dur_band)   // banded switch times outside stage 3: decoupled unknowns, unit diagonal
+    for (int i = tid; i < h->n_dur; i += nt) {
+      const int k = vk[h->dur_xoff[0] + i];   // the duration variables of all feet are contiguous in x
+      K.band[((size_t)(k >> 3) * K.Q) * 64 + (k & 7) * 9] = 1.0;
+    }
   if (part == 0 && sg.opt_dur && sg.w_dur != 0.0) {   // duration_cost.cpp: w I in the durations = w D^T D in the switch times
     for (int ee = 0; ee < n_ee; ++ee)
       for (int k = tid; k < h->n_phases[ee] - 1; k += nt) {
@@ -780,11 +785,14 @@ __device__ __forceinline__ void chd_kkt_factor(const ChdKktCtx& c, int& s_fail) 
   // window slot of every band group of the current block column (double buffered, no integer division)
   __shared__ int s_rs[2][96];
   __shared__ int s_gnz[2][96];   // per panel group: any non-zero entry in the X tile (zero tiles skip their trailing updates)
-  __shared__ unsigned short s_pairs[3000];
+  // pair table: at most 64 panel groups with the shared-memory window, 96 with the global one (its static shared memory
+  // is not needed for a window)
+  constexpr int kPairs = WS ? 3000 : CHD_KKT_GROUPS_MAX * (CHD_KKT_GROUPS_MAX + 1) / 2;
+  __shared__ unsigned short s_pairs[kPairs];
   __shared__ unsigned char s_cmp[CHD_KKT_THREADS / 32][64];   // per warp: rank -> id of the non-zero panel groups
   __shared__ __align__(16) double s_winv[2][64];   // inverse of the current / next diagonal tile factor, fragment order
   const int GB = K.q, Gm = K.q + nbt_s, npairs = Gm * (Gm + 1) / 2;
-  for (int p = tid; p < npairs && p < 3000; p += nt) {
+  for (int p = tid; p < npairs && p < kPairs; p += nt) {
     int gi = (int)((sqrt(8.0 * p + 1.0) - 1.0) * 0.5);
     while (gi * (gi + 1) / 2 > p) --gi;
     while ((gi + 1) * (gi + 2) / 2 <= p) ++gi;

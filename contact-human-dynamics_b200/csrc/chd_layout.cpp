@@ -1,5 +1,6 @@
 // Host-side layout builder (product code).  See chd_layout.h.
 #include "chd_layout.h"
+#include "chd_dev.h"
 
 #include <algorithm>
 #include <atomic>
@@ -91,7 +92,17 @@ std::vector<double> discretize(double T, double dt) {
   return d;
 }
 
-int build_sequence(const chd_phys_problem& p, SeqBuild& sb) {
+// Whether a KKT system of half bandwidth w_max and nb_max border unknowns fits chd_k_kkt_gwin, the kernel bands this
+// wide run in: its pair table (panel groups) and its shared memory.  Checked for the whole batch, whose strides come
+// from the widest band and the largest border of possibly different sequences.
+bool kkt_fits(int w_max, int nb_max) {
+  const int Q = (w_max + 7) / 8 + 1, nbt = (nb_max + 1 + 7) / 8;
+  return Q - 1 + nbt <= CHD_KKT_GROUPS_MAX && chd_kkt_gwin_smem(Q, nbt) + CHD_KKT_GWIN_STATIC_MAX <= CHD_SMEM_OPTIN;
+}
+
+// Returns 0, a negative code for malformed input, or 1 when banded switch times would make the band too wide for the
+// KKT kernels (the caller then builds the sequence again without them).
+int build_sequence(const chd_phys_problem& p, SeqBuild& sb, int band_above) {
   if (p.n_ee != 2 && p.n_ee != 4) return -2;
   if (p.n_frames < 12) return -3;
   const int F = p.n_frames, n_ee = p.n_ee;
@@ -254,7 +265,8 @@ int build_sequence(const chd_phys_problem& p, SeqBuild& sb) {
   {
     int nd = 0;
     for (int ee = 0; ee < n_ee; ++ee) nd += P[ee] - 1;
-    h.n_dur = nd <= CHD_MAX_DUR ? nd : 0;
+    h.dur_band = band_above >= 0 && nd > band_above;
+    h.n_dur = nd <= CHD_MAX_DUR || h.dur_band ? nd : 0;
     for (int ee = 0; ee < n_ee; ++ee) {
       h.dur_xoff[ee] = xoff;
       if (!h.n_dur) continue;
@@ -282,8 +294,53 @@ int build_sequence(const chd_phys_problem& p, SeqBuild& sb) {
       }
     }
   }
+  // input switch times: ph_end[ee][k] = end of phase k of foot ee
+  std::vector<std::vector<double>> ph_end(n_ee);
+  for (int ee = 0; ee < n_ee; ++ee) {
+    double t = 0.0;
+    for (int k = 0; k < P[ee]; ++k) t += dur[ee][k], ph_end[ee].push_back(t);
+  }
+  const double margin = CHD_TAU_TRUST;   // [s] how far stage 3 may move a switch time (and with it a polynomial boundary)
   for (int v = 0; v < h.n; ++v)
     if (sb.var_dur[v]) sb.var_t0[v] = 0.0, sb.var_t1[v] = T;
+  // banded switch times: tau_k bounds phases k and k+1, whose rows and cost samples are all it touches
+  if (h.dur_band)
+    for (int ee = 0; ee < n_ee; ++ee)
+      for (int k = 0; k < P[ee] - 1; ++k) {
+        const int v = h.dur_xoff[ee] + k;
+        sb.var_t0[v] = (k > 0 ? ph_end[ee][k - 1] : 0.0) - margin;
+        sb.var_t1[v] = (k + 1 < P[ee] - 1 ? ph_end[ee][k + 1] : T) + margin;
+      }
+  // Switch times a sample at time t can depend on in stage 3: a sample in phase j of foot ee depends on tau_{j-1} and
+  // tau_j, and once every switch time has moved by up to the trust margin t may lie in a neighbouring phase instead.
+  // One option (pair of variables, -1 for the fixed ends 0 and T) per phase t can lie in, appended to `opts`.
+  auto tau_reach = [&](int ee, double t, std::vector<std::vector<int>>& opts) {
+    if (!h.dur_band) return;
+    std::vector<int> o;
+    for (int j = 0; j < P[ee]; ++j) {   // (the last phase runs to T whatever the input durations of the foot add up to)
+      const double a = j > 0 ? ph_end[ee][j - 1] : -1e300, b = j < P[ee] - 1 ? ph_end[ee][j] : 1e300;
+      if (t < a - margin || t > b + margin) continue;
+      o.push_back(j >= 1 ? h.dur_xoff[ee] + j - 1 : -1);
+      o.push_back(j <= P[ee] - 2 ? h.dur_xoff[ee] + j : -1);
+    }
+    opts.push_back(o);
+  };
+  // calls fn(cols) with `base` plus one option of every entry of `opts` for each combination (fn(base) when empty)
+  auto for_options = [](const std::vector<int>& base, const std::vector<std::vector<int>>& opts, auto&& fn) {
+    size_t total = 1;
+    for (const auto& o : opts) total *= o.size() / 2;
+    std::vector<int> cols;
+    for (size_t c = 0; c < total; ++c) {
+      cols = base;
+      size_t rem = c;
+      for (const auto& o : opts) {
+        const size_t k = rem % (o.size() / 2);
+        rem /= o.size() / 2;
+        cols.push_back(o[2 * k]), cols.push_back(o[2 * k + 1]);
+      }
+      fn(cols);
+    }
+  };
   // time tables
   sb.t_dyn = discretize(T, 0.1);   // parameters.cpp:58-59 (dynamic and height share dt = 0.1)
   sb.t_rom = discretize(T, 0.08);  // parameters.cpp:57
@@ -340,9 +397,10 @@ int build_sequence(const chd_phys_problem& p, SeqBuild& sb) {
   // In stage 3 the polynomial boundaries of the phase-based splines move with the durations, so the polynomial active
   // at a fixed sample time can change: the node columns of those blocks are re-assigned at run time (chd_k_eval), and
   // the bandwidth below is sized for the neighbouring polynomials too (row_ext = their extra nodes).
+  // With banded switch times, row_tau holds the switch-time options of the feet the row touches (tau_reach).
   std::vector<std::vector<int>> row_ext(h.m);
+  std::vector<std::vector<std::vector<int>>> row_tau(h.m);
   int cur_row = 0;
-  const double margin = CHD_TAU_TRUST;   // [s] how far stage 3 may move a polynomial boundary before a coupling can leave the band
   auto ext_nodes = [&](int s, int poly, double t, std::vector<int>& out) {
     if (s < 2 || !h.n_dur) return;
     auto put = [&](int node) {
@@ -391,6 +449,7 @@ int build_sequence(const chd_phys_problem& p, SeqBuild& sb) {
             sb.row_t[R] = t;
             block(0, t), block(1, t), block(chd_sp_motion(st.a), t);
             tau_slots(1);
+            tau_reach(st.a, t, row_tau[R]);
             const double L = st.a < 2 ? h.max_leg : h.max_heel;  // leg_length_constraint.cpp:21-27
             sb.row_lo[R] = 0.0, sb.row_hi[R] = 0.5 * L * L;
             break;
@@ -401,6 +460,7 @@ int build_sequence(const chd_phys_problem& p, SeqBuild& sb) {
             block(0, t), block(1, t);
             for (int ee = 0; ee < n_ee; ++ee) block(chd_sp_motion(ee), t), block(chd_sp_force(n_ee, ee), t);
             tau_slots(n_ee);
+            for (int ee = 0; ee < n_ee; ++ee) tau_reach(ee, t, row_tau[R]);
             break;
           }
           case CHD_SET_FORCE: {
@@ -418,6 +478,7 @@ int build_sequence(const chd_phys_problem& p, SeqBuild& sb) {
             sb.row_t[R] = t;
             block(chd_sp_motion(st.a), t), block(chd_sp_motion(st.b), t);
             tau_slots(2);
+            tau_reach(st.a, t, row_tau[R]), tau_reach(st.b, t, row_tau[R]);
             sb.row_lo[R] = sb.row_hi[R] = 0.5 * h.heel_dist * h.heel_dist;
             break;
           }
@@ -426,6 +487,7 @@ int build_sequence(const chd_phys_problem& p, SeqBuild& sb) {
             sb.row_t[R] = t;
             block(chd_sp_motion(st.a), t);
             tau_slots(1);
+            tau_reach(st.a, t, row_tau[R]);
             sb.row_lo[R] = 0.0, sb.row_hi[R] = 1e20;
             break;
           }
@@ -463,7 +525,7 @@ int build_sequence(const chd_phys_problem& p, SeqBuild& sb) {
     sb.var_kkt.assign(h.n, -1);
     sb.row_kkt.assign(h.m, -1);
     for (int v = 0; v < h.n; ++v) {
-      if (sb.var_fixed[v] || sb.var_dur[v]) continue;
+      if (sb.var_fixed[v] || (sb.var_dur[v] && !h.dur_band)) continue;
       if (sb.var_stance[v] && sb.var_t1[v] - sb.var_t0[v] > span_max) border.push_back(v);
       else keys.push_back({0.5 * (sb.var_t0[v] + sb.var_t1[v]), 0, v});
     }
@@ -478,9 +540,10 @@ int build_sequence(const chd_phys_problem& p, SeqBuild& sb) {
     h.Na = (int)keys.size();
     h.nb_fix = (int)border.size();
     // the switch times of stage 3 influence every row of two whole phases: dense border unknowns, placed last so that
-    // the fixed-duration stages simply work with the first nb_fix border unknowns
-    for (int v = 0; v < h.n; ++v)
-      if (sb.var_dur[v]) border.push_back(v);
+    // the fixed-duration stages simply work with the first nb_fix border unknowns (unless they are banded, above)
+    if (!h.dur_band)
+      for (int v = 0; v < h.n; ++v)
+        if (sb.var_dur[v]) border.push_back(v);
     h.nb = (int)border.size();
     for (int j = 0; j < h.nb; ++j) sb.var_kkt[border[j]] = h.Na + j;
     // half bandwidth from the coupling cliques: w_fix of the fixed-duration stages (the static pattern), w with the
@@ -491,6 +554,7 @@ int build_sequence(const chd_phys_problem& p, SeqBuild& sb) {
       int lo = 1 << 30, hi = -1;
       for (int i = 0; i < cnt; ++i) {
         if (cols[i] < 0) continue;
+        if (!with_ext && sb.var_dur[cols[i]]) continue;   // the fixed-duration stages never couple a switch time
         int k = sb.var_kkt[cols[i]];
         if (k < 0 || k >= h.Na) continue;
         lo = std::min(lo, k), hi = std::max(hi, k);
@@ -498,37 +562,48 @@ int build_sequence(const chd_phys_problem& p, SeqBuild& sb) {
       if (rowpos >= 0) lo = std::min(lo, rowpos), hi = std::max(hi, rowpos);
       if (hi >= 0) (with_ext ? w : w_fix) = std::max(with_ext ? w : w_fix, hi - lo);
     };
+    auto clique = [&](const std::vector<int>& cols) { span(cols.data(), (int)cols.size(), -1); };
+    // (banded switch times, stage 3: a clique holds the switch times of one phase per foot at a time -- the options of
+    // row_tau / tau_reach are alternatives, not one clique)
+    const std::vector<std::vector<int>> no_opts;
     std::vector<int> merged;
     for (int pass = 0; pass < 2; ++pass)
     for (int r = 0; r < h.m; ++r) {
       with_ext = pass == 1;
       merged.assign(sb.ent_col.begin() + sb.ent_ptr[r], sb.ent_col.begin() + sb.ent_ptr[r + 1]);
       if (with_ext) merged.insert(merged.end(), row_ext[r].begin(), row_ext[r].end());
+      const std::vector<std::vector<int>>& opts = with_ext ? row_tau[r] : no_opts;
       const int* c = merged.data();
       const int cnt = (int)merged.size();
       if (sb.row_kkt[r] >= 0) {  // explicit row: couples the row with each of its variables
         for (int i = 0; i < cnt; ++i) span(c + i, 1, sb.row_kkt[r]);
-        if (sb.row_set[r] == CHD_SET_ROM || sb.row_set[r] == CHD_SET_HEEL) span(c, cnt, -1);  // curvature term y+ Jd^T Jd
+        for (const auto& o : opts)
+          for (size_t i = 0; i < o.size(); ++i) span(&o[i], 1, sb.row_kkt[r]);
+        if (sb.row_set[r] == CHD_SET_ROM || sb.row_set[r] == CHD_SET_HEEL) for_options(merged, opts, clique);  // curvature term y+ Jd^T Jd
       } else {
-        span(c, cnt, -1);        // condensed inequality row: J^T Sigma J clique
+        for_options(merged, opts, clique);        // condensed inequality row: J^T Sigma J clique
       }
     }
-    // cost cliques: data samples (one polynomial) and smoothing samples (polynomials at t and t + dt)
+    // cost cliques: data samples (one polynomial) and smoothing samples (polynomials at t and t + dt); stage 3 adds the
+    // switch times of the foot splines' positions (the duration cost w D^T D couples the same pairs as the DURPOS rows)
     for (int pass = 0; pass < 2; ++pass)
     for (int s = 0; s < 2 + n_ee; ++s) {
       with_ext = pass == 1;
       for (int i = 0; i < F; ++i) {
         std::vector<int> cols;
+        std::vector<std::vector<int>> opts;
         double tl;
         int poly = chd_locate(tend[s].data(), sb.sp[s].npoly(), sb.t_data[i], &tl);
         for (int q = 0; q < 12; ++q) cols.push_back(sb.sp[s].var[poly * 6 + q]);
         if (with_ext) ext_nodes(s, poly, sb.t_data[i], cols);
+        if (with_ext && s >= 2) tau_reach(s - 2, sb.t_data[i], opts);
         if (i < h.n_smooth) {
           int poly2 = chd_locate(tend[s].data(), sb.sp[s].npoly(), sb.t_data[i] + p.dt, &tl);
           for (int q = 0; q < 12; ++q) cols.push_back(sb.sp[s].var[poly2 * 6 + q]);
           if (with_ext) ext_nodes(s, poly2, sb.t_data[i] + p.dt, cols);
+          if (with_ext && s >= 2) tau_reach(s - 2, sb.t_data[i] + p.dt, opts);
         }
-        span(cols.data(), (int)cols.size(), -1);
+        for_options(cols, opts, clique);
       }
     }
     w = std::max(w, w_fix);
@@ -547,12 +622,14 @@ int build_sequence(const chd_phys_problem& p, SeqBuild& sb) {
     if (ci == 0 || cst < 0.9 * best_cost) best = ci, best_cost = cst;   // leave the default unless clearly better
   }
   order_kkt(cand[best]);
+  if (h.dur_band && !kkt_fits(h.w, h.nb)) return 1;
   return 0;
 }
 
 }  // namespace
 
-int chd_build_layout(const chd_phys_problem* problems, int batch, const chd_phys_weights& wt, ChdHostBatch& hb) {
+int chd_build_layout(const chd_phys_problem* problems, int batch, const chd_phys_weights& wt, ChdHostBatch& hb,
+                     int stage3_band_above) {
   std::vector<SeqBuild> sbs(batch);
   {
     // sequences are independent: build their tables on the host cores in parallel (end-to-end latency of a batch)
@@ -560,7 +637,13 @@ int chd_build_layout(const chd_phys_problem* problems, int batch, const chd_phys
     std::vector<int> rcs(batch, 0);
     std::atomic<int> next(0);
     auto work = [&]() {
-      for (int i = next.fetch_add(1); i < batch; i = next.fetch_add(1)) rcs[i] = build_sequence(problems[i], sbs[i]);
+      for (int i = next.fetch_add(1); i < batch; i = next.fetch_add(1)) {
+        rcs[i] = build_sequence(problems[i], sbs[i], stage3_band_above);
+        if (rcs[i] == 1) {   // banded switch times too wide for the kernels: the layout without them
+          sbs[i] = SeqBuild();
+          rcs[i] = build_sequence(problems[i], sbs[i], -1);
+        }
+      }
     };
     std::vector<std::thread> pool;
     for (int t = 1; t < nth; ++t) pool.emplace_back(work);
@@ -568,6 +651,20 @@ int chd_build_layout(const chd_phys_problem* problems, int batch, const chd_phys
     for (auto& t : pool) t.join();
     for (int i = 0; i < batch; ++i)
       if (rcs[i]) return rcs[i];
+  }
+  // The kernels' limits hold for the batch (band strides from the widest band, border from the largest one): while it
+  // does not fit, the banded sequence with the widest band is built again without banded switch times.  A batch that
+  // does not fit without any banded sequence is left to batch creation's own checks, as without the option.
+  while (true) {
+    int w_max = 0, nb_max = 0, widest = -1;
+    for (int i = 0; i < batch; ++i) {
+      w_max = std::max(w_max, sbs[i].h.w), nb_max = std::max(nb_max, sbs[i].h.nb);
+      if (sbs[i].h.dur_band && (widest < 0 || sbs[i].h.w > sbs[widest].h.w)) widest = i;
+    }
+    if (widest < 0 || kkt_fits(w_max, nb_max)) break;
+    sbs[widest] = SeqBuild();
+    const int rc = build_sequence(problems[widest], sbs[widest], -1);
+    if (rc) return rc;
   }
   hb.B = batch;
   auto up = [](int& a, int b) { a = std::max(a, b); };

@@ -33,5 +33,7 @@ struct ChdHostBatch {
   int par_stride() const { return (18 + 3 * n_ee_max) * F_max; }
 };
 
-// returns 0 on success; negative on malformed input
-int chd_build_layout(const chd_phys_problem* problems, int batch, const chd_phys_weights& w, ChdHostBatch& out);
+// returns 0 on success; negative on malformed input.  stage3_band_above: see chd_phys_options (-1: switch times are
+// border unknowns, stage 3 limited to CHD_MAX_DUR of them)
+int chd_build_layout(const chd_phys_problem* problems, int batch, const chd_phys_weights& w, ChdHostBatch& out,
+                     int stage3_band_above = -1);

@@ -77,10 +77,11 @@ class ShardedSolver:
     takes part in a single all_gather of the fixed-size result block (final SaveSolution snapshot + status trailer).
 
     `solve_fn(problems) -> dict(final=(n, fo, stride) array, frames, success, stage_status (6,n), stage_iters (6,n))`
-    replaces the CUDA solve in the CPU (gloo) tests; the default drives `PhysBatch` on `device`."""
+    replaces the CUDA solve in the CPU (gloo) tests; the default drives `PhysBatch` on `device` (`stage3_band_above`:
+    see `PhysBatch`)."""
 
     def __init__(self, problems, weights=(0.4, 1.7, 0.3, 0.1, 0.1), device: int = 0, rank: int = 0, world: int = 1,
-                 group=None, solve_fn=None, tensor_device=None):
+                 group=None, solve_fn=None, tensor_device=None, stage3_band_above=None):
         self.problems, self.rank, self.world, self.group = list(problems), rank, world, group
         self.shards = shard_by_work(work_estimate(self.problems), world)
         self.slots = pad_to(self.shards)
@@ -94,7 +95,8 @@ class ShardedSolver:
         import torch
         if solve_fn is None:
             from . import phys
-            self.batch = phys.PhysBatch([self.problems[i] for i in self.mine], weights=weights, device=device) if self.mine else None
+            self.batch = phys.PhysBatch([self.problems[i] for i in self.mine], weights=weights, device=device,
+                                        stage3_band_above=stage3_band_above) if self.mine else None
             tensor_device = tensor_device or torch.device("cuda", device)
         self.tdev = tensor_device or torch.device("cpu")
         self.send = torch.zeros((self.slots, self.width), dtype=torch.float64, device=self.tdev)
@@ -181,9 +183,9 @@ class ShardedSolver:
 
 
 def solve_sharded(problems, weights=(0.4, 1.7, 0.3, 0.1, 0.1), device: int = 0, rank: int = 0, world: int = 1, group=None,
-                  solve_fn=None, tensor_device=None) -> dict:
+                  solve_fn=None, tensor_device=None, stage3_band_above=None) -> dict:
     """shard -> solve -> one gather -> unshard for a list of `PhysProblem`s (see ShardedSolver)."""
-    s = ShardedSolver(problems, weights, device, rank, world, group, solve_fn, tensor_device)
+    s = ShardedSolver(problems, weights, device, rank, world, group, solve_fn, tensor_device, stage3_band_above)
     try:
         return s.solve()
     finally:

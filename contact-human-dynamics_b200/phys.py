@@ -41,12 +41,16 @@ class _Weights(C.Structure):
                 ("w_dur", C.c_double)]
 
 
+class _Options(C.Structure):
+    _fields_ = [("stage3_band_above", C.c_int32)]
+
+
 class _Dims(C.Structure):
     _fields_ = [(k, C.c_int32) for k in ("batch", "n_max", "m_max", "slots_max", "n_splines", "p_max", "sets_max",
                                           "na_max", "nb_max", "w_max", "frames_out_max")]
 
 
-EXPORTS = ["chd_version", "chd_phys_batch_create", "chd_phys_batch_destroy", "chd_phys_get_dims", "chd_phys_get_sizes",
+EXPORTS = ["chd_version", "chd_phys_batch_create", "chd_phys_batch_create_ex", "chd_phys_batch_destroy", "chd_phys_get_dims", "chd_phys_get_sizes",
            "chd_phys_get_x", "chd_phys_set_x", "chd_phys_eval", "chd_phys_get_layout", "chd_phys_solve_stage",
            "chd_phys_solve", "chd_phys_sample", "chd_phys_sample_device", "chd_phys_launch_count",
            "chd_phys_kernel_times", "chd_phys_set_timing", "chd_phys_h2d_bytes", "chd_phys_reset", "chd_measure_fp64_peak", "chd_phys_get_slot_index", "chd_phys_get_ent_col",
@@ -79,6 +83,8 @@ def load_lib():
         L.chd_phys_launch_count.restype = C.c_int64
         L.chd_phys_batch_create.argtypes = [C.POINTER(_Problem), C.c_int32, C.POINTER(_Weights), C.c_int32,
                                             C.POINTER(C.c_void_p)]
+        L.chd_phys_batch_create_ex.argtypes = [C.POINTER(_Problem), C.c_int32, C.POINTER(_Weights), C.c_int32,
+                                               C.POINTER(_Options), C.POINTER(C.c_void_p)]
         L.chd_phys_batch_destroy.argtypes = [C.c_void_p]
         L.chd_phys_batch_destroy.restype = None
         vp = C.c_void_p
@@ -148,15 +154,23 @@ def make_problem_array(problems):
 
 
 class PhysBatch:
+    """`stage3_band_above`: sequences with more phase-duration variables than this carry their switch times as banded
+    KKT unknowns, which lets stage 3 run beyond the 96 the dense border holds (0 bands every sequence; None: none)."""
+
     def __init__(self, problems: Sequence[PhysProblem], weights=(0.4, 1.7, 0.3, 0.1, 0.1), device: int = -1,
-                 host_only: bool = False):
+                 host_only: bool = False, stage3_band_above: Optional[int] = None):
         self.L = load_lib()
         self.problems = list(problems)
         B = len(self.problems)
         arr, self._keep = make_problem_array(self.problems)
         w = _Weights(*[float(x) for x in weights])
         h = C.c_void_p()
-        rc = self.L.chd_phys_batch_create(arr, B, C.byref(w), -2 if host_only else device, C.byref(h))
+        dev = -2 if host_only else device
+        if stage3_band_above is None:
+            rc = self.L.chd_phys_batch_create(arr, B, C.byref(w), dev, C.byref(h))
+        else:   # values outside 0..96 are rejected by the library (code -1)
+            opt = _Options(int(stage3_band_above))
+            rc = self.L.chd_phys_batch_create_ex(arr, B, C.byref(w), dev, C.byref(opt), C.byref(h))
         if rc != 0:
             raise RuntimeError("chd_phys_batch_create failed with code %d (no CUDA device? no CPU fallback exists)" % rc)
         self.h = h

@@ -27,6 +27,8 @@ def main(argv=None):
     ap.add_argument("--w_smooth", type=float, default=0.1)
     ap.add_argument("--w_dur", type=float, default=0.1)
     ap.add_argument("--n_ee", type=int, default=4)
+    ap.add_argument("--stage3_long", action="store_true",
+                    help="run stage 3 on sequences with more than 96 phase durations too (switch times as band unknowns)")
     args = ap.parse_args(argv)
     import chd
     in_dirs = args.in_dir.split(",")
@@ -39,6 +41,7 @@ def main(argv=None):
     print("Optim weights (%g, %g, %g, %g)\nDuration cost weight %g" % (args.w_com_lin, args.w_com_ang, args.w_ee, args.w_smooth, args.w_dur))
     problems = [chd.io_formats.read_phys_inputs(d, f, n_ee=args.n_ee) for d, f in zip(in_dirs, nframes)]
     weights = (args.w_com_lin, args.w_com_ang, args.w_ee, args.w_smooth, args.w_dur)
+    band = 96 if args.stage3_long else None
     world, rank, local = int(os.environ.get("WORLD_SIZE", 1)), int(os.environ.get("RANK", 0)), int(os.environ.get("LOCAL_RANK", 0))
     if world > 1:
         # torchrun: one process per GPU, sequences sharded by predicted work, one gather of the final trajectories;
@@ -47,7 +50,8 @@ def main(argv=None):
         import torch.distributed as dist
         torch.cuda.set_device(local)
         dist.init_process_group("nccl", device_id=torch.device("cuda", local))
-        out = chd.parallel.solve_sharded(problems, weights=weights, device=local, rank=rank, world=world)
+        out = chd.parallel.solve_sharded(problems, weights=weights, device=local, rank=rank, world=world,
+                                         stage3_band_above=band)
         dist.destroy_process_group()
         if rank == 0:
             ne_max = max(p.n_ee for p in problems)
@@ -58,7 +62,7 @@ def main(argv=None):
                 chd.io_formats.write_solution(os.path.join(od, "sol_out_durations.txt"), p.dt, out["samples"][i, :nf][:, cols], n_ee)
                 chd.io_formats.write_success_log(os.path.join(od, "success_log.txt"), out["success"][i, 0], out["success"][i, 1])
         return
-    batch = chd.phys.PhysBatch(problems, weights=weights)
+    batch = chd.phys.PhysBatch(problems, weights=weights, stage3_band_above=band)
     out = batch.solve()
     for i, (p, od) in enumerate(zip(problems, out_dirs)):
         chd.phys.write_outputs(out, i, p, od, batch.n_ee_max)
