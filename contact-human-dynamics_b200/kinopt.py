@@ -100,43 +100,84 @@ def make_weights(poses2D, conf, cam_center, focal):
 
 
 class _Model:
-    """Residuals and the block structure of their Jacobian, batched over the frames (torch, fp64)."""
+    """Residuals and the block structure of their Jacobian over the concatenated frames of K >= 1 clips of the same
+    skeleton, batched over the frames (torch, fp64).  Offsets and floor are per clip, and the rows that would couple the
+    last frames of one clip with the next clip (velocity, acceleration, contact velocity, Euler smoothness) are dropped,
+    so H has no block coupling two clips.  `probs`: a list of `Problem`s, or one `Problem` for a single clip.  Cost and
+    normal equations return per-clip costs (numpy, K)."""
 
-    def __init__(self, p: Problem, device=None):
+    def __init__(self, probs, device=None):
         import torch
+        if isinstance(probs, Problem):
+            probs = [probs]
+        if not probs:
+            raise ValueError("no clips")
+        parents = np.asarray(probs[0].parents)
+        if any(not np.array_equal(np.asarray(p.parents), parents) for p in probs):
+            raise ValueError("all clips of a batch must use the same skeleton hierarchy")
+        self.lens = np.array([p.poses3D.shape[0] for p in probs], dtype=np.int64)
+        if (self.lens < 1).any():
+            raise ValueError("every clip needs at least one frame")
+        self.K = len(probs)
+        self.seg = np.concatenate([[0], np.cumsum(self.lens)]).astype(np.int64)
+        self.spans = [(int(a), int(b)) for a, b in zip(self.seg[:-1], self.seg[1:])]
         self.t = torch
         self.dev = torch.device(device) if device is not None else torch.device("cpu")
         f64 = dict(dtype=torch.float64, device=self.dev)
         self.f64 = f64
-        self.p = p
-        self.F = p.poses3D.shape[0]
-        self.parents = [int(v) for v in p.parents]
-        self.off = torch.as_tensor(p.offsets, **f64)
+        self.F = F = int(self.seg[-1])
+        self.parents = [int(v) for v in parents]
         self.back = torch.as_tensor(BACKWARD, device=self.dev)
         self.desc = torch.as_tensor(descendants_mask(self.parents).astype(np.float64), **f64)   # [m, k]: k strict descendant of m
         self.par_idx = torch.as_tensor([max(q, 0) for q in self.parents], device=self.dev)
         self.root_mask = torch.as_tensor([q < 0 for q in self.parents], device=self.dev)
         as_t = lambda a: torch.as_tensor(np.asarray(a, dtype=np.float64), **f64)
-        self.poses3D, self.root_trans, self.j2n = as_t(p.poses3D), as_t(p.root_trans), as_t(p.joints2d)
-        self.pw, self.dw, self.con = as_t(p.proj_w), as_t(p.data_w), as_t(p.contacts)
-        self.n, self.pt = as_t(p.floor_normal), as_t(p.floor_point)
+        cat = lambda a: as_t(np.concatenate([np.asarray(getattr(p, a), np.float64) for p in probs], 0))
+        self.poses3D, self.root_trans, self.j2n = cat("poses3D"), cat("root_trans"), cat("joints2d")
+        self.pw, self.dw, self.con = cat("proj_w"), cat("data_w"), cat("contacts")
         self.sw = as_t(SMOOTH_WEIGHTS)[:, None] * as_t(SMOOTH_VEL)[None, :]            # (28, 3)
         self.is_root = torch.zeros(NJ, **f64)
         self.is_root[ROOT_IDX] = 1.0
+        # each clip's skeleton offsets and floor, and per frame (the clip of every frame)
+        per_clip = lambda a: as_t(np.stack([np.asarray(getattr(p, a), np.float64) for p in probs]))
+        self.off_k, self.n_k, self.pt_k = per_clip("offsets"), per_clip("floor_normal"), per_clip("floor_point")
+        self.clip = torch.as_tensor(np.repeat(np.arange(self.K), self.lens), device=self.dev)
+        self.off, self.n, self.pt = self.off_k[self.clip], self.n_k[self.clip], self.pt_k[self.clip]
+        # rows of a group that couples frames f .. f+k: those whose last frame lies in the clip of f
+        end = np.repeat(self.seg[1:], self.lens)
+        self.keep = {k: torch.as_tensor(np.nonzero(np.arange(max(F - k, 0)) + k < end[:max(F - k, 0)])[0], device=self.dev)
+                     for k in (1, 2)}
+        self.all = torch.arange(F, device=self.dev)
+        # On the CPU the products with a clip's offsets and floor are taken clip by clip, as matrix-vector products: a
+        # per-frame batched product rounds differently in the last bit, and Levenberg-Marquardt amplifies that along
+        # weakly determined directions.  So a clip's result on the CPU does not depend on the other clips of its batch.
+        # On a GPU one batched product serves all clips.
+        self.by_clip = self.dev.type == "cpu"
 
-    # ---- what differs between one clip and several clips on one frame axis (_BatchModel) ----
     def _bone(self, gRq, j):
         """Offset of joint j rotated by its parent's global rotation."""
-        return gRq @ self.off[j]
+        if self.by_clip:
+            return self.t.cat([gRq[a:b] @ self.off_k[k, j] for k, (a, b) in enumerate(self.spans)], 0)
+        return (gRq @ self.off[:, j, :, None])[..., 0]
 
     def _rows(self, span, r, G):
-        """A residual group whose row of base frame f couples frames f .. f+span -> (base frames, r, G); 0 = all from 0."""
-        return 0, r, G
+        """A residual group whose row of base frame f couples frames f .. f+span -> (base frames, r, G) without the rows
+        that would couple two clips."""
+        idx = self.keep[span]
+        return idx, r[idx], ({d: g[idx] for d, g in G.items()} if G is not None else None)
 
     def _floor(self, cf, ab, dab, jac):
-        r = cf * ((ab - self.pt) @ self.n)
-        G = {0: cf[..., None] * self.t.einsum("c,fjcv->fjv", self.n, dab)} if jac else None
+        t = self.t
+        if self.by_clip:
+            r = t.cat([cf[a:b] * ((ab[a:b] - self.pt_k[k]) @ self.n_k[k]) for k, (a, b) in enumerate(self.spans)], 0)
+            G = {0: t.cat([cf[a:b, :, None] * t.einsum("c,fjcv->fjv", self.n_k[k], dab[a:b]) for k, (a, b) in enumerate(self.spans)], 0)} if jac else None
+            return r, G
+        r = cf * t.einsum("fjc,fc->fj", ab - self.pt[:, None, :], self.n)
+        G = {0: cf[..., None] * t.einsum("fc,fjcv->fjv", self.n, dab)} if jac else None
         return r, G
+
+    def _base(self, base, Fp):
+        return self.all[:Fp] if isinstance(base, int) else base
 
     # ---- forward kinematics: y (F, 28, 3) in body-25 order (root entry = root translation, others root-relative) ----
     def points(self, x, jac=False):
@@ -251,209 +292,14 @@ class _Model:
         """The reference's f, same ordering (group by group, frame by frame)."""
         return self.t.cat([r.reshape(-1) for _, r, _ in self.residuals(x, w, jac=False)])
 
-    def cost(self, x, w):
-        return 0.5 * float(sum((r * r).sum() for _, r, _ in self.residuals(x, w, jac=False)))
-
-    def dense_jacobian(self, x, w):
-        """(terms, 87 F) -- tests only (small F)."""
-        t = self.t
-        rows = []
-        for _, r, G in self.residuals(x, w, jac=True):
-            Fp, nr_ = r.shape[0], r.reshape(r.shape[0], -1).shape[1]
-            blk = t.zeros(Fp, nr_, self.F * NV, **self.f64)
-            for d, g in G.items():
-                for f in range(Fp):
-                    blk[f, :, (f + d) * NV:(f + d + 1) * NV] = g[f]
-            rows.append(blk.reshape(-1, self.F * NV))
-        return t.cat(rows, 0)
-
-    # ---- Gauss-Newton system: block-pentadiagonal H (diag, +1, +2 block bands) and gradient ----
-    def normal_equations(self, x, w):
-        t = self.t
-        F = self.F
-        H = [t.zeros(F, NV, NV, **self.f64), t.zeros(max(F - 1, 0), NV, NV, **self.f64), t.zeros(max(F - 2, 0), NV, NV, **self.f64)]
-        g = t.zeros(F, NV, **self.f64)
-        cost = 0.0
-        for _, r, G in self.residuals(x, w, jac=True):
-            Fp = r.shape[0]
-            rr = r.reshape(Fp, -1)
-            cost += 0.5 * float((rr * rr).sum())
-            for d, gd in G.items():
-                g[d:d + Fp] += t.einsum("frv,fr->fv", gd, rr)
-                for e_, ge in G.items():
-                    if e_ < d:
-                        continue
-                    H[e_ - d][d:d + Fp] += gd.transpose(1, 2) @ ge if e_ == d else ge.transpose(1, 2) @ gd   # block (f+e, f+d), lower band
-        return cost, H, g
-
-
-DENSE_MAX_UNKNOWNS = 24000      # 4.6 GB of fp64 at the limit (275 frames)
-
-
-def _banded_cholesky_solve(t, H, g, lam, dense=None):
-    """Solves (H + lam * diag(H)) s = g for the symmetric block-pentadiagonal H = (diag blocks, first and second lower block
-    bands: H[1][f] = block (f+1, f), H[2][f] = block (f+2, f)).  One sweep of block Cholesky, F steps of 87 x 87 work."""
-    D, B1, B2 = H
-    F, n = D.shape[0], D.shape[1]
-    Dd = D + lam * t.diag_embed(t.diagonal(D, dim1=1, dim2=2).clamp_min(1e-12))
-    if dense is None:
-        # on the GPU the sweep below is F dependent steps of a few tiny kernels each (launch bound); one dense fp64
-        # Cholesky of the (87 F)^2 matrix is far faster there as long as it fits comfortably
-        dense = D.is_cuda and F * n <= DENSE_MAX_UNKNOWNS
-    if dense:
-        A = t.zeros(F * n, F * n, dtype=D.dtype, device=D.device)
-        A4 = A.view(F, n, F, n)
-        i0 = t.arange(F, device=D.device)
-        A4[i0, :, i0, :] = Dd
-        if F > 1:
-            A4[i0[1:], :, i0[:-1], :] = B1
-        if F > 2:
-            A4[i0[2:], :, i0[:-2], :] = B2
-        L = t.linalg.cholesky(A)                       # reads the lower triangle only
-        return t.cholesky_solve(g.reshape(-1, 1), L).reshape(F, n)
-    L0, L1, L2 = [None] * F, [None] * F, [None] * F                               # L1[f] = L(f+1, f), L2[f] = L(f+2, f)
-    for f in range(F):
-        A = Dd[f].clone()
-        if f >= 1:
-            A -= L1[f - 1] @ L1[f - 1].T
-        if f >= 2:
-            A -= L2[f - 2] @ L2[f - 2].T
-        L0[f] = t.linalg.cholesky(A)
-        if f + 1 < F:
-            A1 = B1[f].clone()
-            if f >= 1:
-                A1 -= L2[f - 1] @ L1[f - 1].T
-            L1[f] = t.linalg.solve_triangular(L0[f], A1.T, upper=False).T
-        if f + 2 < F:
-            L2[f] = t.linalg.solve_triangular(L0[f], B2[f].T, upper=False).T
-    # forward
-    yv = [None] * F
-    for f in range(F):
-        b = g[f].clone()
-        if f >= 1:
-            b -= L1[f - 1] @ yv[f - 1]
-        if f >= 2:
-            b -= L2[f - 2] @ yv[f - 2]
-        yv[f] = t.linalg.solve_triangular(L0[f], b[:, None], upper=False)[:, 0]
-    # backward
-    s = [None] * F
-    for f in range(F - 1, -1, -1):
-        b = yv[f].clone()
-        if f + 1 < F:
-            b -= L1[f].T @ s[f + 1]
-        if f + 2 < F:
-            b -= L2[f].T @ s[f + 2]
-        s[f] = t.linalg.solve_triangular(L0[f].T, b[:, None], upper=True)[:, 0]
-    return t.stack(s, 0)
-
-
-def levenberg_marquardt(model: _Model, x0, w: StageWeights, max_nfev: int = 50, rtol: float = 1e-10, verbose: bool = False):
-    """Minimises 0.5 |f(x)|^2 from x0 (F, 87).  Returns (x, cost, evaluations)."""
-    t = model.t
-    x = t.as_tensor(np.asarray(x0, dtype=np.float64).reshape(model.F, NV), **model.f64).clone()
-    cost, H, g = model.normal_equations(x, w)
-    nfev, lam = 1, 1e-3
-    while nfev < max_nfev:
-        try:
-            step = -_banded_cholesky_solve(t, H, g, lam)
-        except Exception:                 # not positive definite at this damping
-            lam *= 10.0
-            if lam > 1e12:
-                break
-            continue
-        xn = x + step
-        cn = model.cost(xn, w)
-        nfev += 1
-        # predicted decrease of the damped Gauss-Newton model: 0.5 step^T (lam D step - g)
-        dg = t.stack([t.diagonal(H[0][f]) for f in range(model.F)], 0).clamp_min(1e-12)
-        pred = 0.5 * float((step * (lam * dg * step - g)).sum())
-        rho = (cost - cn) / pred if pred > 0 else -1.0
-        if verbose:
-            print("  nfev %3d  cost %.6e -> %.6e  lam %.1e  rho %.2f" % (nfev, cost, cn, lam, rho))
-        if cn < cost:
-            small = (cost - cn) <= rtol * cost
-            x = xn
-            cost, H, g = model.normal_equations(x, w)
-            lam = max(lam * max(1.0 / 3.0, 1.0 - (2.0 * rho - 1.0) ** 3), 1e-9) if rho > 0 else lam
-            if small:
-                break
-        else:
-            lam *= 4.0
-            if lam > 1e12:
-                break
-    return x, cost, nfev
-
-
-# ---------------------------------------------------------------------------------------------------------------------
-# Several clips at once: one concatenated frame axis, one block-banded solve launch per Levenberg-Marquardt round
-# ---------------------------------------------------------------------------------------------------------------------
-class _BatchModel(_Model):
-    """`_Model` over the concatenated frames of K clips of the same skeleton.  Offsets and floor are per frame (each clip
-    keeps its own), and the rows that would couple the last frames of one clip with the next clip (velocity,
-    acceleration, contact velocity, Euler smoothness) are dropped, so H has no block coupling two clips.  The per-frame
-    arithmetic is the single-clip one; cost and normal equations return per-clip costs (numpy, K)."""
-
-    def __init__(self, probs, device=None):
-        if not probs:
-            raise ValueError("no clips")
-        parents = np.asarray(probs[0].parents)
-        if any(not np.array_equal(np.asarray(p.parents), parents) for p in probs):
-            raise ValueError("all clips of a batch must use the same skeleton hierarchy")
-        self.lens = np.array([p.poses3D.shape[0] for p in probs], dtype=np.int64)
-        if (self.lens < 1).any():
-            raise ValueError("every clip needs at least one frame")
-        self.K = len(probs)
-        self.seg = np.concatenate([[0], np.cumsum(self.lens)]).astype(np.int64)
-        cat = lambda a: np.concatenate([np.asarray(getattr(p, a), np.float64) for p in probs], 0)
-        rep = lambda a: np.repeat(np.stack([np.asarray(getattr(p, a), np.float64) for p in probs]), self.lens, axis=0)
-        super().__init__(Problem(parents, rep("offsets"), cat("poses3D"), cat("root_trans"), cat("joints2d"), cat("proj_w"),
-                                 cat("data_w"), cat("contacts"), rep("floor_normal"), rep("floor_point")), device)
-        t, F = self.t, self.F
-        self.clip = t.as_tensor(np.repeat(np.arange(self.K), self.lens), device=self.dev)      # clip of every frame
-        end = np.repeat(self.seg[1:], self.lens)
-        self.keep = {k: t.as_tensor(np.nonzero(np.arange(max(F - k, 0)) + k < end[:max(F - k, 0)])[0], device=self.dev)
-                     for k in (1, 2)}
-        self.all = t.arange(F, device=self.dev)
-        # On the CPU the products with a clip's offsets and floor are taken clip by clip, as the matrix-vector products of
-        # the single-clip model: a per-frame batched product rounds differently in the last bit, and Levenberg-Marquardt
-        # amplifies that along weakly determined directions.  On a GPU one batched product serves all clips.
-        self.by_clip = self.dev.type == "cpu"
-        as_t = lambda a: t.as_tensor(np.stack([np.asarray(getattr(p, a), np.float64) for p in probs]), **self.f64)
-        self.off_k, self.n_k, self.pt_k = as_t("offsets"), as_t("floor_normal"), as_t("floor_point")
-        self.spans = [(int(a), int(b)) for a, b in zip(self.seg[:-1], self.seg[1:])]
-
-    def _bone(self, gRq, j):
-        if self.by_clip:
-            return self.t.cat([gRq[a:b] @ self.off_k[k, j] for k, (a, b) in enumerate(self.spans)], 0)
-        return (gRq @ self.off[:, j, :, None])[..., 0]
-
-    def _rows(self, span, r, G):
-        idx = self.keep[span]
-        return idx, r[idx], ({d: g[idx] for d, g in G.items()} if G is not None else None)
-
-    def _floor(self, cf, ab, dab, jac):
-        t = self.t
-        if self.by_clip:
-            r = t.cat([cf[a:b] * ((ab[a:b] - self.pt_k[k]) @ self.n_k[k]) for k, (a, b) in enumerate(self.spans)], 0)
-            G = {0: t.cat([cf[a:b, :, None] * t.einsum("c,fjcv->fjv", self.n_k[k], dab[a:b]) for k, (a, b) in enumerate(self.spans)], 0)} if jac else None
-            return r, G
-        r = cf * t.einsum("fjc,fc->fj", ab - self.pt[:, None, :], self.n)
-        G = {0: cf[..., None] * t.einsum("fc,fjcv->fjv", self.n, dab)} if jac else None
-        return r, G
-
-    def _base(self, base, Fp):
-        return self.all[:Fp] if isinstance(base, int) else base
-
     def per_clip(self, v):
         """Segment sums of a per-frame numpy vector."""
         return np.add.reduceat(np.asarray(v, dtype=np.float64), self.seg[:-1])
 
     def _costs(self, groups, each):
-        """0.5 * sum of squares per clip of the residual groups [(base, r)]; `each`: halve every group's sum (as
-        `_Model.normal_equations`) instead of the total (as `_Model.cost`).  By clip: one reduction per clip and group, in
-        the single-clip model's order.  Otherwise per frame on the device (a row counts for its first frame), then
-        per clip on the host."""
-        t = self.t
+        """0.5 * sum of squares per clip of the residual groups [(base, r)]; `each`: halve every group's sum (as the
+        normal equations accumulate it) instead of the total (as `cost`).  By clip: one reduction per clip and group.
+        Otherwise per frame on the device (a row counts for its first frame), then per clip on the host."""
         if self.by_clip:
             c = np.zeros(self.K)
             for base, r in groups:
@@ -505,6 +351,7 @@ class _BatchModel(_Model):
             rows.append(blk.reshape(-1, self.F * NV))
         return t.cat(rows, 0)
 
+    # ---- Gauss-Newton system: block-pentadiagonal H (diag, +1, +2 block bands) and gradient ----
     def normal_equations(self, x, w):
         t = self.t
         F = self.F
@@ -521,15 +368,57 @@ class _BatchModel(_Model):
                 for e_, ge in G.items():
                     if e_ < d:
                         continue
-                    H[e_ - d].index_add_(0, bf + d, gd.transpose(1, 2) @ ge if e_ == d else ge.transpose(1, 2) @ gd)
+                    H[e_ - d].index_add_(0, bf + d, gd.transpose(1, 2) @ ge if e_ == d else ge.transpose(1, 2) @ gd)   # block (f+e, f+d), lower band
         return self._costs(groups, each=True), H, g
 
 
+def _banded_cholesky_solve(t, H, g, lam):
+    """Solves (H + lam * diag(H)) s = g for the symmetric block-pentadiagonal H = (diag blocks, first and second lower block
+    bands: H[1][f] = block (f+1, f), H[2][f] = block (f+2, f)).  One sweep of block Cholesky, F steps of 87 x 87 work."""
+    D, B1, B2 = H
+    F = D.shape[0]
+    Dd = D + lam * t.diag_embed(t.diagonal(D, dim1=1, dim2=2).clamp_min(1e-12))
+    L0, L1, L2 = [None] * F, [None] * F, [None] * F                               # L1[f] = L(f+1, f), L2[f] = L(f+2, f)
+    for f in range(F):
+        A = Dd[f].clone()
+        if f >= 1:
+            A -= L1[f - 1] @ L1[f - 1].T
+        if f >= 2:
+            A -= L2[f - 2] @ L2[f - 2].T
+        L0[f] = t.linalg.cholesky(A)
+        if f + 1 < F:
+            A1 = B1[f].clone()
+            if f >= 1:
+                A1 -= L2[f - 1] @ L1[f - 1].T
+            L1[f] = t.linalg.solve_triangular(L0[f], A1.T, upper=False).T
+        if f + 2 < F:
+            L2[f] = t.linalg.solve_triangular(L0[f], B2[f].T, upper=False).T
+    # forward
+    yv = [None] * F
+    for f in range(F):
+        b = g[f].clone()
+        if f >= 1:
+            b -= L1[f - 1] @ yv[f - 1]
+        if f >= 2:
+            b -= L2[f - 2] @ yv[f - 2]
+        yv[f] = t.linalg.solve_triangular(L0[f], b[:, None], upper=False)[:, 0]
+    # backward
+    s = [None] * F
+    for f in range(F - 1, -1, -1):
+        b = yv[f].clone()
+        if f + 1 < F:
+            b -= L1[f].T @ s[f + 1]
+        if f + 2 < F:
+            b -= L2[f].T @ s[f + 2]
+        s[f] = t.linalg.solve_triangular(L0[f].T, b[:, None], upper=True)[:, 0]
+    return t.stack(s, 0)
+
+
 class _KinSolver:
-    """The damped block-banded solves of all live clips of a `_BatchModel` in one step: one `chd_kin_solve` launch on a
+    """The damped block-banded solves of all live clips of a `_Model` in one step: one `chd_kin_solve` launch on a
     CUDA device (libchd is required there), `_banded_cholesky_solve` per clip segment on the CPU."""
 
-    def __init__(self, model: _BatchModel):
+    def __init__(self, model: _Model):
         t = model.t
         self.m = model
         self.cuda = model.dev.type == "cuda"
@@ -571,10 +460,10 @@ class _KinSolver:
         return self.s, self.status
 
 
-def levenberg_marquardt_batch(model: _BatchModel, x0s, w: StageWeights, max_nfev: int = 50, rtol: float = 1e-10, verbose: bool = False):
-    """`levenberg_marquardt` for every clip of `model` at once, from x0s (one (F_k, 87) array per clip).  Each clip keeps
-    its own state (damping, cost, evaluation count) and follows exactly the single-clip state machine; a round solves all
-    live clips in one step and synchronises the host once for the accept decisions.  Returns (xs, costs, nfevs), lists."""
+def levenberg_marquardt(model: _Model, x0s, w: StageWeights, max_nfev: int = 50, rtol: float = 1e-10, verbose: bool = False):
+    """Minimises 0.5 |f_k(x_k)|^2 for every clip k of `model` from x0s (one (F_k, 87) array per clip).  Each clip keeps its
+    own state (damping, cost, evaluation count); a round solves all live clips in one step and synchronises the host once
+    for the accept decisions.  Returns (xs, costs, nfevs), lists."""
     t = model.t
     K, seg = model.K, model.seg
     x = t.as_tensor(np.concatenate([np.asarray(a, np.float64).reshape(-1, NV) for a in x0s], 0), **model.f64).clone()
@@ -663,68 +552,15 @@ def fit_floor(feet_pos, epsilon: float = 1.5):
 
 def optimize_trajectory(poses2D, joint_conf_2d, poses3D, root_pos, joint_angles, parents, offsets, ppx, ppy, cam_focal, vel_constraints,
                         plane_normal=None, plane_point=None, device=None, ik_iterations: int = 200, max_nfev: int = 50, verbose: bool = False):
-    """Driver with the reference's argument meaning (optimize_trajectory.py:522-834); the skeleton is given as (parents,
-    offsets) of the 28-joint `combined` template.  Returns (anim, newPose3D, projPose2D, plane_normal, plane_point,
-    vel_constraints, info)."""
-    poses2D, poses3D, root_pos = np.asarray(poses2D, np.float64), np.asarray(poses3D, np.float64), np.asarray(root_pos, np.float64)
-    vel = np.asarray(vel_constraints, dtype=np.float64).copy()
-    F, J = poses3D.shape[:2]
-    if poses2D.shape[1] != J:
+    """One clip with the reference's signature (optimize_trajectory.py:522-834), run as a batch of one by
+    `optimize_trajectory_batch`.  Returns (anim, newPose3D, projPose2D, plane_normal, plane_point, vel_constraints, info),
+    or None after the reference's message when the 2D and 3D data have different numbers of joints."""
+    if np.shape(poses2D)[1] != np.shape(poses3D)[1]:
         print("2D and 3D data must have the same number of joints!")
         return None
-    given_floor = plane_normal is not None and plane_point is not None
-    targets = poses3D[:, FORWARD] + root_pos[:, None, :]
-    off = update_skeleton(parents, offsets, targets)
-    j2n, pw, dw = make_weights(poses2D, np.asarray(joint_conf_2d, np.float64), (ppx, ppy), cam_focal)
-    # IK initialisation from the given joint angles (axis-angle; the reference negates the axis), no IK on the spine
-    aa = -np.asarray(joint_angles, np.float64)
-    ang = np.linalg.norm(aa, axis=2)
-    axis = aa / (ang + 1e-10)[..., None]
-    K = np.zeros(aa.shape[:2] + (3, 3))
-    K[..., 0, 1], K[..., 0, 2], K[..., 1, 0], K[..., 1, 2], K[..., 2, 0], K[..., 2, 1] = -axis[..., 2], axis[..., 1], axis[..., 2], -axis[..., 0], -axis[..., 1], axis[..., 0]
-    R0 = np.eye(3) + np.sin(ang)[..., None, None] * K + (1.0 - np.cos(ang))[..., None, None] * (K @ K)
-    P0 = np.tile(off[None], (F, 1, 1))
-    P0[:, 0] = root_pos
-    names = ["joint_%d" % i for i in range(J)]
-    anim = SkelAnim(names, np.asarray(parents), off, R0, P0)
-    tm = {j: targets[:, j] for j in range(J) if j not in SPINE_IDX}
-    anim = ik_solve(anim, tm, iterations=ik_iterations, smoothness=0.0, damping=7.0, translate=False, device=device)
-    from .prepare import euler_zyx_from_matrix
-    x = np.concatenate([anim.positions[:, 0], euler_zyx_from_matrix(anim.rotations).reshape(F, -1)], axis=1)
-    zero = np.zeros(3)
-    prob = Problem(np.asarray(parents), off, poses3D, root_pos, j2n, pw, dw, vel, zero if not given_floor else np.asarray(plane_normal, np.float64),
-                   zero if not given_floor else np.asarray(plane_point, np.float64))
-    info = {}
-    # stage 1: no floor term
-    m = _Model(prob, device)
-    xs, c1, n1 = levenberg_marquardt(m, x, StageWeights(floor=0.0), max_nfev, verbose=verbose)
-    info["stage1"] = dict(cost=c1, nfev=n1)
-    x = xs.cpu().numpy()
-    # floor fit on the contact feet, contact pruning
-    gp = _global_positions(parents, off, x)
-    feet_lab = np.array([FORWARD[k] for k in FEET_IDX])
-    sel = vel[:, feet_lab] == 1
-    feet_pos = gp[:, FEET_IDX][sel]
-    if not given_floor:
-        plane_normal, plane_point, _ = fit_floor(feet_pos, 1.5)
-        _, _, _, outl = huber_fit(feet_pos[:, [0, 2]], feet_pos[:, 1], 2.2)
-        fv = vel[:, feet_lab]
-        fv[sel] = np.where(outl, 0.0, 1.0)          # row-major order of the selection = the reference's frame / foot loop
-        vel[:, feet_lab] = fv
-    # stage 2: feet on the floor
-    prob.contacts, prob.floor_normal, prob.floor_point = vel, np.asarray(plane_normal, np.float64), np.asarray(plane_point, np.float64)
-    m = _Model(prob, device)
-    xs, c2, n2 = levenberg_marquardt(m, x, StageWeights(floor=10.0), max_nfev, verbose=verbose)
-    info["stage2"] = dict(cost=c2, nfev=n2)
-    x = xs.cpu().numpy()
-    info["x"] = x
-    gp = _global_positions(parents, off, x)
-    new3d = gp[:, BACKWARD]
-    proj = np.stack([cam_focal[0] * new3d[..., 0] / new3d[..., 2] + ppx, cam_focal[1] * new3d[..., 1] / new3d[..., 2] + ppy], -1)
-    Pl = np.tile(off[None], (F, 1, 1))
-    Pl[:, 0] = x[:, :3]
-    anim = SkelAnim(names, np.asarray(parents), off, rot_zyx(x[:, 3:].reshape(F, J, 3)), Pl)
-    return anim, new3d, proj, np.asarray(plane_normal), np.asarray(plane_point), vel, info
+    return optimize_trajectory_batch([poses2D], [joint_conf_2d], [poses3D], [root_pos], [joint_angles], [parents], [offsets], [ppx], [ppy],
+                                     [cam_focal], [vel_constraints], plane_normal=[plane_normal], plane_point=[plane_point], device=device,
+                                     ik_iterations=ik_iterations, max_nfev=max_nfev, verbose=verbose)[0]
 
 
 def _global_positions(parents, off, x):
@@ -737,10 +573,12 @@ def _global_positions(parents, off, x):
 
 def optimize_trajectory_batch(poses2D, joint_conf_2d, poses3D, root_pos, joint_angles, parents, offsets, ppx, ppy, cam_focal, vel_constraints,
                               plane_normal=None, plane_point=None, device=None, ik_iterations: int = 200, max_nfev: int = 50, verbose: bool = False):
-    """`optimize_trajectory` for K clips at once: every per-clip argument is a list with one entry per clip (plane_normal /
-    plane_point: None, or a list whose None entries mean "fit the floor" for that clip).  The IK initialisation is one
-    call over all frames, each Levenberg-Marquardt stage runs all clips together (`levenberg_marquardt_batch`); the
-    skeleton fit, the floor fit and the contact pruning stay per clip.  Returns the list of `optimize_trajectory`'s tuples."""
+    """Driver with the reference's argument meaning (optimize_trajectory.py:522-834) for K clips at once; the skeleton is
+    given as (parents, offsets) of the 28-joint `combined` template.  Every per-clip argument is a list with one entry per
+    clip (plane_normal / plane_point: None, or a list whose None entries mean "fit the floor" for that clip).  The IK
+    initialisation is one call over all frames, each Levenberg-Marquardt stage runs all clips together; the skeleton fit,
+    the floor fit and the contact pruning stay per clip.  Returns one (anim, newPose3D, projPose2D, plane_normal,
+    plane_point, vel_constraints, info) per clip."""
     from .prepare import euler_zyx_from_matrix
     K = len(poses3D)
     pn_in = plane_normal if plane_normal is not None else [None] * K
@@ -759,7 +597,8 @@ def optimize_trajectory_batch(poses2D, joint_conf_2d, poses3D, root_pos, joint_a
                           vel=np.asarray(vel_constraints[k], dtype=np.float64).copy(), parents=np.asarray(parents[k]),
                           pn=np.asarray(pn_in[k], np.float64) if given else None, pp=np.asarray(pp_in[k], np.float64) if given else None))
     J = clips[0]["p3"].shape[1]
-    # IK initialisation of every frame of every clip in one call (smoothness 0: the frames are independent)
+    # IK initialisation from the given joint angles (axis-angle; the reference negates the axis), no IK on the spine; every
+    # frame of every clip in one call (smoothness 0: the frames are independent)
     R0, P0 = [], []
     for k, c in enumerate(clips):
         aa = -np.asarray(joint_angles[k], np.float64)
@@ -782,7 +621,7 @@ def optimize_trajectory_batch(poses2D, joint_conf_2d, poses3D, root_pos, joint_a
     probs = [Problem(c["parents"], c["off"], c["p3"], c["rp"], c["j2n"], c["pw"], c["dw"], c["vel"], c["pn"] if c["given"] else zero,
                      c["pp"] if c["given"] else zero) for c in clips]
     # stage 1: no floor term
-    out1, c1, n1 = levenberg_marquardt_batch(_BatchModel(probs, device), xs, StageWeights(floor=0.0), max_nfev, verbose=verbose)
+    out1, c1, n1 = levenberg_marquardt(_Model(probs, device), xs, StageWeights(floor=0.0), max_nfev, verbose=verbose)
     xs = [v.cpu().numpy() for v in out1]
     # floor fit on the contact feet, contact pruning (per clip)
     feet_lab = np.array([FORWARD[k] for k in FEET_IDX])
@@ -795,11 +634,11 @@ def optimize_trajectory_batch(poses2D, joint_conf_2d, poses3D, root_pos, joint_a
             c["pn"], c["pp"], _ = fit_floor(feet_pos, 1.5)
             _, _, _, outl = huber_fit(feet_pos[:, [0, 2]], feet_pos[:, 1], 2.2)
             fv = vel[:, feet_lab]
-            fv[sel] = np.where(outl, 0.0, 1.0)
+            fv[sel] = np.where(outl, 0.0, 1.0)          # row-major order of the selection = the reference's frame / foot loop
             vel[:, feet_lab] = fv
         probs[k].contacts, probs[k].floor_normal, probs[k].floor_point = vel, np.asarray(c["pn"], np.float64), np.asarray(c["pp"], np.float64)
     # stage 2: feet on the floor
-    out2, c2, n2 = levenberg_marquardt_batch(_BatchModel(probs, device), xs, StageWeights(floor=10.0), max_nfev, verbose=verbose)
+    out2, c2, n2 = levenberg_marquardt(_Model(probs, device), xs, StageWeights(floor=10.0), max_nfev, verbose=verbose)
     res = []
     for k, c in enumerate(clips):
         x = out2[k].cpu().numpy()
@@ -874,53 +713,15 @@ def optimize_2d_3d(input_path: str, skel_path: str, output_path: str, min_idx: i
                    device=None, frametime: float = 1.0 / 24.0):
     """kinematic_optimizer.optimize_2d_3d: reads `<dir>/openpose_result/*.json`, `<dir>/tracked_results.json`,
     `<dir>/foot_contacts.npy` next to `input_path`; writes `foot_contacts.npy` (refined, int), `floor_out.txt` and
-    `final_test.bvh` into `output_path`."""
-    import os
-    from . import contact
-    from .prepare import load_bvh
-    from .results import save_bvh
-    os.makedirs(output_path, exist_ok=True)
-    d = os.path.dirname(input_path)
-    op_dir, tc_path, fc_path = os.path.join(d, "openpose_result"), os.path.join(d, "tracked_results.json"), os.path.join(d, "foot_contacts.npy")
-    if not os.path.isdir(op_dir):
-        print("Could not find openpose results in " + op_dir + "!")
-        return None
-    if not os.path.isfile(tc_path):
-        print("Could not find total capture results!")
-        return None
-    if not os.path.isfile(fc_path):
-        print("Could not find foot contact labels!")
-        return None
-    kp = contact.load_keypoint_dir(op_dir)
-    poses3D, root_pos, ang = combined_inputs(load_totalcap_results(tc_path))
-    sl = slice(min_idx, max_idx)
-    n = len(range(*sl.indices(kp.shape[0])))
-    poses2D = np.concatenate([kp[sl, :, :2], np.zeros((n, 3, 2))], axis=1)
-    conf = np.concatenate([kp[sl, :, 2], np.zeros((n, 3))], axis=1)
-    fc = np.load(fc_path)
-    vel = contacts_to_constraints(fc[sl])
-    normal = point = None
-    if use_gt_floor:
-        with open(os.path.join(d, "floor_gt.txt")) as f:
-            normal = np.array([float(v) for v in f.readline().split()])
-            point = np.array([float(v) for v in f.readline().split()]) * 100.0
-    b = load_bvh(skel_path)
-    res = optimize_trajectory(poses2D, conf, poses3D[sl], root_pos[sl], ang[sl], b.parents, b.offsets, MTC_SIZE[0] / 2, MTC_SIZE[1] / 2,
-                              np.array(MTC_FOCAL), vel, plane_normal=normal, plane_point=point, device=device)
-    anim, new3d, proj, pn, pp, newvel, info = res
-    anim.names = list(b.names)
-    np.save(os.path.join(output_path, "foot_contacts"), constraints_to_contacts(newvel))
-    with open(os.path.join(output_path, "floor_out.txt"), "w") as f:
-        f.write("%s %s %s\n%s %s %s" % tuple(str(float(v)) for v in list(pn) + list(pp)))
-    save_bvh(os.path.join(output_path, "final_test.bvh"), anim, b.names, frametime)
-    print("Finished kinematic optimization!")
-    return res
+    `final_test.bvh` into `output_path`.  Returns `optimize_trajectory`'s tuple, or None after a message naming the missing
+    input; a batch of one of `optimize_2d_3d_batch`."""
+    return optimize_2d_3d_batch([(input_path, skel_path, output_path, min_idx, max_idx, use_gt_floor)], device, frametime)[0]
 
 
 def optimize_2d_3d_batch(jobs, device=None, frametime: float = 1.0 / 24.0):
     """`optimize_2d_3d` for several videos with one `optimize_trajectory_batch` call.  `jobs`: list of (input_path,
     skel_path, output_path, min_idx, max_idx, use_gt_floor); every video gets the three files `optimize_2d_3d` writes.
-    Returns one result per job (None for a video whose inputs are missing, as `optimize_2d_3d`)."""
+    Returns one result per job (None for a video whose inputs are missing, after a message naming the missing input)."""
     import os
     from . import contact
     from .prepare import load_bvh

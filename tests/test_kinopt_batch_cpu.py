@@ -92,7 +92,7 @@ def test_no_row_couples_two_clips(chd, clips):
     probs[1].proj_w, probs[1].data_w, probs[1].contacts = probs[1].proj_w[:4], probs[1].data_w[:4], probs[1].contacts[:4]
     xs = [xs[0][:5], xs[1][:4]]
     w = ko.StageWeights(floor=10.0)
-    bm = ko._BatchModel(probs, None)
+    bm = ko._Model(probs, None)
     Jb = bm.dense_jacobian(torch.as_tensor(np.concatenate(xs)), w).numpy()
     Js = [ko._Model(p).dense_jacobian(torch.as_tensor(x), w).numpy() for p, x in zip(probs, xs)]
     assert Jb.shape == (sum(J.shape[0] for J in Js), sum(J.shape[1] for J in Js))

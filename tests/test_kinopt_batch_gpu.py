@@ -94,7 +94,7 @@ def test_kin_solve_mixed_batch_matches_references(chd, systems):
     assert (st == 0).all(), st
     for (H, g), lam, s in zip(systems, LAMS, sols):
         F = g.shape[0]
-        ref = ko._banded_cholesky_solve(torch, H, g, lam, dense=False)
+        ref = ko._banded_cholesky_solve(torch, H, g, lam)
         np.testing.assert_allclose(s.numpy(), ref.numpy(), rtol=1e-8, atol=1e-10)
         Dd = damped(H, lam)
         if F <= 120:
@@ -152,11 +152,10 @@ def test_optimize_2d_3d_batch_on_gpu_matches_cpu(chd, tmp_path):
     assert torch.cuda.is_available()
     ko = chd.kinopt
     jobs = []
-    for F, seed in ((24, 31), (40, 32), (290, 33)):       # 290 frames: past the dense path's size limit
+    for F, seed in ((24, 31), (40, 32), (290, 33)):
         vd = str(tmp_path / ("v%d" % F))
         chd.synth.write_mocap_clip(vd, F, seed=seed)
         jobs.append((os.path.join(vd, "w.mp4"), os.path.join(vd, "skeleton.bvh"), str(tmp_path / ("g%d" % F)), 0, F, False))
-    assert 290 * ko.NV > ko.DENSE_MAX_UNKNOWNS
     gpu = ko.optimize_2d_3d_batch(jobs, device="cuda:0")
     for job, rg in zip(jobs, gpu):
         rc = ko.optimize_2d_3d(job[0], job[1], job[2] + "_cpu", job[3], job[4], job[5])
