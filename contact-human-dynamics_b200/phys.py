@@ -54,7 +54,8 @@ EXPORTS = ["chd_version", "chd_phys_batch_create", "chd_phys_batch_create_ex", "
            "chd_phys_get_x", "chd_phys_set_x", "chd_phys_eval", "chd_phys_get_layout", "chd_phys_solve_stage",
            "chd_phys_solve", "chd_phys_sample", "chd_phys_sample_device", "chd_phys_launch_count",
            "chd_phys_kernel_times", "chd_phys_set_timing", "chd_phys_h2d_bytes", "chd_phys_reset", "chd_measure_fp64_peak", "chd_phys_get_slot_index", "chd_phys_get_ent_col",
-           "chd_phys_get_duals", "chd_phys_stage_stats", "chd_phys_get_sizes_fixed", "chd_kin_solve", "chd_kin_work_bytes"]
+           "chd_phys_get_duals", "chd_phys_stage_stats", "chd_phys_get_sizes_fixed", "chd_kin_solve", "chd_kin_work_bytes",
+           "chd_ik_solve", "chd_ik_work_bytes"]
 
 
 def measure_fp64_peak():
@@ -112,6 +113,10 @@ def load_lib():
         L.chd_kin_solve.argtypes = [vp] * 7 + [C.c_int32] * 3 + [vp] * 4
         L.chd_kin_work_bytes.argtypes = [C.c_int32]
         L.chd_kin_work_bytes.restype = C.c_int64
+        i32 = C.c_int32
+        L.chd_ik_solve.argtypes = [i32, vp, i32, vp, vp, i32, i32, vp, vp, vp, i32, C.c_double, C.c_double, i32, vp, vp]
+        L.chd_ik_work_bytes.argtypes = [i32] * 3
+        L.chd_ik_work_bytes.restype = C.c_int64
         _LIB = L
     return _LIB
 

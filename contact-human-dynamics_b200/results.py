@@ -15,6 +15,9 @@ device is given:
   over all frames;
 * the smoothing term couples a frame only to the previous iterate of its two neighbours, so the frames stay independent
   inside an iteration.
+Many clips of one skeleton at once (`ik_solve_batch`, `apply_results_batch`, `retarget_batch`): one `chd_ik_solve` call
+(csrc/chd_ik.cu, one CTA per frame, the Jacobian never formed) on a CUDA device, the single-clip functions per clip on
+the host.
 
 Pinned to the reference's own functions by tests/golden/make_towr_golden.py (tests/test_results_cpu.py).
 """
@@ -211,11 +214,77 @@ def ik_solve(anim: SkelAnim, targets: Dict[int, np.ndarray], iterations: int = 3
     return SkelAnim(anim.names, anim.parents, anim.offsets, Rl.cpu().numpy(), Pl.cpu().numpy())
 
 
-def apply_results(res: TowrResults, anim_bvh: str, start_idx, end_idx, info: CharacterInfo, run_ik: bool = True, device=None,
-                  iterations: int = 30):
-    """towr_utils.apply_results: returns (anim, names, anim_og, com_og).  The root follows the optimised COM (keeping every
-    upper-body joint's offset from the COM) and base orientation; with `run_ik` the upper-body joints, toes and (4-foot
-    results) heels are IK targets."""
+IK_MAX_JOINTS = 128     # limits of the chd_ik_solve kernel (include/chd.h)
+IK_MAX_TARGETS = 64
+
+
+def _check_ik_batch(anims: Sequence[SkelAnim], targets: Sequence[Dict[int, np.ndarray]]) -> List[int]:
+    """Raises ValueError unless the clips can go through one chd_ik_solve call; returns the target joints in order."""
+    if len(anims) != len(targets):
+        raise ValueError("ik_solve_batch: %d anims but %d target dicts" % (len(anims), len(targets)))
+    parents = np.asarray(anims[0].parents)
+    tj = [int(k) for k in targets[0].keys()]
+    J, T = len(parents), len(tj)
+    for a, tg in zip(anims, targets):
+        if not np.array_equal(np.asarray(a.parents), parents):
+            raise ValueError("ik_solve_batch: every anim must have the same parents")
+        if set(int(k) for k in tg.keys()) != set(tj):
+            raise ValueError("ik_solve_batch: every targets dict must have the same keys")
+        F = a.rotations.shape[0]
+        if a.rotations.shape != (F, J, 3, 3) or a.positions.shape != (F, J, 3) or any(np.shape(v) != (F, 3) for v in tg.values()):
+            raise ValueError("ik_solve_batch: rotations (F, J, 3, 3), positions (F, J, 3) and targets (F, 3) must agree")
+    if J < 1 or J > IK_MAX_JOINTS:
+        raise ValueError("ik_solve_batch: %d joints, the kernel takes 1 .. %d" % (J, IK_MAX_JOINTS))
+    if T < 1 or T > IK_MAX_TARGETS:
+        raise ValueError("ik_solve_batch: %d targets, the kernel takes 1 .. %d" % (T, IK_MAX_TARGETS))
+    if parents[0] != -1 or any(not (-1 <= parents[j] < j) for j in range(1, J)):
+        raise ValueError("ik_solve_batch: parents must be ordered (parents[0] = -1, parents[j] < j)")
+    if any(not (0 <= t < J) for t in tj):
+        raise ValueError("ik_solve_batch: a target joint is out of range")
+    return tj
+
+
+def ik_solve_batch(anims: Sequence[SkelAnim], targets: Sequence[Dict[int, np.ndarray]], iterations: int = 30, damping: float = 7.0,
+                   smoothness: float = 0.001, device=None, translate: bool = True) -> List[SkelAnim]:
+    """`ik_solve` for many clips of one skeleton (same `parents`, same target joints): on a CUDA device one upload, one
+    `chd_ik_solve` call (every frame of every clip, each clip smoothed on its own) and one download; on the host
+    `ik_solve` per clip, bitwise.  Raises ValueError for clips that differ in skeleton or target joints and for more
+    joints / targets than the kernel takes, before any device work."""
+    anims, targets = list(anims), list(targets)
+    if not anims and not targets:
+        return []
+    tj = _check_ik_batch(anims, targets)
+    import torch
+    dev = torch.device(device) if device is not None else torch.device("cpu")
+    if dev.type != "cuda":
+        return [ik_solve(a, tg, iterations=iterations, damping=damping, smoothness=smoothness, device=device, translate=translate)
+                for a, tg in zip(anims, targets)]
+    from .phys import _ptr, load_lib
+    L = load_lib()
+    parents = np.ascontiguousarray(anims[0].parents, dtype=np.int32)
+    tjn = np.asarray(tj, dtype=np.int32)
+    J, T, K = len(parents), len(tj), len(anims)
+    seg = np.zeros(K + 1, dtype=np.int32)
+    seg[1:] = np.cumsum([a.rotations.shape[0] for a in anims])
+    Ft = int(seg[-1])
+    nR, nP = Ft * J * 9, Ft * J * 3
+    host = np.concatenate([np.concatenate([a.rotations for a in anims]).reshape(-1), np.concatenate([a.positions for a in anims]).reshape(-1),
+                           np.concatenate([np.stack([np.asarray(tg[k], dtype=np.float64) for k in tj], axis=1) for tg in targets]).reshape(-1)])
+    buf = torch.as_tensor(host, dtype=torch.float64).to(dev)
+    work = torch.empty(max(L.chd_ik_work_bytes(Ft, J, T) // 8, 1), dtype=torch.float64, device=dev)
+    base = buf.data_ptr()
+    with torch.cuda.device(dev):
+        rc = L.chd_ik_solve(J, _ptr(parents), T, _ptr(tjn), _ptr(seg), K, Ft, base, base + 8 * nR, base + 8 * (nR + nP), int(iterations),
+                            float(damping), float(smoothness), int(bool(translate)), work.data_ptr(), torch.cuda.current_stream(dev).cuda_stream)
+    if rc != 0:
+        raise RuntimeError("chd_ik_solve failed with code %d" % rc)
+    out = buf[:nR + nP].cpu().numpy()
+    R, P = out[:nR].reshape(Ft, J, 3, 3), out[nR:].reshape(Ft, J, 3)
+    return [SkelAnim(a.names, a.parents, a.offsets, R[seg[k]:seg[k + 1]].copy(), P[seg[k]:seg[k + 1]].copy()) for k, a in enumerate(anims)]
+
+
+def _apply_setup(res: TowrResults, anim_bvh: str, start_idx, end_idx, info: CharacterInfo, run_ik: bool, device):
+    """apply_results up to the IK: (anim with the optimised root, anim_og, com, IK targets or None)."""
     b = load_bvh(anim_bvh)
     start_idx = 0 if start_idx is None else start_idx
     end_idx = b.n_frames if end_idx is None else end_idx
@@ -234,6 +303,7 @@ def apply_results(res: TowrResults, anim_bvh: str, start_idx, end_idx, info: Cha
     desired = upper_off + res.base_pos[:seq_len, None, :] * 100.0
     anim.rotations[:, 0] = rot_zyx(res.base_rot)[:seq_len]
     anim.positions[:, 0] = desired[:, 0]
+    targets = None
     if run_ik:
         targets = {upper[i]: desired[:, i] for i in range(len(upper))}
         targets[info.toes[0]] = res.feet_pos[:seq_len, 0] * 100.0
@@ -242,8 +312,36 @@ def apply_results(res: TowrResults, anim_bvh: str, start_idx, end_idx, info: Cha
             lh, rh = info.heel_inds if info.heel_inds is not None else (anim.positions.shape[1] - 2, anim.positions.shape[1] - 1)
             targets[lh] = res.feet_pos[:seq_len, 2] * 100.0
             targets[rh] = res.feet_pos[:seq_len, 3] * 100.0
+    return anim, anim_og, com, targets
+
+
+def apply_results(res: TowrResults, anim_bvh: str, start_idx, end_idx, info: CharacterInfo, run_ik: bool = True, device=None,
+                  iterations: int = 30):
+    """towr_utils.apply_results: returns (anim, names, anim_og, com_og).  The root follows the optimised COM (keeping every
+    upper-body joint's offset from the COM) and base orientation; with `run_ik` the upper-body joints, toes and (4-foot
+    results) heels are IK targets."""
+    anim, anim_og, com, targets = _apply_setup(res, anim_bvh, start_idx, end_idx, info, run_ik, device)
+    if run_ik:
         anim = ik_solve(anim, targets, iterations=iterations, smoothness=0.001, damping=7.0, device=device)
     return anim, anim.names, anim_og, com
+
+
+def apply_results_batch(jobs, info: CharacterInfo, run_ik: bool = True, device=None, iterations: int = 30):
+    """apply_results for every job (TowrResults, anim_bvh, start_idx, end_idx); returns one (anim, names, anim_og, com)
+    per job.  Jobs with the same skeleton and target joints (e.g. all 2-foot or all 4-foot results of one character)
+    share one `ik_solve_batch` call."""
+    setups = [_apply_setup(res, anim_bvh, s, e, info, run_ik, device) for res, anim_bvh, s, e in jobs]
+    anims = [s[0] for s in setups]
+    if run_ik:
+        groups: Dict[tuple, List[int]] = {}
+        for i, (anim, _, _, targets) in enumerate(setups):
+            groups.setdefault((tuple(int(p) for p in anim.parents), tuple(targets)), []).append(i)
+        for idx in groups.values():
+            solved = ik_solve_batch([anims[i] for i in idx], [setups[i][3] for i in idx], iterations=iterations, smoothness=0.001,
+                                    damping=7.0, device=device)
+            for i, a in zip(idx, solved):
+                anims[i] = a
+    return [(a, a.names, s[1], s[2]) for a, s in zip(anims, setups)]
 
 
 def save_bvh(path: str, anim: SkelAnim, names: Optional[Sequence[str]] = None, frametime: float = 1.0 / 24.0):
@@ -276,6 +374,27 @@ def retarget(src_bvh: str, skel_bvh: str, info: CharacterInfo, out_bvh: Optional
     soft minimum of the foot heights), initialises the character's angles from the mapped source Euler angles, runs the
     damped least-squares IK (translating joints, 200 iterations, damping 7) towards the mapped joints, restores the bone
     offsets and corrects the root height by the median ankle difference.  Returns the SkelAnim (and saves it if asked)."""
+    sk, skel_height = _retarget_skeleton(skel_bvh, info)
+    anim, tm, targets, src_floor = _retarget_setup(src_bvh, sk, skel_height, info)
+    anim = ik_solve(anim, tm, iterations=iterations, smoothness=0.0, damping=7.0, translate=True, device=device)
+    return _retarget_finish(anim, sk, targets, src_floor, info, out_bvh)
+
+
+def retarget_batch(src_bvhs: Sequence[str], skel_bvh: str, info: CharacterInfo, out_bvhs: Optional[Sequence[Optional[str]]] = None,
+                   device=None, iterations: int = 200) -> List[SkelAnim]:
+    """retarget for every source clip onto one character skeleton, the IK of all clips in one `ik_solve_batch` call."""
+    if out_bvhs is not None and len(out_bvhs) != len(src_bvhs):
+        raise ValueError("retarget_batch: %d sources but %d outputs" % (len(src_bvhs), len(out_bvhs)))
+    sk, skel_height = _retarget_skeleton(skel_bvh, info)
+    setups = [_retarget_setup(s, sk, skel_height, info) for s in src_bvhs]
+    anims = ik_solve_batch([s[0] for s in setups], [s[1] for s in setups], iterations=iterations, smoothness=0.0, damping=7.0,
+                           translate=True, device=device)
+    return [_retarget_finish(a, sk, s[2], s[3], info, out_bvhs[i] if out_bvhs is not None else None)
+            for i, (a, s) in enumerate(zip(anims, setups))]
+
+
+def _retarget_skeleton(skel_bvh: str, info: CharacterInfo):
+    """The character skeleton and its height from the hips to the lowest foot joint, rotations zeroed."""
     sk = load_bvh(skel_bvh)
     J = len(sk.names)
     Rk, Tk = local_transforms(sk)
@@ -284,6 +403,12 @@ def retarget(src_bvh: str, skel_bvh: str, info: CharacterInfo, out_bvh: Optional
     fh = np.minimum(skel_targets[:, foot[:2], 1], skel_targets[:, foot[2:], 1]).min(axis=1)
     skel_targets[:, :, 1] -= _softmin(fh)
     skel_height = np.abs(np.amax(skel_targets[:, 0, 1]) - np.amin(skel_targets[:, foot, 1], axis=1)).max()
+    return sk, skel_height
+
+
+def _retarget_setup(src_bvh: str, sk: Bvh, skel_height, info: CharacterInfo):
+    """retarget up to the IK: (initial anim, IK targets, scaled source joint positions, source floor height)."""
+    J = len(sk.names)
     src = load_bvh(src_bvh)
     Rs, Ts = local_transforms(src)
     at = forward_kinematics(src.parents, Rs, Ts)[0]
@@ -307,7 +432,11 @@ def retarget(src_bvh: str, skel_bvh: str, info: CharacterInfo, out_bvh: Optional
     P0 = np.tile(sk.offsets[None], (F, 1, 1))
     P0[:, 0] = targets[:, 0]
     anim = SkelAnim(list(sk.names), sk.parents.copy(), sk.offsets.copy(), rot_zyx(ref), P0)
-    anim = ik_solve(anim, tm, iterations=iterations, smoothness=0.0, damping=7.0, translate=True, device=device)
+    return anim, tm, targets, src_floor
+
+
+def _retarget_finish(anim: SkelAnim, sk: Bvh, targets, src_floor, info: CharacterInfo, out_bvh: Optional[str]) -> SkelAnim:
+    """retarget after the IK: bone offsets restored, root height corrected, saved if asked."""
     anim.positions[:, 1:] = sk.offsets[None, 1:]
     ank = targets[:, COMBINED_ANKLE_INDS, 1] - anim.global_positions()[:, info.ankles, 1]
     anim.positions[:, 0, 1] += np.median(ank)

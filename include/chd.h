@@ -229,6 +229,25 @@ int chd_kin_solve(const double* D, const double* B1, const double* B2, const dou
 /* Bytes of `work` chd_kin_solve needs for F_total frames (three padded 88 x 88 fp64 blocks per frame); -1 if F_total < 0. */
 int64_t chd_kin_work_bytes(int32_t F_total);
 
+/* ---------------------------------------------------------------------------------------------------------
+ * Full-body IK: JacobianInverseKinematicsCK (InverseKinematics.py:326-540; unit weights, gamma 1, no angle limits) for
+ * K clips of one skeleton, `iterations` damped least-squares steps with damping lambda = damping / 1.001 and the
+ * smoothing term smoothness * (x_{f-1} + x_{f+1} - 2 x_f) (a clip's first / last frame stands in for its missing
+ * neighbour); x = [Euler angles; local translations] with `translate`, the Euler angles alone otherwise.
+ * parents [host] J, parents[0] = -1, -1 <= parents[j] < j;  targets [host] T joint indices;
+ * seg [host] K+1 frame offsets (0 .. F_total, non-decreasing): clip k owns frames seg[k] .. seg[k+1]-1;
+ * R [device] F_total x J x 3 x 3 and P [device] F_total x J x 3 local rotations / translations, updated in place;
+ * goal [device] F_total x T x 3 world positions of the targets;  work [device] chd_ik_work_bytes(F_total, J, T) bytes.
+ * Returns 0, -1 bad argument (J outside 1..128, T outside 1..64, parents not ordered, a target out of range, bad seg;
+ * nothing is launched), <= -100 CUDA error.  Asynchronous on `stream`, except that the upload of the ancestor tables
+ * from pageable host memory may wait for earlier work on the stream.  Each clip's result is bitwise independent of the
+ * rest of the batch. */
+int chd_ik_solve(int32_t J, const int32_t* parents, int32_t T, const int32_t* targets, const int32_t* seg, int32_t K,
+                 int32_t F_total, double* R, double* P, const double* goal, int32_t iterations, double damping,
+                 double smoothness, int32_t translate, double* work, void* stream);
+/* Bytes of `work` chd_ik_solve needs (ancestor tables and two copies of the state); -1 outside the limits above. */
+int64_t chd_ik_work_bytes(int32_t F_total, int32_t J, int32_t T);
+
 const char* chd_version(void);
 
 /* Measurement helper (no reference counterpart): sustained fp64 throughput of the current device in GFLOP/s, for the
