@@ -28,7 +28,7 @@ from typing import Optional
 
 import numpy as np
 
-from .results import SkelAnim, descendants_mask, ik_solve, rot_zyx
+from .results import SkelAnim, descendants_mask, ik_solve_batch, rot_zyx
 
 # ---- the `combined` skeleton <-> BODY_25(+3 spine) correspondence and per-joint weights (SkeletonDefinitions.py:62-140) ----
 ROOT_IDX = 8                                    # MidHip in body-25 order
@@ -613,7 +613,7 @@ def optimize_trajectory_batch(poses2D, joint_conf_2d, poses3D, root_pos, joint_a
     names = ["joint_%d" % i for i in range(J)]
     anim = SkelAnim(names, clips[0]["parents"], clips[0]["off"], np.concatenate(R0), np.concatenate(P0))
     tm = {j: np.concatenate([c["targets"][:, j] for c in clips]) for j in range(J) if j not in SPINE_IDX}
-    anim = ik_solve(anim, tm, iterations=ik_iterations, smoothness=0.0, damping=7.0, translate=False, device=device)
+    anim = ik_solve_batch([anim], [tm], iterations=ik_iterations, smoothness=0.0, damping=7.0, translate=False, device=device)[0]
     xall = np.concatenate([anim.positions[:, 0], euler_zyx_from_matrix(anim.rotations).reshape(anim.rotations.shape[0], -1)], axis=1)
     seg = np.concatenate([[0], np.cumsum([c["F"] for c in clips])])
     xs = [xall[seg[k]:seg[k + 1]] for k in range(K)]

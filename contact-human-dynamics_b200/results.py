@@ -6,8 +6,10 @@ Reference: `src/utils/towr_utils.py:51-122` (load_results), `:779-857` (apply_re
 (`src/skeleton_fitting/ik/InverseKinematics.py:326-565`, JacobianInverseKinematicsCK with translate=True, 30 iterations,
 damping 7, smoothness 0.001) and `BVH.save` (`src/skeleton_fitting/ik/BVH.py:174-291`).
 
-Own formulation (rotation matrices, no quaternion library), batched over the frames with torch -- on the GPU when a
-device is given:
+Own formulation (rotation matrices, no quaternion library).  Every IK goes through `ik_solve_batch` (many clips of one
+skeleton; a single clip is a batch of one): on a CUDA device one `chd_ik_solve` call (csrc/chd_ik.cu, one CTA per
+frame, the Jacobian never formed), on the host `ik_solve` per clip.  `ik_solve` is the host reference, batched over the
+frames with torch on the CPU:
 * every IK iteration is one batched pass: forward kinematics, the 3T x 6J Jacobian of the T target joints with respect
   to every joint's Euler angles (R = Rz Ry Rx) and local translation, and the damped step.  The reference factors the
   6J x 6J matrix J^T J + lambda^2 I per frame with a dense LU (414 x 414 for the 69-joint character); because the damping
@@ -15,9 +17,6 @@ device is given:
   over all frames;
 * the smoothing term couples a frame only to the previous iterate of its two neighbours, so the frames stay independent
   inside an iteration.
-Many clips of one skeleton at once (`ik_solve_batch`, `apply_results_batch`, `retarget_batch`): one `chd_ik_solve` call
-(csrc/chd_ik.cu, one CTA per frame, the Jacobian never formed) on a CUDA device, the single-clip functions per clip on
-the host.
 
 Pinned to the reference's own functions by tests/golden/make_towr_golden.py (tests/test_results_cpu.py).
 """
@@ -131,13 +130,13 @@ def descendants_mask(parents) -> np.ndarray:
 
 
 def ik_solve(anim: SkelAnim, targets: Dict[int, np.ndarray], iterations: int = 30, damping: float = 7.0, smoothness: float = 0.001,
-             device=None, gamma: float = 1.0, history: Optional[list] = None, translate: bool = True) -> SkelAnim:
+             history: Optional[list] = None, translate: bool = True) -> SkelAnim:
     """Damped least-squares full-body IK (JacobianInverseKinematicsCK, unit weights, no references / angle limits), all
-    frames at once; `translate`: the joints' local translations are unknowns too.  `targets`: joint index -> (F, 3)
-    world positions."""
+    frames at once in torch on the CPU: the host reference `chd_ik_solve` is tested against.  `translate`: the joints'
+    local translations are unknowns too.  `targets`: joint index -> (F, 3) world positions.  `history`, if given, gets
+    the mean target distance before every iteration and after the last."""
     import torch
-    dev = torch.device(device) if device is not None else torch.device("cpu")
-    f64 = dict(dtype=torch.float64, device=dev)
+    f64 = dict(dtype=torch.float64)
     parents = [int(p) for p in anim.parents]
     J, F = len(parents), anim.rotations.shape[0]
     tj = list(targets.keys())
@@ -172,8 +171,8 @@ def ik_solve(anim: SkelAnim, targets: Dict[int, np.ndarray], iterations: int = 3
                 torch.stack([sz * cy, sz * sy * sx + cz * cx, sz * sy * cx - cz * sx], -1), torch.stack([-sy, cy * sx, cy * cx], -1)]
         return torch.stack(rows, -2)
 
-    par_idx = torch.as_tensor([max(p, 0) for p in parents], device=dev)
-    root_mask = torch.as_tensor([p < 0 for p in parents], device=dev)
+    par_idx = torch.as_tensor([max(p, 0) for p in parents])
+    root_mask = torch.as_tensor([p < 0 for p in parents])
     for it in range(iterations):
         gR, gP = fk(Rl, Pl)
         e = euler_of(Rl)                                               # (F, J, 3)
@@ -196,7 +195,7 @@ def ik_solve(anim: SkelAnim, targets: Dict[int, np.ndarray], iterations: int = 3
             Jm = torch.cat([jr.reshape(F, 3 * J, 3 * T), jt.reshape(F, 3 * J, 3 * T)], dim=1).transpose(1, 2)     # (F, 3T, 6J)
         else:
             Jm = jr.reshape(F, 3 * J, 3 * T).transpose(1, 2)
-        err = gamma * (goal - tp).reshape(F, 3 * T)
+        err = (goal - tp).reshape(F, 3 * T)
         if history is not None:
             history.append(float(torch.sqrt(((goal - tp) ** 2).sum(-1)).mean()))
         A = Jm @ Jm.transpose(1, 2) + lam2 * I3T
@@ -211,7 +210,7 @@ def ik_solve(anim: SkelAnim, targets: Dict[int, np.ndarray], iterations: int = 3
     if history is not None:
         _, gP = fk(Rl, Pl)
         history.append(float(torch.sqrt(((goal - gP[:, tj]) ** 2).sum(-1)).mean()))
-    return SkelAnim(anim.names, anim.parents, anim.offsets, Rl.cpu().numpy(), Pl.cpu().numpy())
+    return SkelAnim(anim.names, anim.parents, anim.offsets, Rl.numpy(), Pl.numpy())
 
 
 IK_MAX_JOINTS = 128     # limits of the chd_ik_solve kernel (include/chd.h)
@@ -257,30 +256,40 @@ def ik_solve_batch(anims: Sequence[SkelAnim], targets: Sequence[Dict[int, np.nda
     import torch
     dev = torch.device(device) if device is not None else torch.device("cpu")
     if dev.type != "cuda":
-        return [ik_solve(a, tg, iterations=iterations, damping=damping, smoothness=smoothness, device=device, translate=translate)
+        return [ik_solve(a, tg, iterations=iterations, damping=damping, smoothness=smoothness, translate=translate)
                 for a, tg in zip(anims, targets)]
-    from .phys import _ptr, load_lib
-    L = load_lib()
-    parents = np.ascontiguousarray(anims[0].parents, dtype=np.int32)
-    tjn = np.asarray(tj, dtype=np.int32)
-    J, T, K = len(parents), len(tj), len(anims)
-    seg = np.zeros(K + 1, dtype=np.int32)
-    seg[1:] = np.cumsum([a.rotations.shape[0] for a in anims])
-    Ft = int(seg[-1])
+    frames = [a.rotations.shape[0] for a in anims]
+    J, T, Ft = len(anims[0].parents), len(tj), sum(frames)
     nR, nP = Ft * J * 9, Ft * J * 3
     host = np.concatenate([np.concatenate([a.rotations for a in anims]).reshape(-1), np.concatenate([a.positions for a in anims]).reshape(-1),
                            np.concatenate([np.stack([np.asarray(tg[k], dtype=np.float64) for k in tj], axis=1) for tg in targets]).reshape(-1)])
     buf = torch.as_tensor(host, dtype=torch.float64).to(dev)
+    _ik_kernel(anims[0].parents, tj, frames, buf[:nR].view(Ft, J, 3, 3), buf[nR:nR + nP].view(Ft, J, 3), buf[nR + nP:].view(Ft, T, 3),
+               iterations, damping, smoothness, translate)
+    out = buf[:nR + nP].cpu().numpy()
+    cut = np.cumsum(frames)[:-1]
+    R, P = np.split(out[:nR].reshape(Ft, J, 3, 3), cut), np.split(out[nR:].reshape(Ft, J, 3), cut)
+    return [SkelAnim(a.names, a.parents, a.offsets, r.copy(), p.copy()) for a, r, p in zip(anims, R, P)]
+
+
+def _ik_kernel(parents, tj, frames, R, P, goal, iterations, damping, smoothness, translate):
+    """One `chd_ik_solve` call on clips of `frames` frames stacked on the frame axis of the contiguous fp64 tensors on one
+    CUDA device R (Ft, J, 3, 3) and P (Ft, J, 3), which it updates in place, and goal (Ft, T, 3); target joints `tj`.
+    Allocates the kernel's work space on that device and runs on its current stream."""
+    import torch
+    from .phys import _ptr, load_lib
+    L = load_lib()
+    par, tjn = np.ascontiguousarray(parents, dtype=np.int32), np.ascontiguousarray(tj, dtype=np.int32)
+    seg = np.zeros(len(frames) + 1, dtype=np.int32)
+    seg[1:] = np.cumsum(frames)
+    J, T, Ft = len(par), len(tjn), int(seg[-1])
+    dev = R.device
     work = torch.empty(max(L.chd_ik_work_bytes(Ft, J, T) // 8, 1), dtype=torch.float64, device=dev)
-    base = buf.data_ptr()
     with torch.cuda.device(dev):
-        rc = L.chd_ik_solve(J, _ptr(parents), T, _ptr(tjn), _ptr(seg), K, Ft, base, base + 8 * nR, base + 8 * (nR + nP), int(iterations),
+        rc = L.chd_ik_solve(J, _ptr(par), T, _ptr(tjn), _ptr(seg), len(frames), Ft, R.data_ptr(), P.data_ptr(), goal.data_ptr(), int(iterations),
                             float(damping), float(smoothness), int(bool(translate)), work.data_ptr(), torch.cuda.current_stream(dev).cuda_stream)
     if rc != 0:
         raise RuntimeError("chd_ik_solve failed with code %d" % rc)
-    out = buf[:nR + nP].cpu().numpy()
-    R, P = out[:nR].reshape(Ft, J, 3, 3), out[nR:].reshape(Ft, J, 3)
-    return [SkelAnim(a.names, a.parents, a.offsets, R[seg[k]:seg[k + 1]].copy(), P[seg[k]:seg[k + 1]].copy()) for k, a in enumerate(anims)]
 
 
 def _apply_setup(res: TowrResults, anim_bvh: str, start_idx, end_idx, info: CharacterInfo, run_ik: bool, device):
@@ -319,11 +328,8 @@ def apply_results(res: TowrResults, anim_bvh: str, start_idx, end_idx, info: Cha
                   iterations: int = 30):
     """towr_utils.apply_results: returns (anim, names, anim_og, com_og).  The root follows the optimised COM (keeping every
     upper-body joint's offset from the COM) and base orientation; with `run_ik` the upper-body joints, toes and (4-foot
-    results) heels are IK targets."""
-    anim, anim_og, com, targets = _apply_setup(res, anim_bvh, start_idx, end_idx, info, run_ik, device)
-    if run_ik:
-        anim = ik_solve(anim, targets, iterations=iterations, smoothness=0.001, damping=7.0, device=device)
-    return anim, anim.names, anim_og, com
+    results) heels are IK targets.  A batch of one of `apply_results_batch`."""
+    return apply_results_batch([(res, anim_bvh, start_idx, end_idx)], info, run_ik, device, iterations)[0]
 
 
 def apply_results_batch(jobs, info: CharacterInfo, run_ik: bool = True, device=None, iterations: int = 30):
@@ -373,11 +379,9 @@ def retarget(src_bvh: str, skel_bvh: str, info: CharacterInfo, out_bvh: Optional
     """combined_to_mixamo.retarget: scales the source joint positions by the ratio of the hip heights (floor at 0 through a
     soft minimum of the foot heights), initialises the character's angles from the mapped source Euler angles, runs the
     damped least-squares IK (translating joints, 200 iterations, damping 7) towards the mapped joints, restores the bone
-    offsets and corrects the root height by the median ankle difference.  Returns the SkelAnim (and saves it if asked)."""
-    sk, skel_height = _retarget_skeleton(skel_bvh, info)
-    anim, tm, targets, src_floor = _retarget_setup(src_bvh, sk, skel_height, info)
-    anim = ik_solve(anim, tm, iterations=iterations, smoothness=0.0, damping=7.0, translate=True, device=device)
-    return _retarget_finish(anim, sk, targets, src_floor, info, out_bvh)
+    offsets and corrects the root height by the median ankle difference.  Returns the SkelAnim (and saves it if asked).
+    A batch of one of `retarget_batch`."""
+    return retarget_batch([src_bvh], skel_bvh, info, [out_bvh], device, iterations)[0]
 
 
 def retarget_batch(src_bvhs: Sequence[str], skel_bvh: str, info: CharacterInfo, out_bvhs: Optional[Sequence[Optional[str]]] = None,

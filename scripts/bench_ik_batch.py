@@ -1,6 +1,7 @@
 """Batched full-body IK on cuda:0 (`chd.results.apply_results_batch` / `retarget_batch`, kernel `chd_ik_solve`) against
-the per-clip loops of `apply_results(device="cuda:0")` / `retarget(device="cuda:0")`, on the 69-joint ybot-like character
-of scripts/bench_skeletons.py (67 joints in the files, the two heels added by apply_results).  Prints one JSON line:
+the per-clip loops of `apply_results(device="cuda:0")` / `retarget(device="cuda:0")`, i.e. one batch-of-one kernel call
+per clip (per result file for apply), on the 69-joint ybot-like character of scripts/bench_skeletons.py (67 joints in
+the files, the two heels added by apply_results).  Prints one JSON line:
   per workload K x F (clips x frames), for `apply` (3 result files per clip x 30 iterations, 61 targets) and `retarget`
   (200 iterations): host-clock seconds of both arms over `--runs` alternating runs after one warm-up call of each arm,
   peak device memory of each arm, max |difference| between the arms' outputs (rotation entries, local translations in
@@ -114,35 +115,25 @@ def max_diff(xs, ys):
 def kernel_time(anims, targets, iterations, smoothness, translate, reps):
     """CUDA-event ms per iteration of one chd_ik_solve call on the stacked clips."""
     import torch
-    L = chd.phys.load_lib()
     dev = torch.device("cuda:0")
     tj = list(targets[0])
-    parents = np.ascontiguousarray(anims[0].parents, np.int32)
-    tjn = np.asarray(tj, np.int32)
-    seg = np.zeros(len(anims) + 1, np.int32)
-    seg[1:] = np.cumsum([a.rotations.shape[0] for a in anims])
-    Ft, J, T = int(seg[-1]), len(parents), len(tj)
+    frames = [a.rotations.shape[0] for a in anims]
     R0 = torch.as_tensor(np.concatenate([a.rotations for a in anims]), device=dev)
     P0 = torch.as_tensor(np.concatenate([a.positions for a in anims]), device=dev)
     goal = torch.as_tensor(np.concatenate([np.stack([tg[j] for j in tj], 1) for tg in targets]), device=dev).contiguous()
     R, P = R0.clone(), P0.clone()
-    work = torch.empty(L.chd_ik_work_bytes(Ft, J, T) // 8, dtype=torch.float64, device=dev)
-    vp = lambda a: a.ctypes.data_as(chd.phys.C.c_void_p)
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     ms = []
     for r in range(reps + 1):
         R.copy_(R0)
         P.copy_(P0)
         e0.record()
-        rc = L.chd_ik_solve(J, vp(parents), T, vp(tjn), vp(seg), len(anims), Ft, R.data_ptr(), P.data_ptr(), goal.data_ptr(), iterations,
-                            7.0, smoothness, int(translate), work.data_ptr(), torch.cuda.current_stream().cuda_stream)
+        chd.results._ik_kernel(anims[0].parents, tj, frames, R, P, goal, iterations, 7.0, smoothness, translate)
         e1.record()
         torch.cuda.synchronize()
-        if rc != 0:
-            raise RuntimeError("chd_ik_solve failed with code %d" % rc)
         if r:                                # the first call is a warm-up
             ms.append(e0.elapsed_time(e1) / iterations)
-    return float(np.median(ms)), Ft, parents, tj
+    return float(np.median(ms)), sum(frames), anims[0].parents, tj
 
 
 def timed(fn):

@@ -1,6 +1,7 @@
-"""Timing of the two torch-batched steps around the hot path (not part of bench.py's contract): the kinematic optimiser
+"""Timing of the two kinematic steps around the hot path (not part of bench.py's contract): the kinematic optimiser
 (`chd.kinopt.optimize_trajectory`, 2 x 50 evaluations like the reference's two least_squares stages) and the IK of
-`apply_results` (30 iterations, 69-joint character), on cuda:0 and on the host cores.  One JSON line.
+`apply_results` (30 iterations, 69-joint character), on cuda:0 (`chd_kin_solve` / `chd_ik_solve`) and on the host
+cores (torch).  One JSON line.
 The reference's own optimize_trajectory needed 7.5 s for the 14-frame golden clip in the build container
 (tests/golden/kinopt/run.npz `seconds`); its dense Jacobian is 4 GB at 120 frames."""
 import json
@@ -48,9 +49,10 @@ def main():
         tag = dev or "cpu"
         for rep in range(2):
             t0 = time.perf_counter()
-            chd.results.ik_solve(anim, targets, iterations=30, damping=7.0, smoothness=0.001, device=dev)
-            if dev:
-                torch.cuda.synchronize()
+            if dev:          # returns host arrays, so the time includes the kernel
+                chd.results.ik_solve_batch([anim], [targets], iterations=30, damping=7.0, smoothness=0.001, device=dev)
+            else:
+                chd.results.ik_solve(anim, targets, iterations=30, damping=7.0, smoothness=0.001)
             dt = time.perf_counter() - t0
         out["ik_s_" + tag] = dt
     print(json.dumps(out))

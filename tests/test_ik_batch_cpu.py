@@ -1,5 +1,6 @@
 """The batched IK entry points on the host: `ik_solve_batch`, `apply_results_batch` and `retarget_batch` give bitwise
-what the single-clip functions give, and refuse batches the `chd_ik_solve` kernel cannot take."""
+what `ik_solve` per clip gives (and the single-clip functions, a batch of one each, what the batch gives), and refuse
+batches the `chd_ik_solve` kernel cannot take."""
 import os
 
 import numpy as np
@@ -53,6 +54,14 @@ def golden_jobs(chd):
     return jobs
 
 
+def host_apply(rs, job, info, iterations=3, run_ik=True):
+    """apply_results composed from its steps on the host: the set-up, then `ik_solve`."""
+    anim, anim_og, com, targets = rs._apply_setup(*job, info, run_ik, None)
+    if run_ik:
+        anim = rs.ik_solve(anim, targets, iterations=iterations, smoothness=0.001, damping=7.0)
+    return anim, anim.names, anim_og, com
+
+
 @pytest.mark.parametrize("case", list(CASES))
 def test_apply_results_batch_host_is_apply_results(chd, case):
     rs = chd.results
@@ -60,11 +69,16 @@ def test_apply_results_batch_host_is_apply_results(chd, case):
     info = chd.prepare.CHARACTERS[case.split("_")[0]]()
     got = rs.apply_results_batch([j[1:] for j in jobs], info, iterations=3)
     for j, g in zip(jobs, got):
-        ref = rs.apply_results(*j[1:], info, iterations=3)
+        ref = host_apply(rs, j[1:], info)
         assert_same(g[0], ref[0])
         assert_same(g[2], ref[2])
         assert g[1] == ref[1]
         np.testing.assert_array_equal(g[3], ref[3])
+        one = rs.apply_results(*j[1:], info, iterations=3)          # a batch of one
+        assert_same(one[0], g[0])
+        assert_same(one[2], g[2])
+        assert one[1] == g[1]
+        np.testing.assert_array_equal(one[3], g[3])
 
 
 def test_apply_results_batch_mixes_2_and_4_feet(chd):
@@ -74,10 +88,10 @@ def test_apply_results_batch_mixes_2_and_4_feet(chd):
     info = chd.prepare.combined_info()
     got = rs.apply_results_batch([j[1:] for j in jobs], info, iterations=3)
     for j, g in zip(jobs, got):
-        assert_same(g[0], rs.apply_results(*j[1:], info, iterations=3)[0])
+        assert_same(g[0], host_apply(rs, j[1:], info)[0])
     got0 = rs.apply_results_batch([j[1:] for j in jobs], info, run_ik=False)
     for j, g in zip(jobs, got0):
-        assert_same(g[0], rs.apply_results(*j[1:], info, run_ik=False)[0])
+        assert_same(g[0], host_apply(rs, j[1:], info, run_ik=False)[0])
 
 
 def test_retarget_batch_host_is_retarget(chd, tmp_path):
@@ -85,10 +99,17 @@ def test_retarget_batch_host_is_retarget(chd, tmp_path):
     src, skel, info = os.path.join(G, "combined", "anim.bvh"), os.path.join(G, "retarget", "ybot_skel.bvh"), chd.prepare.ybot_info()
     outs = [str(tmp_path / "a.bvh"), None]
     got = rs.retarget_batch([src, src], skel, info, out_bvhs=outs, iterations=3)
-    ref = rs.retarget(src, skel, info, out_bvh=str(tmp_path / "r.bvh"), iterations=3)
+    # retarget composed from its steps on the host: skeleton, set-up, `ik_solve`, finish
+    sk, h = rs._retarget_skeleton(skel, info)
+    anim, tm, targets, src_floor = rs._retarget_setup(src, sk, h, info)
+    anim = rs.ik_solve(anim, tm, iterations=3, smoothness=0.0, damping=7.0, translate=True)
+    ref = rs._retarget_finish(anim, sk, targets, src_floor, info, str(tmp_path / "r.bvh"))
     for g in got:
         assert_same(g, ref)
     assert open(outs[0]).read() == open(str(tmp_path / "r.bvh")).read()
+    one = rs.retarget(src, skel, info, out_bvh=str(tmp_path / "one.bvh"), iterations=3)     # a batch of one
+    assert_same(one, got[0])
+    assert open(str(tmp_path / "one.bvh")).read() == open(outs[0]).read()
 
 
 def test_ik_solve_batch_refuses(chd):

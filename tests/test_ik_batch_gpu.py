@@ -67,7 +67,12 @@ def test_apply_results_batch_matches_reference(chd, case):
     toe_err = np.linalg.norm(an.global_positions()[:, info.toes[0]] - r.feet_pos[:s1 - s0, 0] * 100.0, axis=1).mean()
     toe_err0 = np.linalg.norm(out[0][2].global_positions()[:, info.toes[0]] - r.feet_pos[:s1 - s0, 0] * 100.0, axis=1).mean()
     assert toe_err < 0.25 * toe_err0
-    for j, o in zip(jobs[1:], out[1:]):          # the 2-foot job of `combined`, solved in its own group
+    # every job (for `combined` also the 2-foot one, solved in its own group): the single-clip call on the device is the
+    # batch element bitwise, and the host IK within tolerance
+    for j, o in zip(jobs, out):
+        one = rs.apply_results(*j, info, device=DEV)[0]
+        np.testing.assert_array_equal(one.rotations, o[0].rotations)
+        np.testing.assert_array_equal(one.positions, o[0].positions)
         ref = rs.apply_results(*j, info)[0]
         assert np.abs(o[0].rotations - ref.rotations).max() <= ROT_TOL
         assert np.abs(o[0].positions - ref.positions).max() <= POS_TOL
@@ -76,12 +81,18 @@ def test_apply_results_batch_matches_reference(chd, case):
 def test_retarget_batch_matches_reference(chd):
     rs = chd.results
     g = np.load(os.path.join(G, "retarget", "retarget.npz"))
-    src = os.path.join(G, "combined", "anim.bvh")
-    for a in rs.retarget_batch([src, src], os.path.join(G, "retarget", "ybot_skel.bvh"), chd.prepare.ybot_info(), device=DEV):
+    src, skel, info = os.path.join(G, "combined", "anim.bvh"), os.path.join(G, "retarget", "ybot_skel.bvh"), chd.prepare.ybot_info()
+    one = rs.retarget(src, skel, info, device=DEV)
+    host = rs.retarget(src, skel, info)
+    assert np.abs(one.rotations - host.rotations).max() <= ROT_TOL
+    assert np.abs(one.positions - host.positions).max() <= POS_TOL
+    for a in rs.retarget_batch([src, src], skel, info, device=DEV):
         np.testing.assert_allclose(a.rotations, qmat(g["rot_q"]), atol=5e-7)
         np.testing.assert_allclose(a.positions, g["pos"], atol=2e-6)
         np.testing.assert_allclose(a.global_positions(), g["gpos"], atol=2e-5)
         np.testing.assert_allclose(a.positions[:, 1:], np.tile(a.offsets[None, 1:], (a.positions.shape[0], 1, 1)), atol=0)
+        np.testing.assert_array_equal(a.rotations, one.rotations)          # the single-clip call is a batch of one
+        np.testing.assert_array_equal(a.positions, one.positions)
 
 
 def test_batch_invariance(chd):

@@ -140,7 +140,8 @@ def test_run_phys_mocap_whole_chain(chd, tmp_path):
 
 
 def test_torch_batched_solvers_same_on_gpu_and_cpu(chd, tmp_path):
-    """The kinematic optimiser and the IK are torch-batched over the frames: same numbers on cuda:0 and on the host."""
+    """The kinematic optimiser with its IK initialisation (on cuda:0 through `chd_kin_solve` and `chd_ik_solve`): same
+    numbers on cuda:0 and on the host."""
     import torch
     assert torch.cuda.is_available()
     vd = str(tmp_path / "w")
