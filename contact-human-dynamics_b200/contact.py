@@ -28,7 +28,6 @@ def load_keypoint_files(files: Sequence[str], num_joints: int = 25, threads: int
     L = load_lib()
     out = np.empty((len(files), num_joints, 3), dtype=np.float64)
     arr = (C.c_char_p * len(files))(*[os.fsencode(f) for f in files])
-    L.chd_openpose_load.argtypes = [C.POINTER(C.c_char_p), C.c_int32, C.c_int32, C.c_void_p, C.c_int32]
     rc = L.chd_openpose_load(arr, len(files), num_joints, out.ctypes.data_as(C.c_void_p), threads)
     if rc:
         raise RuntimeError("chd_openpose_load failed: %d (-2 unreadable file, -3 malformed keypoint file)" % rc)
@@ -102,17 +101,7 @@ class ContactNet:
 
     def __init__(self, state_dict: Dict[str, np.ndarray], device: int = -1, bn_eps: float = 1e-5, precision: str = "fp32"):
         code = precision_code(precision)
-        self.L = load_lib()
-        L = self.L
-        L.chd_contact_create.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_float, C.c_int32, C.POINTER(C.c_void_p)]
-        L.chd_contact_destroy.argtypes = [C.c_void_p]
-        L.chd_contact_destroy.restype = None
-        L.chd_contact_forward.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-        L.chd_contact_preprocess.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]
-        L.chd_contact_detect.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]
-        L.chd_contact_launch_count.argtypes = [C.c_void_p]
-        L.chd_contact_launch_count.restype = C.c_int64
-        L.chd_contact_set_precision.argtypes = [C.c_void_p, C.c_int32]
+        self.L = L = load_lib()
         w, b, bn = pack_state_dict(state_dict)
         assert w.size == sum(i * o for i, o in zip(DIMS[:-1], DIMS[1:])) and b.size == sum(DIMS[1:])
         h = C.c_void_p()

@@ -254,12 +254,7 @@ static int batch_create_impl(const chd_phys_problem* problems, int32_t batch, co
                              const chd_phys_options& opt, chd_phys_batch* b);
 
 int chd_phys_batch_create(const chd_phys_problem* problems, int32_t batch, const chd_phys_weights* weights, int32_t device,
-                          chd_phys_batch** out) {
-  return chd_phys_batch_create_ex(problems, batch, weights, device, nullptr, out);
-}
-
-int chd_phys_batch_create_ex(const chd_phys_problem* problems, int32_t batch, const chd_phys_weights* weights, int32_t device,
-                             const chd_phys_options* opt, chd_phys_batch** out) {
+                          const chd_phys_options* opt, chd_phys_batch** out) {
   if (!problems || batch <= 0 || !out) return -1;
   chd_phys_options o = {-1};
   if (opt) o = *opt;
@@ -532,15 +527,6 @@ int chd_phys_get_duals(const chd_phys_batch* b, double* y, double* zL, double* z
     CHD_CUDA(cudaMemcpy(ipm.data(), b->D.ipm, B * sizeof(ChdIpm), cudaMemcpyDeviceToHost));
     for (size_t i = 0; i < B; ++i) obj_scale[i] = ipm[i].sf;
   }
-  return 0;
-}
-
-/* diagnostic: line-search inputs of the last KKT solve of sequence i (a_pr, a_du, dphi, phi0, theta0, theta_ref, mu, delta_w) */
-int chd_phys_debug_ipm(const chd_phys_batch* b, int32_t i, double* out8) {
-  if (!b || !out8 || b->host_only || !b->h_ipm || i < 0 || i >= b->hb.B) return -1;
-  const ChdIpm& I = b->h_ipm[i];
-  out8[0] = I.a_pr, out8[1] = I.a_du, out8[2] = I.dphi, out8[3] = I.phi0, out8[4] = I.theta0, out8[5] = I.theta_ref, out8[6] = I.mu, out8[7] = I.delta_w;
-  for (int q = 0; q < 8; ++q) out8[8 + q] = I.dbg[q];
   return 0;
 }
 

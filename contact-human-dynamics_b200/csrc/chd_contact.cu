@@ -16,7 +16,6 @@
 // wgmma has no fp32-input kind).  The opt-in 3xTF32 tensor-core mode of the three large layers (CHD_CONTACT_TF32X3)
 // is in chd_contact_tc.cu; this file's kernels are the default FP32 mode.
 #include <cuda_runtime.h>
-#include <cstdlib>
 
 #include <algorithm>
 #include <cstdint>
@@ -216,8 +215,6 @@ struct chd_contact_net {
   float* ws = nullptr;     // activation workspace of one slab: A0 [Mp][352] | A1 [Mp][1024] | A2 [Mp][512] | A3 [Mp][128]
   int ws_rows = 0;
   // grow-only device buffers of the host entry points (no allocation per call, nothing to leak on an error path)
-  cudaStream_t copy_stream = nullptr;   // uploads of chd_contact_detect run ahead of the compute stream, chunk by chunk
-  cudaEvent_t ev_up[4] = {nullptr, nullptr, nullptr, nullptr};
   void* io[8] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
   size_t io_bytes[8] = {0, 0, 0, 0, 0, 0, 0, 0};
   // CHD_CONTACT_TF32X3: split weight planes (one allocation) and the slab workspace of the tensor-core layers
@@ -313,8 +310,6 @@ int chd_contact_create(const float* weights, const float* biases, const float* b
   const int dims[6] = {CT_IN, 1024, 512, 128, 32, 20};
   chd_contact_net* net = new chd_contact_net();
   CT_CUDA(cudaStreamCreate(&net->stream));
-  CT_CUDA(cudaStreamCreateWithFlags(&net->copy_stream, cudaStreamNonBlocking));
-  for (int q = 0; q < 4; ++q) CT_CUDA(cudaEventCreateWithFlags(&net->ev_up[q], cudaEventDisableTiming));
   auto up = [&](const std::vector<float>& h, const float** d) -> int {
     void* p = nullptr;
     CT_CUDA(cudaMalloc(&p, h.size() * sizeof(float)));
@@ -359,9 +354,6 @@ void chd_contact_destroy(chd_contact_net* net) {
   if (net->tc_ws) cudaFree(net->tc_ws);
   for (int q = 0; q < 8; ++q)
     if (net->io[q]) cudaFree(net->io[q]);
-  for (int q = 0; q < 4; ++q)
-    if (net->ev_up[q]) cudaEventDestroy(net->ev_up[q]);
-  if (net->copy_stream) cudaStreamDestroy(net->copy_stream);
   if (net->stream) cudaStreamDestroy(net->stream);
   delete net;
 }
@@ -482,61 +474,21 @@ int chd_contact_detect(chd_contact_net* net, const double* raw, const int32_t* s
                        float* min_abs_logit) {
   if (!net || !raw || !seq_offsets || V <= 0 || dim_w <= 0 || !labels_out) return -1;
   int Fmax = 0;
-  const int total = seq_offsets[V];
-  for (int v = 0; v < V; ++v) {
-    if (seq_offsets[v + 1] <= seq_offsets[v]) return -1;
-    Fmax = std::max(Fmax, seq_offsets[v + 1] - seq_offsets[v]);
-  }
-  if (Fmax < CT_WIN) return -1;
-  const size_t Wn = Fmax - (CT_WIN - 1), nlog = (size_t)V * Wn * 20, nlab = (size_t)V * Fmax * 4;
-  int rc;
-  if ((rc = ct_reserve(net, IO_RAW, (size_t)total * 75 * sizeof(double))) || (rc = ct_reserve(net, IO_OFFS, (V + 1) * sizeof(int))) ||
-      (rc = ct_reserve(net, IO_FRAMES, (size_t)V * Fmax * 75 * sizeof(double))) || (rc = ct_reserve(net, IO_LENS, V * sizeof(int))) ||
-      (rc = ct_reserve(net, IO_LABELS, nlab * sizeof(long long))) || (rc = ct_reserve(net, IO_LOGITS, nlog * sizeof(float))) ||
-      (rc = ct_reserve(net, IO_MIN, 4 * sizeof(float))) || (rc = ct_reserve(net, IO_PACKED, (size_t)total * 4 * sizeof(long long))))
+  int rc = ct_prep_device(net, raw, seq_offsets, V, dim_w, &Fmax);
+  if (rc) return rc;
+  const size_t total = seq_offsets[V], Wn = Fmax - (CT_WIN - 1), nlog = (size_t)V * Wn * 20, nlab = (size_t)V * Fmax * 4;
+  if ((rc = ct_reserve(net, IO_LABELS, nlab * sizeof(long long))) || (rc = ct_reserve(net, IO_LOGITS, nlog * sizeof(float))) ||
+      (rc = ct_reserve(net, IO_MIN, sizeof(float))) || (rc = ct_reserve(net, IO_PACKED, total * 4 * sizeof(long long))))
     return rc;
-  // Videos are independent: the batch is cut into up to four chunks whose keypoints are uploaded on a copy stream while
-  // the previous chunk is preprocessed, classified and voted on the compute stream (the 65 MB upload of the 100k-window
-  // configuration otherwise sits in front of about 6 ms of compute on an H100); every chunk is padded to the global
-  // Fmax, so the labels do not depend on the cut.
-  int nchunk = 1;
-  if (const char* e = getenv("CHD_CONTACT_CHUNKS")) nchunk = std::max(1, std::min(4, atoi(e)));
-  if (V < 16 * nchunk) nchunk = 1;
-  const int per = (V + nchunk - 1) / nchunk;
-  const double scale = 1280.0 / dim_w;
-  double* d_raw = (double*)net->io[IO_RAW];
-  int* d_off = (int*)net->io[IO_OFFS];
-  CT_CUDA(cudaMemcpyAsync(d_off, seq_offsets, (V + 1) * sizeof(int), cudaMemcpyHostToDevice, net->copy_stream));
-  for (int c = 0; c < nchunk; ++c) {
-    const int v0 = c * per, v1 = std::min(V, v0 + per);
-    if (v0 >= v1) break;
-    const size_t f0 = seq_offsets[v0], f1 = seq_offsets[v1];
-    CT_CUDA(cudaMemcpyAsync(d_raw + f0 * 75, raw + f0 * 75, (f1 - f0) * 75 * sizeof(double), cudaMemcpyHostToDevice, net->copy_stream));
-    CT_CUDA(cudaEventRecord(net->ev_up[c], net->copy_stream));
-  }
-  for (int c = 0; c < nchunk; ++c) {
-    const int v0 = c * per, v1 = std::min(V, v0 + per);
-    if (v0 >= v1) break;
-    const int Vc = v1 - v0;
-    CT_CUDA(cudaStreamWaitEvent(net->stream, net->ev_up[c], 0));
-    double* fr = (double*)net->io[IO_FRAMES] + (size_t)v0 * Fmax * 75;
-    int* lens = (int*)net->io[IO_LENS] + v0;
-    long long* lab = (long long*)net->io[IO_LABELS] + (size_t)v0 * Fmax * 4;
-    chd_k_contact_prep<<<(Vc * 25 + 127) / 128, 128, 0, net->stream>>>(d_raw, d_off + v0, Vc, Fmax, scale, 200.4160302695367, 0.2, fr, lens);
-    net->launches += 1;
-    rc = chd_contact_forward_device(net, fr, Vc, Fmax, lens, (int64_t*)lab, (float*)net->io[IO_LOGITS] + (size_t)v0 * Wn * 20,
-                                    (float*)net->io[IO_MIN] + c, net->stream);
-    if (rc) return rc;
-    chd_k_contact_pack<<<dim3(4, Vc), 256, 0, net->stream>>>(lab, d_off + v0, Vc, Fmax, (long long*)net->io[IO_PACKED]);
-    net->launches += 1;
-    const size_t f0 = seq_offsets[v0], f1 = seq_offsets[v1];
-    CT_CUDA(cudaMemcpyAsync(labels_out + f0 * 4, (long long*)net->io[IO_PACKED] + f0 * 4, (f1 - f0) * 4 * sizeof(long long), cudaMemcpyDeviceToHost,
-                            net->stream));
-  }
-  float mins[4] = {3.4e38f, 3.4e38f, 3.4e38f, 3.4e38f};
-  CT_CUDA(cudaMemcpyAsync(mins, net->io[IO_MIN], nchunk * sizeof(float), cudaMemcpyDeviceToHost, net->stream));
+  long long* d_lab = (long long*)net->io[IO_LABELS];
+  rc = chd_contact_forward_device(net, (const double*)net->io[IO_FRAMES], V, Fmax, (const int*)net->io[IO_LENS], (int64_t*)d_lab,
+                                  (float*)net->io[IO_LOGITS], (float*)net->io[IO_MIN], net->stream);
+  if (rc) return rc;
+  chd_k_contact_pack<<<dim3(4, V), 256, 0, net->stream>>>(d_lab, (const int*)net->io[IO_OFFS], V, Fmax, (long long*)net->io[IO_PACKED]);
+  net->launches += 1;
+  CT_CUDA(cudaMemcpyAsync(labels_out, net->io[IO_PACKED], total * 4 * sizeof(long long), cudaMemcpyDeviceToHost, net->stream));
+  if (min_abs_logit) CT_CUDA(cudaMemcpyAsync(min_abs_logit, net->io[IO_MIN], sizeof(float), cudaMemcpyDeviceToHost, net->stream));
   CT_CUDA(cudaStreamSynchronize(net->stream));
-  if (min_abs_logit) *min_abs_logit = std::min(std::min(mins[0], mins[1]), std::min(mins[2], mins[3]));
   return 0;
 }
 

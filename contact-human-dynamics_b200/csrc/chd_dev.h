@@ -47,7 +47,6 @@ struct ChdIpm {
   double mu, delta_w, sf, theta_max, theta_min, mu_filter, tau;
   double f, E0, viol_u, dual_u, compl_u;          // error measures at the current iterate
   double phi0, theta0, dphi, a_pr, a_du;          // line-search inputs produced by the KKT kernel
-  double dbg[8];                                  // diagnostics of the last line search: alpha, backtracks, theta_t, phi_t, guard / trust refusals
   double dw_floor;                                // current floor of delta_w (adaptive: CHD_AF_N)
   int af_cnt, af_off;                             // consecutive full steps taken at the floor; 1: the lowered floor was taken back for this stage
   int af_it, af_pad;                              // iteration of the first drop of the floor
@@ -103,7 +102,7 @@ struct ChdDev {
   double* snapshots;                          // 3 x B x fo_max x (6 + 7 n_ee_max)
 };
 
-// IPM constants (oracle/ipm_proto.py Opts; IPOPT defaults unless noted)
+// IPM constants (Opts of oracle/ipm_oracle.cpp; IPOPT defaults unless noted)
 #define CHD_TOL 1e-3            /* phys_optim.cpp:578 */
 #define CHD_CONSTR_VIOL_TOL 1e-4
 #define CHD_DUAL_INF_TOL 1.0

@@ -258,8 +258,6 @@ __global__ void __launch_bounds__(CHD_THREADS) chd_k_linesearch(ChdDev D) {
       bool ok = isfinite(phit) && isfinite(theta_t) && theta_t <= I.theta_max;
       // nonlinearity guard of stage 3: the linearised constraints predict theta(alpha) = (1 - alpha) theta; the trial
       // point is refused while the second-order error exceeds the predicted decrease (or a small absolute level)
-      if (ls == 0) I.dbg[4] = 0.0, I.dbg[5] = 0.0;
-      I.dbg[0] = alpha, I.dbg[1] = ls, I.dbg[2] = theta_t, I.dbg[3] = phit;
       if (sg.opt_dur && s_trust) ok = false;
       if (sg.opt_dur && ok && theta_t - (1.0 - alpha) * theta > CHD_NL_GUARD * fmax(alpha * theta, CHD_NL_FLOOR * fmax(1.0, theta_ref))) ok = false;
       for (int q = 0; ok && q < I.nfilt; ++q)
@@ -284,7 +282,7 @@ __global__ void __launch_bounds__(CHD_THREADS) chd_k_linesearch(ChdDev D) {
     alpha *= 0.5;
   }
   if (!accepted) {
-    alpha *= 2.0;  // the last (smallest) trial step is taken, as in oracle/ipm_proto.py
+    alpha *= 2.0;  // the last (smallest) trial step is taken, as in the filter line search of oracle/ipm_oracle.cpp
     ls = CHD_MAX_BACKTRACK;
   }
   // x was left at the accepted trial point in xt

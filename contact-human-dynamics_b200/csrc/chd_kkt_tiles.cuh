@@ -81,25 +81,6 @@ __device__ __forceinline__ void chd_tile_sub_xyT(double* C, const double* X, con
   C[r * 8 + 2 * k + 1] = c1;
 }
 
-// Reciprocal of a pivot: hardware approximation (MUFU.RCP64H, ~20 bits) + three Newton steps instead of the IEEE division
-// routine -- the divide -> multiply -> fma chain of the eight sequential pivots of a diagonal tile is the critical path
-// of a block column (warp 0), and the division is its longest link.  Result within 1 ulp of 1/d.
-__device__ __forceinline__ double chd_rcp(double d) {
-  double r;
-  asm("rcp.approx.ftz.f64 %0, %1;" : "=d"(r) : "d"(d));
-  r = fma(fma(-d, r, 1.0), r, r);
-  r = fma(fma(-d, r, 1.0), r, r);
-  r = fma(fma(-d, r, 1.0), r, r);
-  return r;
-}
-
-// (benchmark batch on an H100 SXM at 400 W: 1.115 ms per KKT launch with chd_rcp, 1.144 ms with the IEEE division.
-// The correctly rounded division stays the default, as in the CPU oracle; chd_rcp is available with -DCHD_FAST_RCP)
-#ifdef CHD_FAST_RCP
-#define CHD_RCP(d) chd_rcp(d)
-#else
-#define CHD_RCP(d) (1.0 / (d))
-#endif
 // In-place LDL^T of the lower triangle of an 8x8 row-major tile by one warp (lanes replicate rows r = lane&7).
 // On exit: strict lower part = unit L, diagonal = d.  dinv[8] receives 1/d and winv[64] the inverse W = L^-1
 // (unit lower triangular) in fragment order, so that the panel below the tile becomes one tensor-core product
@@ -120,7 +101,7 @@ __device__ __forceinline__ bool chd_tile_ldl(double* T, double* dinv, double* wi
   for (int p = 0; p < 8; ++p) {
     const double dp = __shfl_sync(0xffffffffu, a[p], p, 8);
     ok = ok && (fabs(dp) > 1e-300) && isfinite(dp);
-    const double inv = CHD_RCP(dp);
+    const double inv = 1.0 / dp;   // correctly rounded, as in the CPU oracle (DESIGN §9 item 0)
     const double lr = a[p] * inv;
 #pragma unroll
     for (int c = p + 1; c < 8; ++c) {

@@ -7,8 +7,6 @@
 #include <thread>
 #include <cmath>
 #include <cstring>
-#include <cstdio>
-#include <cstdlib>
 #include <numeric>
 
 namespace {
@@ -618,7 +616,6 @@ int build_sequence(const chd_phys_problem& p, SeqBuild& sb, int band_above) {
   double best_cost = 0;
   for (int ci = 0; ci < 4; ++ci) {
     const double cst = order_kkt(cand[ci]);
-    if (getenv("CHD_LAYOUT_DEBUG")) fprintf(stderr, "cand %g: Na %d nb %d/%d w %d/%d cost %g\n", cand[ci], h.Na, h.nb_fix, h.nb, h.w_fix, h.w, cst);
     if (ci == 0 || cst < 0.9 * best_cost) best = ci, best_cost = cst;   // leave the default unless clearly better
   }
   order_kkt(cand[best]);

@@ -50,12 +50,50 @@ class _Dims(C.Structure):
                                           "na_max", "nb_max", "w_max", "frames_out_max")]
 
 
-EXPORTS = ["chd_version", "chd_phys_batch_create", "chd_phys_batch_create_ex", "chd_phys_batch_destroy", "chd_phys_get_dims", "chd_phys_get_sizes",
-           "chd_phys_get_x", "chd_phys_set_x", "chd_phys_eval", "chd_phys_get_layout", "chd_phys_solve_stage",
-           "chd_phys_solve", "chd_phys_sample", "chd_phys_sample_device", "chd_phys_launch_count",
-           "chd_phys_kernel_times", "chd_phys_set_timing", "chd_phys_h2d_bytes", "chd_phys_reset", "chd_measure_fp64_peak", "chd_phys_get_slot_index", "chd_phys_get_ent_col",
-           "chd_phys_get_duals", "chd_phys_stage_stats", "chd_phys_get_sizes_fixed", "chd_kin_solve", "chd_kin_work_bytes",
-           "chd_ik_solve", "chd_ik_work_bytes"]
+_vp, _i32, _i64, _int, _f64 = C.c_void_p, C.c_int32, C.c_int64, C.c_int, C.c_double
+
+# Every function of include/chd.h, name -> (restype, argtypes); load_lib applies it.  Arrays, handles and streams are
+# passed as c_void_p.
+SIGNATURES = {
+    "chd_phys_batch_create": (_int, [C.POINTER(_Problem), _i32, C.POINTER(_Weights), _i32, C.POINTER(_Options),
+                                     C.POINTER(_vp)]),
+    "chd_phys_batch_destroy": (None, [_vp]),
+    "chd_phys_get_dims": (_int, [_vp, C.POINTER(_Dims)]),
+    "chd_phys_get_sizes": (_int, [_vp, _vp]),
+    "chd_phys_get_sizes_fixed": (_int, [_vp, _vp]),
+    "chd_phys_get_x": (_int, [_vp, _vp]),
+    "chd_phys_set_x": (_int, [_vp, _vp]),
+    "chd_phys_eval": (_int, [_vp, _i32, _vp, _vp, _vp, _vp]),
+    "chd_phys_get_layout": (_int, [_vp] * 8),
+    "chd_phys_get_slot_index": (_int, [_vp] * 4),
+    "chd_phys_get_ent_col": (_int, [_vp, _vp]),
+    "chd_phys_get_duals": (_int, [_vp] * 7),
+    "chd_phys_stage_stats": (_int, [_vp, _vp]),
+    "chd_phys_solve_stage": (_int, [_vp, _i32, _i32, _vp, _vp, _vp]),
+    "chd_phys_solve": (_int, [_vp] * 6),
+    "chd_phys_sample": (_int, [_vp, _vp, _vp]),
+    "chd_phys_sample_device": (_int, [_vp, _vp, _vp]),
+    "chd_phys_launch_count": (_i64, [_vp]),
+    "chd_phys_h2d_bytes": (_i64, [_vp]),
+    "chd_phys_reset": (_int, [_vp]),
+    "chd_phys_kernel_times": (_int, [_vp, _vp, _vp, _int]),
+    "chd_phys_set_timing": (_int, [_vp, _int]),
+    "chd_contact_create": (_int, [_vp, _vp, _vp, C.c_float, _i32, C.POINTER(_vp)]),
+    "chd_contact_destroy": (None, [_vp]),
+    "chd_contact_forward": (_int, [_vp, _vp, _i32, _i32, _vp, _vp, _vp, _vp]),
+    "chd_contact_forward_device": (_int, [_vp, _vp, _i32, _i32, _vp, _vp, _vp, _vp, _vp]),
+    "chd_contact_preprocess": (_int, [_vp, _vp, _vp, _i32, _i32, _vp, _vp]),
+    "chd_contact_detect": (_int, [_vp, _vp, _vp, _i32, _i32, _vp, _vp]),
+    "chd_contact_launch_count": (_i64, [_vp]),
+    "chd_contact_set_precision": (_int, [_vp, _i32]),
+    "chd_openpose_load": (_int, [C.POINTER(C.c_char_p), _i32, _i32, _vp, _i32]),
+    "chd_kin_solve": (_int, [_vp] * 7 + [_i32] * 3 + [_vp] * 4),
+    "chd_kin_work_bytes": (_i64, [_i32]),
+    "chd_ik_solve": (_int, [_i32, _vp, _i32, _vp, _vp, _i32, _i32, _vp, _vp, _vp, _i32, _f64, _f64, _i32, _vp, _vp]),
+    "chd_ik_work_bytes": (_i64, [_i32] * 3),
+    "chd_version": (C.c_char_p, []),
+    "chd_measure_fp64_peak": (_int, [C.POINTER(_f64), C.POINTER(_f64)]),
+}
 
 
 def measure_fp64_peak():
@@ -80,43 +118,9 @@ def load_lib():
         if not os.path.exists(path):
             raise RuntimeError("libchd.so is missing (%s): run `python -c 'import __graft_entry__ as g; g.build()'`" % path)
         L = C.CDLL(path)
-        L.chd_version.restype = C.c_char_p
-        L.chd_phys_launch_count.restype = C.c_int64
-        L.chd_phys_batch_create.argtypes = [C.POINTER(_Problem), C.c_int32, C.POINTER(_Weights), C.c_int32,
-                                            C.POINTER(C.c_void_p)]
-        L.chd_phys_batch_create_ex.argtypes = [C.POINTER(_Problem), C.c_int32, C.POINTER(_Weights), C.c_int32,
-                                               C.POINTER(_Options), C.POINTER(C.c_void_p)]
-        L.chd_phys_batch_destroy.argtypes = [C.c_void_p]
-        L.chd_phys_batch_destroy.restype = None
-        vp = C.c_void_p
-        L.chd_phys_get_dims.argtypes = [vp, C.POINTER(_Dims)]
-        L.chd_phys_get_sizes.argtypes = [vp, vp]
-        L.chd_phys_get_x.argtypes = [vp, vp]
-        L.chd_phys_set_x.argtypes = [vp, vp]
-        L.chd_phys_eval.argtypes = [vp, C.c_int32, vp, vp, vp, vp]
-        L.chd_phys_get_layout.argtypes = [vp] * 8
-        L.chd_phys_solve_stage.argtypes = [vp, C.c_int32, C.c_int32, vp, vp, vp]
-        L.chd_phys_solve.argtypes = [vp] * 6
-        L.chd_phys_sample.argtypes = [vp, vp, vp]
-        L.chd_phys_sample_device.argtypes = [vp, vp, vp]
-        L.chd_phys_launch_count.argtypes = [vp]
-        L.chd_phys_kernel_times.argtypes = [vp, vp, vp, C.c_int]
-        L.chd_phys_set_timing.argtypes = [vp, C.c_int]
-        L.chd_phys_h2d_bytes.argtypes = [vp]
-        L.chd_phys_h2d_bytes.restype = C.c_int64
-        L.chd_phys_reset.argtypes = [vp]
-        L.chd_phys_get_ent_col.argtypes = [vp, vp]
-        L.chd_phys_get_duals.argtypes = [vp] * 7
-        L.chd_phys_stage_stats.argtypes = [vp, vp]
-        L.chd_phys_get_sizes_fixed.argtypes = [vp, vp]
-        L.chd_phys_get_slot_index.argtypes = [vp] * 4
-        L.chd_kin_solve.argtypes = [vp] * 7 + [C.c_int32] * 3 + [vp] * 4
-        L.chd_kin_work_bytes.argtypes = [C.c_int32]
-        L.chd_kin_work_bytes.restype = C.c_int64
-        i32 = C.c_int32
-        L.chd_ik_solve.argtypes = [i32, vp, i32, vp, vp, i32, i32, vp, vp, vp, i32, C.c_double, C.c_double, i32, vp, vp]
-        L.chd_ik_work_bytes.argtypes = [i32] * 3
-        L.chd_ik_work_bytes.restype = C.c_int64
+        for name, (restype, argtypes) in SIGNATURES.items():
+            fn = getattr(L, name)
+            fn.restype, fn.argtypes = restype, argtypes
         _LIB = L
     return _LIB
 
@@ -171,11 +175,9 @@ class PhysBatch:
         w = _Weights(*[float(x) for x in weights])
         h = C.c_void_p()
         dev = -2 if host_only else device
-        if stage3_band_above is None:
-            rc = self.L.chd_phys_batch_create(arr, B, C.byref(w), dev, C.byref(h))
-        else:   # values outside 0..96 are rejected by the library (code -1)
-            opt = _Options(int(stage3_band_above))
-            rc = self.L.chd_phys_batch_create_ex(arr, B, C.byref(w), dev, C.byref(opt), C.byref(h))
+        # values outside 0..96 are rejected by the library (code -1)
+        opt = None if stage3_band_above is None else C.byref(_Options(int(stage3_band_above)))
+        rc = self.L.chd_phys_batch_create(arr, B, C.byref(w), dev, opt, C.byref(h))
         if rc != 0:
             raise RuntimeError("chd_phys_batch_create failed with code %d (no CUDA device? no CPU fallback exists)" % rc)
         self.h = h

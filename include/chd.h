@@ -58,21 +58,19 @@ typedef struct chd_phys_dims {
   int32_t batch, n_max, m_max, slots_max, n_splines, p_max, sets_max, na_max, nb_max, w_max, frames_out_max;
 } chd_phys_dims;
 
-/* Builds the NLP layouts of `batch` sequences on the host and uploads them to the current CUDA device.
- * device < 0 keeps the current device. */
-int chd_phys_batch_create(const chd_phys_problem* problems, int32_t batch, const chd_phys_weights* weights,
-                          int32_t device, chd_phys_batch** out);
-/* Layout options of chd_phys_batch_create_ex.
+/* Layout options of chd_phys_batch_create.
  *   stage3_band_above: a sequence with more phase-duration variables than this carries its switch times as banded
  *   KKT unknowns (time ordered with the node values) instead of dense border unknowns, which lifts the limit of 96
- *   that stage 3 otherwise has.  -1: no sequence (what chd_phys_batch_create does); 0 .. 96 otherwise.  A banded
- *   sequence whose band would be too wide for the KKT kernels keeps stage 3 off (status -3). */
+ *   that stage 3 otherwise has.  -1: no sequence (the default); 0 .. 96 otherwise.  A banded sequence whose band would
+ *   be too wide for the KKT kernels keeps stage 3 off (status -3). */
 typedef struct chd_phys_options {
   int32_t stage3_band_above;
 } chd_phys_options;
-/* chd_phys_batch_create with options (opt may be NULL: the defaults).  Returns -1 for an option out of range. */
-int chd_phys_batch_create_ex(const chd_phys_problem* problems, int32_t batch, const chd_phys_weights* weights,
-                             int32_t device, const chd_phys_options* opt, chd_phys_batch** out);
+/* Builds the NLP layouts of `batch` sequences on the host and uploads them to the current CUDA device.
+ * device < 0 keeps the current device.  weights and opt may be NULL: the defaults.  Returns -1 for a bad argument or an
+ * option out of range. */
+int chd_phys_batch_create(const chd_phys_problem* problems, int32_t batch, const chd_phys_weights* weights,
+                          int32_t device, const chd_phys_options* opt, chd_phys_batch** out);
 void chd_phys_batch_destroy(chd_phys_batch* b);
 int chd_phys_get_dims(const chd_phys_batch* b, chd_phys_dims* dims);
 /* Per-sequence sizes: n (variables: node values, then the P-1 free phase durations of every foot), m (master rows),

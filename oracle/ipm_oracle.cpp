@@ -1,6 +1,6 @@
 // TEST INFRASTRUCTURE ONLY -- CPU oracle of the interior-point loop ("chd-ipm", DESIGN.md section IPM).
 //
-// Single-threaded C++ restatement of oracle/ipm_proto.py: IPOPT's primal-dual barrier framework (slack
+// Single-threaded C++ statement of the interior-point algorithm the CUDA solver runs: IPOPT's primal-dual barrier framework (slack
 // reformulation, fraction-to-the-boundary, monotone barrier update, scaled optimality error and
 // termination test of phys_optim.cpp:568-578's options, gradient-based scaling) with a Gauss-Newton
 // Hessian model, Levenberg-Marquardt regularisation and a filter line search without restoration.

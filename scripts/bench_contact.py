@@ -9,7 +9,6 @@ e2e   : windows/s through the public host call `ContactNet.detect` (`chd_contact
 --dump-outputs DIR : labels and logits of the last timed device-resident step as DIR/<name>.npy (float32)
 """
 import argparse
-import ctypes as C
 import json
 import os
 import sys
@@ -89,7 +88,6 @@ def main():
     e2e = float(np.mean(te))
     # ---- device resident ----
     L = net.L
-    L.chd_contact_forward_device.argtypes = [C.c_void_p] * 2 + [C.c_int32] * 2 + [C.c_void_p] * 5
     frames, lens = net.preprocess(raw)
     fr, sl = torch.from_numpy(frames).cuda(), torch.from_numpy(lens).cuda()
     lab = torch.empty((V, F, 4), dtype=torch.int64, device="cuda")

@@ -12,7 +12,6 @@ window of the three large layers), max |logit difference|, the fraction of video
 and the smallest |fp32 logit| of each video whose labels differ.
 """
 import argparse
-import ctypes as C
 import json
 import os
 import subprocess
@@ -73,7 +72,6 @@ def main():
                torch.empty(1, dtype=torch.float32, device="cuda")) for m in MODES}
     st = torch.cuda.current_stream().cuda_stream
     fwd = nets["fp32"].L.chd_contact_forward_device
-    fwd.argtypes = [C.c_void_p] * 2 + [C.c_int32] * 2 + [C.c_void_p] * 5
 
     def device_step(m):
         lab, lg, mn = out[m]

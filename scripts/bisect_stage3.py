@@ -28,10 +28,4 @@ for k in ks:
     d = np.abs(xg - xo)
     top = np.argsort(-d)[:6]
     print("     largest |x_gpu - x_oracle|:", [(int(i), names[int(np.searchsorted(offs, i, side="right") - 1)], "%.3e" % d[i], "%.6g" % xg[i], "%.6g" % xo[i]) for i in top])
-    import ctypes as C
-    dbg = np.zeros(16)
-    b.L.chd_phys_debug_ipm.argtypes = [C.c_void_p, C.c_int32, C.c_void_p]
-    b.L.chd_phys_debug_ipm(b.h, 0, dbg.ctypes.data)
-    print("     gpu last KKT: a_pr %.6e a_du %.6e dphi %.6e phi0 %.9e theta0 %.6e theta_ref %.6e" % tuple(dbg[:6]))
-    print("     gpu last line search: alpha %.6e ls %d theta_t %.6e phi_t %.9e guard refusals %d trust refusals %d" % (dbg[8], dbg[9], dbg[10], dbg[11], dbg[12], dbg[13]))
     b.close()

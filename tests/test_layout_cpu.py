@@ -1,9 +1,15 @@
 """CPU tests of the host-side NLP layout (chd_layout.cpp, reached through the C ABI in host-only mode)
 against the oracle's independent TOWR-style construction."""
+import os
+import re
+import subprocess
+
 import numpy as np
 import pytest
 
 from tests.util import master_to_oracle_perm
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 @pytest.mark.parametrize("n_ee,seed", [(2, 0), (2, 3), (4, 1)])
@@ -71,16 +77,44 @@ def test_ragged_batch_padding(chd):
         np.testing.assert_array_equal(s.get_x()[0, :n], b.get_x()[i, :n])
 
 
-def test_library_exports(chd):
-    import ctypes
-    L = ctypes.CDLL(chd.phys.lib_path())
-    for name in chd.phys.EXPORTS:
-        assert hasattr(L, name), name
-    hdr = open(chd.phys.lib_path().replace("contact-human-dynamics_b200/libchd.so", "include/chd.h")).read()
-    import re
-    declared = set(re.findall(r"\b(chd_[a-z_0-9]+)\s*\(", hdr))
-    for name in declared:
-        assert hasattr(L, name), "declared in include/chd.h but not exported: " + name
+def _header_prototypes(path):
+    """{name: (return type, [parameter types])} of every chd_ function a C header declares."""
+    src = re.sub(r"/\*.*?\*/|//[^\n]*", " ", open(path).read(), flags=re.S)
+    src = "\n".join(l for l in src.splitlines() if not l.lstrip().startswith("#"))
+    out = {}
+    for stmt in src.split(";"):
+        stmt = " ".join(re.split(r"[{}]", stmt)[-1].split())
+        m = re.fullmatch(r"(.+?)\s*\b(chd_\w+)\s*\((.*)\)", stmt)
+        if m:
+            params = m.group(3).strip()
+            out[m.group(2)] = (m.group(1).replace(" *", "*"),
+                               [] if params in ("", "void") else [re.sub(r"\w+$", "", p).strip() for p in params.split(",")])
+    return out
+
+
+def test_binding_table_matches_header_and_exports(chd):
+    """include/chd.h, the ctypes table of phys.py and the dynamic symbols of libchd.so agree: the same functions, and
+    each declared to ctypes with the header's return type and parameter list."""
+    import ctypes as C
+    proto = _header_prototypes(os.path.join(ROOT, "include", "chd.h"))
+    table = chd.phys.SIGNATURES
+    assert set(proto) == set(table), (sorted(set(proto) - set(table)), sorted(set(table) - set(proto)))
+    scalar = {"int32_t": C.c_int32, "int64_t": C.c_int64, "int": C.c_int, "double": C.c_double, "float": C.c_float}
+    ret = {"int": C.c_int, "int64_t": C.c_int64, "const char*": C.c_char_p, "void": None}
+    for name, (rtype, params) in proto.items():
+        restype, argtypes = table[name]
+        assert restype is ret[rtype], (name, rtype, restype)
+        assert len(argtypes) == len(params), (name, params, argtypes)
+        for p, a in zip(params, argtypes):
+            if "*" in p:
+                assert a in (C.c_void_p, C.c_char_p) or issubclass(a, C._Pointer), (name, p, a)
+            else:
+                assert a is scalar[p.replace("const ", "")], (name, p, a)
+    chd.phys.load_lib()          # applies the table: every declared function resolves
+    nm = subprocess.run(["nm", "-D", "--defined-only", chd.phys.lib_path()], check=True, capture_output=True, text=True)
+    exported = {w[-1] for w in map(str.split, nm.stdout.splitlines()) if w and re.fullmatch(r"chd_\w+", w[-1])}
+    assert exported == set(proto), ("exported, not declared", sorted(exported - set(proto)),
+                                    "declared, not exported", sorted(set(proto) - exported))
 
 
 def test_column_oriented_slot_index(chd):

@@ -1,4 +1,4 @@
-"""CPU tests of banded switch times (`PhysBatch(stage3_band_above=...)`, `chd_phys_batch_create_ex`): host-only layouts.
+"""CPU tests of banded switch times (`PhysBatch(stage3_band_above=...)`, `chd_phys_options`): host-only layouts.
 
 Default layouts must not change; banded ones must put every switch time into the time-ordered band and size the band
 for every coupling stage 3 can produce, which is recomputed here from the problem's phase table and the oracle's row
@@ -31,7 +31,7 @@ def _problems(chd):
 
 @pytest.mark.parametrize("name", ["walk2", "dense150", "dense600"])
 def test_option_unset_keeps_layout(chd, name):
-    """-1 (and, for batches without more than 96 phase durations, 96) gives exactly chd_phys_batch_create's tables."""
+    """-1 (and, for batches without more than 96 phase durations, 96) gives exactly the tables of chd_phys_batch_create without options."""
     ps = _problems(chd)[name]
     ref = _tables(chd.phys.PhysBatch(ps, host_only=True))
     values = [-1] + ([96] if all(sum(len(d) - 1 for d in p.ee_durations) <= 96 for p in ps) else [])
@@ -128,14 +128,22 @@ def test_small_counts_banded_on_request(chd):
     np.testing.assert_array_equal(b.get_x(), ref.get_x())
 
 
-@pytest.mark.parametrize("value", [-2, 97, 1000, -(2 ** 31)])
-def test_out_of_range_option_rejected(chd, value):
+@pytest.mark.parametrize("value", [-2, 97, 1000, -(2 ** 31), None, -1, 0, 96])
+def test_create_option_range(chd, value):
+    """chd_phys_batch_create takes a NULL option pointer (the defaults) or stage3_band_above in -1 .. 96; any other value
+    returns -1 and no batch, through the C call and through PhysBatch."""
     ps = [chd.synth.make_problem(0, n_ee=2)]
     L = chd.phys.load_lib()
     arr, keep = chd.phys.make_problem_array(ps)
-    opt = chd.phys._Options(value)
+    opt = None if value is None else C.byref(chd.phys._Options(value))
     h = C.c_void_p()
-    assert L.chd_phys_batch_create_ex(arr, 1, None, -2, C.byref(opt), C.byref(h)) == -1
+    if value is None or -1 <= value <= 96:
+        assert L.chd_phys_batch_create(arr, 1, None, -2, opt, C.byref(h)) == 0
+        assert h.value
+        L.chd_phys_batch_destroy(h)
+        chd.phys.PhysBatch(ps, host_only=True, stage3_band_above=value).close()
+        return
+    assert L.chd_phys_batch_create(arr, 1, None, -2, opt, C.byref(h)) == -1
     assert not h.value
     with pytest.raises(RuntimeError):
         chd.phys.PhysBatch(ps, host_only=True, stage3_band_above=value)
