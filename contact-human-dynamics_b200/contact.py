@@ -4,12 +4,15 @@ src/contact_learning/test.py --full-video --save-contacts --real-data).
 Keypoint loading (JSON) happens on the host; the dataset preprocessing (padding, scaling, low-confidence
 interpolation, normalisation: real_video_dataset.py:132-163, openpose_dataset.py:49-121), window construction, the MLP
 and the vote aggregation run in hand-written CUDA behind `chd_contact_*` (include/chd.h).  No CPU fallback.
+With ground truth (test.py --full-video on labelled videos or on the synthetic dataset's test split) `ContactNet.evaluate`
+also scores the windows on the device (`chd_contact_evaluate`); `read_real_videos` / `read_synthetic_videos` read the two
+dataset layouts.
 """
 from __future__ import annotations
 
 import ctypes as C
 import os
-from typing import Dict, List, Sequence
+from typing import Dict, List, NamedTuple, Optional, Sequence
 
 import numpy as np
 
@@ -20,6 +23,11 @@ TRAIN_NORMALIZATION = 200.4160302695367      # real_video_dataset.py:18
 WINDOW, PRED = 9, 5
 LIN_IDS, BN_IDS = [0, 3, 6, 10, 13], [1, 4, 7, 11]
 DIMS = [351, 1024, 512, 128, 32, 20]
+
+
+def video_scale(dimensions=(1920, 1080)) -> float:
+    """xy factor of real videos, TRAIN_DIM[0] / dimensions[0] (real_video_dataset.py:149)."""
+    return float(TRAIN_DIM[0]) / dimensions[0]
 
 
 def load_keypoint_files(files: Sequence[str], num_joints: int = 25, threads: int = 0) -> np.ndarray:
@@ -145,14 +153,17 @@ class ContactNet:
             raise RuntimeError("chd_contact_forward failed with code %d" % rc)
         return (labels, logits, float(mabs[0])) if want_logits else (labels, float(mabs[0]))
 
-    def preprocess(self, raw: Sequence[np.ndarray], dimensions=(1920, 1080)):
-        """RealVideoDataset.__init__ on the device (`chd_contact_preprocess`): list of raw (F_i,25,3) keypoints ->
-        (frames (V,Fmax,25,3) fp64, seq_lens (V,) int32), bit identical to the reference's numpy result."""
+    def preprocess(self, raw: Sequence[np.ndarray], dimensions=(1920, 1080), scale: Optional[float] = None, norm: float = TRAIN_NORMALIZATION):
+        """RealVideoDataset.__init__ on the device (`chd_contact_preprocess_scaled`): list of raw (F_i,25,3) keypoints ->
+        (frames (V,Fmax,25,3) fp64, seq_lens (V,) int32), bit identical to the reference's numpy result.  `scale`
+        (default 1280 / dimensions[0]) and `norm` are the dataset's constants; `SyntheticVideos` carries its own."""
         cat, offs = concat_videos(raw)
         V, Fmax = len(raw), int(np.diff(offs).max())
         frames = np.zeros((V, Fmax, 25, 3))
         lens = np.zeros(V, dtype=np.int32)
-        rc = self.L.chd_contact_preprocess(self.h, cat.ctypes.data, offs.ctypes.data, V, int(dimensions[0]), frames.ctypes.data, lens.ctypes.data)
+        scale = video_scale(dimensions) if scale is None else scale
+        rc = self.L.chd_contact_preprocess_scaled(self.h, cat.ctypes.data, offs.ctypes.data, V, float(scale), float(norm), frames.ctypes.data,
+                                                  lens.ctypes.data)
         if rc != 0:
             raise RuntimeError("chd_contact_preprocess failed with code %d" % rc)
         return frames, lens
@@ -171,8 +182,167 @@ class ContactNet:
             raise RuntimeError("chd_contact_detect failed with code %d" % rc)
         return [lab[offs[i]:offs[i + 1]] for i in range(V)], float(mabs[0])
 
+    def evaluate(self, raw: Sequence[np.ndarray], truth: Sequence[Optional[np.ndarray]], scale: float, norm: float,
+                 classify_thresh: float = 0.5, cat=None, offs=None) -> Dict:
+        """test.py --full-video with ground truth (`chd_contact_evaluate`: preprocessing with `scale` / `norm`, windows,
+        network, votes and scoring on the device; one upload, one download).  truth[i]: (T_i,4) contacts of video i (any
+        length: padded with the last row or trimmed to the longest video, as fix_data_len does) or None.  Returns a dict:
+          labels       list of (F_i,4) int64, what `detect` returns
+          loss_sum     (V,) sum of the BCE-with-logits terms of every window of a labelled video
+          conf_frames  (V,5,4) (tp, fp, fn, tn) of each predicted frame, sigmoid(x) > classify_thresh
+          conf_merged  (V,4) (tp, fp, fn, tn) of the 0.5-vote labels over all frames of the padded video
+          frames_total (5,4), merged_total (4,): the sums over the videos
+          labelled, windows, loss_count: labelled videos, windows per video, terms in the mean loss
+          mean_loss    loss_sum.sum() / loss_count (test.py:84-85, 214), None without labelled videos
+          min_abs_logit"""
+        if cat is None:
+            cat, offs = concat_videos(raw)
+        V = len(offs) - 1
+        if len(truth) != V:
+            raise ValueError("evaluate: %d videos but %d truth entries" % (V, len(truth)))
+        rows = [np.zeros((0, 4), dtype=np.int32) if t is None else np.asarray(t).reshape(-1, 4) for t in truth]
+        toffs = np.zeros(V + 1, dtype=np.int32)
+        toffs[1:] = np.cumsum([r.shape[0] for r in rows])
+        tcat = np.ascontiguousarray(np.concatenate(rows, axis=0) != 0, dtype=np.int32) if toffs[-1] else np.zeros((1, 4), dtype=np.int32)
+        lab = np.zeros((int(offs[-1]), 4), dtype=np.int64)
+        loss = np.zeros(V, dtype=np.float64)
+        cf = np.zeros((V, PRED, 4), dtype=np.int64)
+        cm = np.zeros((V, 4), dtype=np.int64)
+        mabs = np.zeros(1, dtype=np.float32)
+        rc = self.L.chd_contact_evaluate(self.h, cat.ctypes.data, offs.ctypes.data, V, float(scale), float(norm), tcat.ctypes.data, toffs.ctypes.data,
+                                         C.c_float(classify_thresh), lab.ctypes.data, loss.ctypes.data, cf.ctypes.data, cm.ctypes.data, mabs.ctypes.data)
+        if rc != 0:
+            raise RuntimeError("chd_contact_evaluate failed with code %d" % rc)
+        windows = int(np.diff(offs).max()) - (WINDOW - 1)
+        labelled = int((np.diff(toffs) > 0).sum())
+        count = PRED * 4 * windows * labelled
+        return dict(labels=[lab[offs[i]:offs[i + 1]] for i in range(V)], loss_sum=loss, conf_frames=cf, conf_merged=cm,
+                    frames_total=cf.sum(0), merged_total=cm.sum(0), labelled=labelled, windows=windows, loss_count=count,
+                    mean_loss=float(loss.sum() / count) if count else None, min_abs_logit=float(mabs[0]))
+
     def launch_count(self) -> int:
         return int(self.L.chd_contact_launch_count(self.h))
+
+
+class Videos(NamedTuple):
+    """A dataset read for the classifier: names, raw keypoints (F_i,25,3), ground truth (T_i,4) or None per video, and
+    the preprocessing constants (`ContactNet.preprocess` / `.evaluate`)."""
+    names: List[str]
+    raw: List[np.ndarray]
+    truth: List[Optional[np.ndarray]]
+    scale: float
+    norm: float
+
+
+def _subdirs(path: str, prefix: str = "") -> List[str]:
+    """contact_data_utils.py / real_video_dataset.py:72: sorted directories, hidden ones skipped."""
+    return sorted(d for d in os.listdir(path) if os.path.isdir(os.path.join(path, d)) and d[0] != "." and d.startswith(prefix))
+
+
+def read_real_videos(data_root: str, dimensions=(1920, 1080)) -> Videos:
+    """RealVideoDataset's inputs (real_video_dataset.py:72-120): every video directory of `data_root` with its
+    `openpose_result/` and, when present, its `foot_contacts.npy`."""
+    vids = _subdirs(data_root)
+    raw = load_keypoint_dirs([os.path.join(data_root, v, "openpose_result") for v in vids])
+    truth = []
+    for v in vids:
+        p = os.path.join(data_root, v, "foot_contacts.npy")
+        truth.append(np.load(p) if os.path.exists(p) else None)
+    return Videos(vids, raw, truth, video_scale(dimensions), TRAIN_NORMALIZATION)
+
+
+def data_layout(data_root: str) -> str:
+    """"real" when a video directory of `data_root` has an `openpose_result/`, "synthetic" when a
+    `<character>/<motion>/view*` directory exists; ValueError otherwise."""
+    subs = _subdirs(data_root)
+    if any(os.path.isdir(os.path.join(data_root, s, "openpose_result")) for s in subs):
+        return "real"
+    for s in subs:
+        for m in _subdirs(os.path.join(data_root, s)):
+            if _subdirs(os.path.join(data_root, s, m), "view"):
+                return "synthetic"
+    raise ValueError("%s holds neither real videos (<video>/openpose_result/) nor the synthetic dataset "
+                     "(<character>/<motion>/view<k>/)" % data_root)
+
+
+SPLITS = ("train", "test", "val")
+
+
+def synthetic_splits(n_characters: int, n_motions: int, n_views: int, train_frac: float = 0.8) -> Dict[str, List[int]]:
+    """OpenPoseDataset's split (openpose_dataset.py:214-238): the motions of each character in turn are shuffled by one
+    stream seeded with 0 (np.random.seed(0) + np.random.shuffle, here a RandomState(0)), the first 80 % train, then half
+    of the rest test, the remainder val; every view of a motion follows it.  Global sequence indices (character-major,
+    then motion, then view) in the reference's order."""
+    rs = np.random.RandomState(0)
+    out = {k: [] for k in SPLITS}
+    for c in range(n_characters):
+        inds = np.arange(n_motions)
+        rs.shuffle(inds)
+        ntr = int(train_frac * n_motions)
+        nte = (n_motions - ntr) // 2
+        for k, part in zip(SPLITS, (inds[:ntr], inds[ntr:ntr + nte], inds[ntr + nte:])):
+            for m in part:
+                g = (c * n_motions + int(m)) * n_views
+                out[k] += range(g, g + n_views)
+    return out
+
+
+class SyntheticVideos(NamedTuple):
+    """`read_synthetic_videos`: the videos of one split plus what the split and the normalisation were made from."""
+    videos: Videos
+    splits: Dict[str, List[int]]          # global sequence indices of train / test / val
+    all_names: List[str]                  # "<character>/<motion>/view<k>" of every sequence, global order
+    median: float
+    num_frames: int
+
+
+def read_synthetic_videos(data_root: str, split: str = "test") -> SyntheticVideos:
+    """OpenPoseDataset(data_root, split, overlap_test=True) (openpose_dataset.py:126-269) up to the preprocessing: sorted
+    character / motion / view directories, the frame count from the `*.png` of the first view, one foot_contacts.npy per
+    motion shared by its views, the seeded split, and as `norm` the median MidHip -> LBigToe distance over the raw
+    keypoints of every sequence of every split (:212, :368-382).  `scale` is 1: no padding, no 1280 scaling.  Raises
+    ValueError for a tree whose characters differ in motion count, whose motions differ in view count, or a sequence whose
+    keypoint count differs from the frame count (the reference assumes all three)."""
+    if split not in SPLITS:
+        raise ValueError("split must be one of %s" % ", ".join(SPLITS))
+    chars = _subdirs(data_root)
+    if not chars:
+        raise ValueError("no character directories under %s" % data_root)
+    motions = [[os.path.join(data_root, c, m) for m in _subdirs(os.path.join(data_root, c))] for c in chars]
+    if not motions[0] or any(len(m) != len(motions[0]) for m in motions):
+        raise ValueError("every character of %s must hold the same number of motions" % data_root)
+    mdirs = [m for ms in motions for m in ms]
+    views = [_subdirs(m, "view") for m in mdirs]
+    if not views[0] or any(len(v) != len(views[0]) for v in views):
+        raise ValueError("every motion of %s must hold the same number of view directories" % data_root)
+    v0 = os.path.join(mdirs[0], views[0][0])
+    num_frames = len([f for f in os.listdir(v0) if f[0] != "." and f.split(".")[-1] == "png"])
+    names, kdirs, cpaths = [], [], []
+    for m, vs in zip(mdirs, views):
+        for v in vs:
+            names.append("/".join(os.path.normpath(os.path.join(m, v)).split(os.sep)[-3:]))
+            kdirs.append(os.path.join(m, "keypoints_" + v))
+            cpaths.append(os.path.join(m, "foot_contacts.npy"))
+    raw = load_keypoint_dirs(kdirs)
+    for n, r in zip(names, raw):
+        if r.shape[0] != num_frames:
+            raise ValueError("%s: %d keypoint files but %d frames (*.png in %s)" % (n, r.shape[0], num_frames, v0))
+    dists = np.concatenate([np.linalg.norm(r[:, 8, :2] - r[:, 19, :2], axis=1) for r in raw])    # MidHip, LBigToe
+    median = float(np.median(dists))
+    splits = synthetic_splits(len(chars), len(motions[0]), len(views[0]))
+    sel = splits[split]
+    truth = {p: np.load(p) for p in set(cpaths[i] for i in sel) if os.path.exists(p)}
+    vids = Videos([names[i] for i in sel], [raw[i] for i in sel], [truth.get(cpaths[i]) for i in sel], 1.0, median)
+    return SyntheticVideos(vids, splits, names, median, num_frames)
+
+
+def read_videos(data_root: str, real_data: bool = False, dimensions=(1920, 1080)):
+    """What test.py --full-video reads: (layout, Videos).  `real_data` or a root in the real-video layout -> every video
+    (`read_real_videos`); otherwise the test split of the synthetic dataset (`read_synthetic_videos`)."""
+    layout = "real" if real_data else data_layout(data_root)
+    if layout == "real":
+        return layout, read_real_videos(data_root, dimensions)
+    return layout, read_synthetic_videos(data_root, "test").videos
 
 
 def detect_contacts(data_root: str, out_root: str, state_dict, dimensions=(1920, 1080), precision: str = "fp32") -> List[str]:
@@ -180,14 +350,18 @@ def detect_contacts(data_root: str, out_root: str, state_dict, dimensions=(1920,
     `openpose_result/` writes O/contact_results/<video>/foot_contacts.npy (int64, F x 4), test.py:143-152.
     `precision`: numerical mode of the network (see `ContactNet`)."""
     precision_code(precision)
-    vids = sorted(d for d in os.listdir(data_root) if os.path.isdir(os.path.join(data_root, d)) and d[0] != ".")
-    raw = load_keypoint_dirs([os.path.join(data_root, v, "openpose_result") for v in vids])
+    vids = read_real_videos(data_root, dimensions)
     net = ContactNet(state_dict, precision=precision)
-    labels, _ = net.detect(raw, dimensions)
+    labels, _ = net.detect(vids.raw, dimensions)
+    return save_contacts(out_root, vids.names, labels)
+
+
+def save_contacts(out_root: str, names: Sequence[str], labels: Sequence[np.ndarray]) -> List[str]:
+    """out_root/contact_results/<name>/foot_contacts.npy (int64, F x 4) per video, test.py:143-152."""
     written = []
-    for i, v in enumerate(vids):
-        od = os.path.join(out_root, "contact_results", v)
+    for n, lab in zip(names, labels):
+        od = os.path.join(out_root, "contact_results", n)
         os.makedirs(od, exist_ok=True)
-        np.save(os.path.join(od, "foot_contacts"), labels[i].astype(np.int64))
+        np.save(os.path.join(od, "foot_contacts"), lab.astype(np.int64))
         written.append(os.path.join(od, "foot_contacts.npy"))
     return written

@@ -207,6 +207,90 @@ __global__ void chd_k_contact_vote(const float* __restrict__ logits, int V, int 
   if ((threadIdx.x & 31) == 0 && mabs < 3.0e38f) atomicMin(reinterpret_cast<int*>(min_abs), __float_as_int(mabs));  // positive floats order as ints
 }
 
+// Scores the logits of every window against ground-truth contacts (test.py:64-140 val_full_video with labels: the
+// OpenPoseModel.loss / .accuracy calls and the merged-label count).  One CTA per video, CT_SCORE_THREADS threads; a
+// multiple of 20 and of 4, so a thread always sees the same (predicted frame, contact) pair in the window pass and the
+// same contact in the frame pass and keeps four counters.  Video v's truth rows are truth[toffs[v] .. toffs[v+1]), padded
+// with their last row or trimmed to Fmax (fix_data_len, real_video_dataset.py:165-191); a video without rows gets zeros.
+//   loss_sum[v]          sum over windows x 5 x 4 of BCE-with-logits (1 - y) x - log_sigmoid(x), fp32 terms, fp64 sum
+//   conf_frames[v][p][.] (tp, fp, fn, tn) of sigmoid(x) > thresh against truth row w + 2 + p of window w
+//   conf_merged[v][.]    (tp, fp, fn, tn) over all Fmax x 4 of the 0.5 vote before trimming (recomputed: the vote kernel
+//                        zeroes rows >= seq_len) against truth row clamp(f, 2, Fmax - 3), test.py:124-140
+// Fixed-order reductions, no atomics: a video's outputs depend only on its own logits, truth and Fmax.
+#define CT_SCORE_THREADS 320
+__global__ void __launch_bounds__(CT_SCORE_THREADS) chd_k_contact_score(const float* __restrict__ logits, int Fmax, const int* __restrict__ truth,
+                                                                       const int* __restrict__ toffs, float thresh, double* __restrict__ loss_sum,
+                                                                       long long* __restrict__ conf_frames, long long* __restrict__ conf_merged) {
+  __shared__ int s_cnt[CT_SCORE_THREADS][4];
+  __shared__ double s_loss[CT_SCORE_THREADS / 32];
+  const int v = blockIdx.x, tid = threadIdx.x;
+  const int Wn = Fmax - (CT_WIN - 1), nv = Wn + 2 * (CT_PRED / 2), off = (CT_WIN - CT_PRED) / 2;
+  const int t0 = toffs[v], nrow = toffs[v + 1] - t0;
+  const float* lg = logits + (size_t)v * Wn * 20;
+  auto label = [&](int r, int c) { return truth[(size_t)(t0 + (r < nrow ? r : nrow - 1)) * 4 + c] != 0; };
+  // ---- per window: loss and per-frame counts; this thread's (p, c) = (tid % 20) / 4, tid % 4 ----
+  int cnt[4] = {0, 0, 0, 0};
+  double loss = 0.0;
+  if (nrow > 0) {
+    const int p = (tid % 20) / 4, c = tid % 4;
+    for (int i = tid; i < Wn * 20; i += CT_SCORE_THREADS) {
+      const float x = lg[i];
+      const bool y = label(i / 20 + off + p, c);
+      const float log_sig = fminf(x, 0.f) - log1pf(expf(-fabsf(x)));        // torch's log_sigmoid
+      loss += (double)((y ? 0.f : x) - log_sig);                               // (1 - y) * x - log_sigmoid(x)
+      const bool pred = 1.0f / (1.0f + expf(-x)) > thresh;                     // the vote kernel's predicate
+      ++cnt[pred ? (y ? 0 : 1) : (y ? 2 : 3)];
+    }
+  }
+  for (int q = 0; q < 4; ++q) s_cnt[tid][q] = cnt[q];
+  for (int o = 16; o > 0; o >>= 1) loss += __shfl_xor_sync(0xffffffffu, loss, o);
+  if ((tid & 31) == 0) s_loss[tid >> 5] = loss;
+  __syncthreads();
+  if (tid < CT_PRED * 4) {    // tid = (p, q): sum over the contacts c and the threads c + 4p, c + 4p + 20, ...
+    const int p = tid / 4, q = tid % 4;
+    long long sum = 0;
+    for (int c = 0; c < 4; ++c)
+      for (int t = p * 4 + c; t < CT_SCORE_THREADS; t += 20) sum += s_cnt[t][q];
+    conf_frames[(size_t)v * 20 + tid] = sum;
+  }
+  if (tid == 0) {
+    double s = 0.0;
+    for (int w = 0; w < CT_SCORE_THREADS / 32; ++w) s += s_loss[w];
+    loss_sum[v] = s;
+  }
+  __syncthreads();
+  // ---- per frame: merged counts ----
+  int mc[4] = {0, 0, 0, 0};
+  if (nrow > 0) {
+    for (int i = tid; i < Fmax * 4; i += CT_SCORE_THREADS) {
+      const int c = i & 3, f = i >> 2;
+      int fv = f - off;
+      fv = fv < 0 ? 0 : (fv >= nv ? nv - 1 : fv);
+      int votes = 0;
+      for (int p = 0; p < CT_PRED; ++p) {
+        const int w = fv - p;
+        if (w < 0 || w >= Wn) continue;
+        const float x = lg[w * 20 + p * 4 + c];
+        votes += 1.0f / (1.0f + expf(-x)) > 0.5f ? 1 : 0;
+      }
+      int th = (CT_PRED + 1) / 2;
+      const int e0 = fv, e1 = nv - 1 - fv;
+      if (e0 < CT_PRED - 1) th = e0 / 2 + 1;
+      if (e1 < CT_PRED - 1) th = e1 / 2 + 1;
+      const bool pred = votes >= th;
+      const bool y = label(f < off ? off : (f > Fmax - 1 - off ? Fmax - 1 - off : f), c);
+      ++mc[pred ? (y ? 0 : 1) : (y ? 2 : 3)];
+    }
+  }
+  for (int q = 0; q < 4; ++q) s_cnt[tid][q] = mc[q];
+  __syncthreads();
+  if (tid < 4) {              // count q over all threads (every contact)
+    long long sum = 0;
+    for (int t = 0; t < CT_SCORE_THREADS; ++t) sum += s_cnt[t][tid];
+    conf_merged[(size_t)v * 4 + tid] = sum;
+  }
+}
+
 struct chd_contact_net {
   std::vector<void*> allocs;
   ContactDev dev;
@@ -215,8 +299,8 @@ struct chd_contact_net {
   float* ws = nullptr;     // activation workspace of one slab: A0 [Mp][352] | A1 [Mp][1024] | A2 [Mp][512] | A3 [Mp][128]
   int ws_rows = 0;
   // grow-only device buffers of the host entry points (no allocation per call, nothing to leak on an error path)
-  void* io[8] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
-  size_t io_bytes[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+  void* io[11] = {};
+  size_t io_bytes[11] = {};
   // CHD_CONTACT_TF32X3: split weight planes (one allocation) and the slab workspace of the tensor-core layers
   int precision = CHD_CONTACT_FP32;
   ChdContactTcNet tc = {};
@@ -224,7 +308,9 @@ struct chd_contact_net {
   float* tc_ws = nullptr;
   int tc_ws_rows = 0;
 };
-enum { IO_FRAMES = 0, IO_LENS = 1, IO_LABELS = 2, IO_LOGITS = 3, IO_MIN = 4, IO_RAW = 5, IO_OFFS = 6, IO_PACKED = 7 };
+enum { IO_FRAMES = 0, IO_LENS = 1, IO_LABELS = 2, IO_LOGITS = 3, IO_MIN = 4, IO_RAW = 5, IO_OFFS = 6, IO_PACKED = 7, IO_TRUTH = 8, IO_TOFFS = 9,
+       IO_SCORE = 10, IO_COUNT = 11 };
+static_assert(sizeof(chd_contact_net::io) / sizeof(void*) == IO_COUNT, "one io slot per IO_* id");
 
 #define CT_CUDA(x)                                                                           \
   do {                                                                                       \
@@ -352,7 +438,7 @@ void chd_contact_destroy(chd_contact_net* net) {
   if (net->ws) cudaFree(net->ws);
   if (net->tc_w) cudaFree(net->tc_w);
   if (net->tc_ws) cudaFree(net->tc_ws);
-  for (int q = 0; q < 8; ++q)
+  for (int q = 0; q < IO_COUNT; ++q)
     if (net->io[q]) cudaFree(net->io[q]);
   if (net->stream) cudaStreamDestroy(net->stream);
   delete net;
@@ -435,8 +521,9 @@ int chd_contact_forward(chd_contact_net* net, const double* frames, int32_t V, i
   return 0;
 }
 
-// raw OpenPose keypoints -> preprocessed frames on the device (shared by chd_contact_preprocess / chd_contact_detect)
-static int ct_prep_device(chd_contact_net* net, const double* raw, const int32_t* offs, int32_t V, int32_t dim_w, int* Fmax_out) {
+// raw OpenPose keypoints -> preprocessed frames on the device (shared by the preprocess / detect / evaluate entries):
+// xy multiplied by `scale`, gaps interpolated, xy divided by `norm`
+static int ct_prep_device(chd_contact_net* net, const double* raw, const int32_t* offs, int32_t V, double scale, double norm, int* Fmax_out) {
   int Fmax = 0, total = offs[V];
   for (int v = 0; v < V; ++v) {
     if (offs[v + 1] <= offs[v]) return -1;
@@ -449,20 +536,23 @@ static int ct_prep_device(chd_contact_net* net, const double* raw, const int32_t
     return rc;
   CT_CUDA(cudaMemcpyAsync(net->io[IO_RAW], raw, (size_t)total * 75 * sizeof(double), cudaMemcpyHostToDevice, net->stream));
   CT_CUDA(cudaMemcpyAsync(net->io[IO_OFFS], offs, (V + 1) * sizeof(int), cudaMemcpyHostToDevice, net->stream));
-  const double scale = 1280.0 / dim_w;                       // TRAIN_DIM[0] / dimensions[0], real_video_dataset.py:17,149-155
   chd_k_contact_prep<<<(V * 25 + 127) / 128, 128, 0, net->stream>>>((const double*)net->io[IO_RAW], (const int*)net->io[IO_OFFS], V, Fmax, scale,
-                                                                    200.4160302695367, 0.2, (double*)net->io[IO_FRAMES], (int*)net->io[IO_LENS]);
+                                                                    norm, 0.2, (double*)net->io[IO_FRAMES], (int*)net->io[IO_LENS]);
   net->launches += 1;
   CT_CUDA(cudaGetLastError());
   *Fmax_out = Fmax;
   return 0;
 }
 
-int chd_contact_preprocess(chd_contact_net* net, const double* raw, const int32_t* seq_offsets, int32_t V, int32_t dim_w, double* frames_out,
-                           int32_t* seq_lens_out) {
-  if (!net || !raw || !seq_offsets || V <= 0 || dim_w <= 0 || !frames_out) return -1;
+// the real-video preprocessing: TRAIN_DIM[0] / dimensions[0] and the training normalisation, real_video_dataset.py:17-18,149-161
+static double ct_video_scale(int32_t dim_w) { return 1280.0 / dim_w; }
+static const double CT_TRAIN_NORMALIZATION = 200.4160302695367;
+
+int chd_contact_preprocess_scaled(chd_contact_net* net, const double* raw, const int32_t* seq_offsets, int32_t V, double scale, double norm,
+                                  double* frames_out, int32_t* seq_lens_out) {
+  if (!net || !raw || !seq_offsets || V <= 0 || !(scale > 0) || !(norm > 0) || !frames_out) return -1;
   int Fmax = 0;
-  int rc = ct_prep_device(net, raw, seq_offsets, V, dim_w, &Fmax);
+  int rc = ct_prep_device(net, raw, seq_offsets, V, scale, norm, &Fmax);
   if (rc) return rc;
   CT_CUDA(cudaMemcpyAsync(frames_out, net->io[IO_FRAMES], (size_t)V * Fmax * 75 * sizeof(double), cudaMemcpyDeviceToHost, net->stream));
   if (seq_lens_out) CT_CUDA(cudaMemcpyAsync(seq_lens_out, net->io[IO_LENS], V * sizeof(int), cudaMemcpyDeviceToHost, net->stream));
@@ -470,24 +560,90 @@ int chd_contact_preprocess(chd_contact_net* net, const double* raw, const int32_
   return 0;
 }
 
-int chd_contact_detect(chd_contact_net* net, const double* raw, const int32_t* seq_offsets, int32_t V, int32_t dim_w, int64_t* labels_out,
-                       float* min_abs_logit) {
-  if (!net || !raw || !seq_offsets || V <= 0 || dim_w <= 0 || !labels_out) return -1;
+int chd_contact_preprocess(chd_contact_net* net, const double* raw, const int32_t* seq_offsets, int32_t V, int32_t dim_w, double* frames_out,
+                           int32_t* seq_lens_out) {
+  if (dim_w <= 0) return -1;
+  return chd_contact_preprocess_scaled(net, raw, seq_offsets, V, ct_video_scale(dim_w), CT_TRAIN_NORMALIZATION, frames_out, seq_lens_out);
+}
+
+// prep + forward + vote of chd_contact_detect / chd_contact_evaluate on the net's stream; *Fmax_out = longest video
+static int ct_detect_device(chd_contact_net* net, const double* raw, const int32_t* seq_offsets, int32_t V, double scale, double norm, int* Fmax_out) {
   int Fmax = 0;
-  int rc = ct_prep_device(net, raw, seq_offsets, V, dim_w, &Fmax);
+  int rc = ct_prep_device(net, raw, seq_offsets, V, scale, norm, &Fmax);
   if (rc) return rc;
   const size_t total = seq_offsets[V], Wn = Fmax - (CT_WIN - 1), nlog = (size_t)V * Wn * 20, nlab = (size_t)V * Fmax * 4;
   if ((rc = ct_reserve(net, IO_LABELS, nlab * sizeof(long long))) || (rc = ct_reserve(net, IO_LOGITS, nlog * sizeof(float))) ||
       (rc = ct_reserve(net, IO_MIN, sizeof(float))) || (rc = ct_reserve(net, IO_PACKED, total * 4 * sizeof(long long))))
     return rc;
-  long long* d_lab = (long long*)net->io[IO_LABELS];
-  rc = chd_contact_forward_device(net, (const double*)net->io[IO_FRAMES], V, Fmax, (const int*)net->io[IO_LENS], (int64_t*)d_lab,
-                                  (float*)net->io[IO_LOGITS], (float*)net->io[IO_MIN], net->stream);
-  if (rc) return rc;
-  chd_k_contact_pack<<<dim3(4, V), 256, 0, net->stream>>>(d_lab, (const int*)net->io[IO_OFFS], V, Fmax, (long long*)net->io[IO_PACKED]);
+  *Fmax_out = Fmax;
+  return chd_contact_forward_device(net, (const double*)net->io[IO_FRAMES], V, Fmax, (const int*)net->io[IO_LENS], (int64_t*)net->io[IO_LABELS],
+                                    (float*)net->io[IO_LOGITS], (float*)net->io[IO_MIN], net->stream);
+}
+
+// (V, Fmax, 4) labels -> the packed rows on the device, then their download (and min |logit|) on the net's stream
+static int ct_pack_download(chd_contact_net* net, const int32_t* seq_offsets, int32_t V, int Fmax, int64_t* labels_out, float* min_abs_logit) {
+  const size_t total = seq_offsets[V];
+  chd_k_contact_pack<<<dim3(4, V), 256, 0, net->stream>>>((const long long*)net->io[IO_LABELS], (const int*)net->io[IO_OFFS], V, Fmax,
+                                                          (long long*)net->io[IO_PACKED]);
   net->launches += 1;
+  CT_CUDA(cudaGetLastError());
   CT_CUDA(cudaMemcpyAsync(labels_out, net->io[IO_PACKED], total * 4 * sizeof(long long), cudaMemcpyDeviceToHost, net->stream));
   if (min_abs_logit) CT_CUDA(cudaMemcpyAsync(min_abs_logit, net->io[IO_MIN], sizeof(float), cudaMemcpyDeviceToHost, net->stream));
+  return 0;
+}
+
+int chd_contact_detect(chd_contact_net* net, const double* raw, const int32_t* seq_offsets, int32_t V, int32_t dim_w, int64_t* labels_out,
+                       float* min_abs_logit) {
+  if (!net || !raw || !seq_offsets || V <= 0 || dim_w <= 0 || !labels_out) return -1;
+  int Fmax = 0, rc;
+  if ((rc = ct_detect_device(net, raw, seq_offsets, V, ct_video_scale(dim_w), CT_TRAIN_NORMALIZATION, &Fmax))) return rc;
+  if ((rc = ct_pack_download(net, seq_offsets, V, Fmax, labels_out, min_abs_logit))) return rc;
+  CT_CUDA(cudaStreamSynchronize(net->stream));
+  return 0;
+}
+
+int chd_contact_score_device(chd_contact_net* net, const float* logits_dev, int32_t V, int32_t Fmax, const int32_t* truth_dev,
+                             const int32_t* truth_offsets_dev, float classify_thresh, double* loss_sum_dev, int64_t* conf_frames_dev,
+                             int64_t* conf_merged_dev, void* stream) {
+  if (!net || !logits_dev || !truth_offsets_dev || !loss_sum_dev || !conf_frames_dev || !conf_merged_dev || V <= 0 || Fmax < CT_WIN) return -1;
+  cudaStream_t s = stream ? (cudaStream_t)stream : net->stream;
+  chd_k_contact_score<<<V, CT_SCORE_THREADS, 0, s>>>(logits_dev, Fmax, truth_dev, truth_offsets_dev, classify_thresh, loss_sum_dev,
+                                                     (long long*)conf_frames_dev, (long long*)conf_merged_dev);
+  net->launches += 1;
+  CT_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int chd_contact_evaluate(chd_contact_net* net, const double* raw, const int32_t* seq_offsets, int32_t V, double scale, double norm,
+                         const int32_t* truth, const int32_t* truth_offsets, float classify_thresh, int64_t* labels_out, double* loss_sum,
+                         int64_t* conf_frames, int64_t* conf_merged, float* min_abs_logit) {
+  if (!net || !raw || !seq_offsets || V <= 0 || !(scale > 0) || !(norm > 0) || !truth_offsets || !labels_out || !loss_sum || !conf_frames ||
+      !conf_merged)
+    return -1;
+  if (truth_offsets[0] != 0) return -1;
+  for (int v = 0; v < V; ++v)
+    if (truth_offsets[v + 1] < truth_offsets[v]) return -1;
+  const size_t nrows = truth_offsets[V];
+  if (nrows > 0 && !truth) return -1;
+  int rc;
+  // the truth goes up first: the prep / forward reservations below do not touch these slots
+  if ((rc = ct_reserve(net, IO_TRUTH, std::max<size_t>(nrows, 1) * 4 * sizeof(int))) || (rc = ct_reserve(net, IO_TOFFS, (V + 1) * sizeof(int))) ||
+      (rc = ct_reserve(net, IO_SCORE, (size_t)V * (1 + 20 + 4) * 8)))
+    return rc;
+  if (nrows) CT_CUDA(cudaMemcpyAsync(net->io[IO_TRUTH], truth, nrows * 4 * sizeof(int), cudaMemcpyHostToDevice, net->stream));
+  CT_CUDA(cudaMemcpyAsync(net->io[IO_TOFFS], truth_offsets, (V + 1) * sizeof(int), cudaMemcpyHostToDevice, net->stream));
+  int Fmax = 0;
+  if ((rc = ct_detect_device(net, raw, seq_offsets, V, scale, norm, &Fmax))) return rc;
+  double* d_loss = (double*)net->io[IO_SCORE];
+  int64_t* d_frames = (int64_t*)(d_loss + V);
+  int64_t* d_merged = d_frames + (size_t)V * 20;
+  if ((rc = chd_contact_score_device(net, (const float*)net->io[IO_LOGITS], V, Fmax, (const int*)net->io[IO_TRUTH], (const int*)net->io[IO_TOFFS],
+                                     classify_thresh, d_loss, d_frames, d_merged, net->stream)))
+    return rc;
+  if ((rc = ct_pack_download(net, seq_offsets, V, Fmax, labels_out, min_abs_logit))) return rc;
+  CT_CUDA(cudaMemcpyAsync(loss_sum, d_loss, V * sizeof(double), cudaMemcpyDeviceToHost, net->stream));
+  CT_CUDA(cudaMemcpyAsync(conf_frames, d_frames, (size_t)V * 20 * sizeof(int64_t), cudaMemcpyDeviceToHost, net->stream));
+  CT_CUDA(cudaMemcpyAsync(conf_merged, d_merged, (size_t)V * 4 * sizeof(int64_t), cudaMemcpyDeviceToHost, net->stream));
   CT_CUDA(cudaStreamSynchronize(net->stream));
   return 0;
 }

@@ -234,13 +234,10 @@ def make_batch(batch: int, n_frames: int = 120, n_ee: int = 2, seed0: int = 0, d
 # A synthetic video directory for the pipeline on either side of phys-optim (no capture data ships with the reference):
 # OpenPose BODY_25 JSON files, a Monocular-Total-Capture `tracked_results.json`, contact labels, and the skeleton template.
 # ---------------------------------------------------------------------------------------------------------------------
-def write_mocap_clip(video_dir: str, n_frames: int = 48, seed: int = 0, fps: float = 30.0, noise_px: float = 1.0, noise_cm: float = 0.5):
-    """Walking clip in the MTC camera frame (x right, y down, z forward, cm; focal 2000 px, 1920 x 1080): feet planted during
-    stance, joint angles from an IK fit of the `combined` template.  Writes `<video_dir>/openpose_result/*_keypoints.json`,
-    `tracked_results.json`, `foot_contacts.npy`, `skeleton.bvh`; returns the ground truth (dict)."""
-    import json
-    import os
-    from . import kinopt, prepare, results
+def _mocap_walk(n_frames: int, seed: int, fps: float):
+    """The walk behind `write_mocap_clip`: (rng after its draws, IK-fitted SkelAnim, global joint positions (F, 28, 3), root
+    (F, 3), foot contacts (F, 4) int64 [L heel, L toe, R heel, R toe], floor height) in the MTC camera frame, cm."""
+    from . import prepare, results
     rng = np.random.default_rng(seed)
     F, J = n_frames, len(prepare.COMBINED_NAMES)
     t = np.arange(F) / fps
@@ -271,16 +268,41 @@ def write_mocap_clip(video_dir: str, n_frames: int = 48, seed: int = 0, fps: flo
     targets = {4: l_heel, 5: l_toe, 10: r_heel, 11: r_toe, 16: root + np.array([4.0, -51.0, 0.0])}
     anim = results.ik_solve(anim, targets, iterations=80, damping=2.0, smoothness=0.0, translate=False)
     gp = anim.global_positions()                                                            # (F, 28, 3) absolute, skeleton order
-    body = gp[:, kinopt.BACKWARD]                                                           # body-25 order (+3 spine)
     fc = np.stack([l_st, l_st, r_st, r_st], axis=1).astype(np.int64)                        # L heel, L toe, R heel, R toe
-    os.makedirs(os.path.join(video_dir, "openpose_result"), exist_ok=True)
-    name = os.path.basename(os.path.normpath(video_dir))
-    kp2d = body[:, :25, :2] / body[:, :25, 2:3] * 2000.0 + np.array([960.0, 540.0]) + rng.normal(0, noise_px, (F, 25, 2))
+    return rng, anim, gp, root, fc, floor_y
+
+
+def _project_keypoints(body, rng, noise_px: float, shift=(0.0, 0.0)):
+    """BODY_25 joints (F, 25, 3) in the camera frame -> OpenPose keypoints (F, 25, 3) [x, y, confidence] at focal 2000 px,
+    1920 x 1080, principal point moved by `shift` px."""
+    F = body.shape[0]
+    kp2d = body[:, :25, :2] / body[:, :25, 2:3] * 2000.0 + np.array([960.0 + shift[0], 540.0 + shift[1]]) + rng.normal(0, noise_px, (F, 25, 2))
     conf = rng.uniform(0.4, 1.0, (F, 25))
-    for f in range(F):
-        doc = {"version": 1.3, "people": [{"person_id": [-1], "pose_keypoints_2d": [float(v) for v in np.concatenate([kp2d[f], conf[f, :, None]], axis=1).reshape(-1)]}]}
-        with open(os.path.join(video_dir, "openpose_result", "%s_%012d_keypoints.json" % (name, f)), "w") as fh:
+    return np.concatenate([kp2d, conf[..., None]], axis=2)
+
+
+def _write_openpose_dir(path: str, name: str, kp):
+    import json
+    import os
+    os.makedirs(path, exist_ok=True)
+    for f in range(kp.shape[0]):
+        doc = {"version": 1.3, "people": [{"person_id": [-1], "pose_keypoints_2d": [float(v) for v in kp[f].reshape(-1)]}]}
+        with open(os.path.join(path, "%s_%012d_keypoints.json" % (name, f)), "w") as fh:
             json.dump(doc, fh)
+
+
+def write_mocap_clip(video_dir: str, n_frames: int = 48, seed: int = 0, fps: float = 30.0, noise_px: float = 1.0, noise_cm: float = 0.5):
+    """Walking clip in the MTC camera frame (x right, y down, z forward, cm; focal 2000 px, 1920 x 1080): feet planted during
+    stance, joint angles from an IK fit of the `combined` template.  Writes `<video_dir>/openpose_result/*_keypoints.json`,
+    `tracked_results.json`, `foot_contacts.npy`, `skeleton.bvh`; returns the ground truth (dict)."""
+    import json
+    import os
+    from . import kinopt, prepare
+    F, J = n_frames, len(prepare.COMBINED_NAMES)
+    rng, anim, gp, root, fc, floor_y = _mocap_walk(n_frames, seed, fps)
+    body = gp[:, kinopt.BACKWARD]                                                           # body-25 order (+3 spine)
+    name = os.path.basename(os.path.normpath(video_dir))
+    _write_openpose_dir(os.path.join(video_dir, "openpose_result"), name, _project_keypoints(body, rng, noise_px))
     # MTC results: BODY_25 joints relative to the root translation, 22 SMPL joints (root + spine positions, joint angles)
     Rl = anim.rotations
     ang = np.arccos(np.clip((np.trace(Rl, axis1=-2, axis2=-1) - 1.0) / 2.0, -1.0, 1.0))
@@ -302,3 +324,41 @@ def write_mocap_clip(video_dir: str, n_frames: int = 48, seed: int = 0, fps: flo
     np.save(os.path.join(video_dir, "foot_contacts.npy"), fc)
     prepare.write_combined_template(os.path.join(video_dir, "skeleton.bvh"))
     return dict(root=root, joints=gp, contacts=fc, floor_y=floor_y, euler=None, fps=fps)
+
+
+def write_contact_dataset(root: str, characters: int, motions: int, views: int, frames: int, seed: int = 0) -> List[str]:
+    """A labelled tree in the layout of the reference's synthetic contact dataset (contact_data_utils.py:8-27), read by
+    `chd.contact.read_synthetic_videos`:
+
+        <root>/character<c>/motion<m>/foot_contacts.npy                 (frames, 4) int64, shared by the motion's views
+        <root>/character<c>/motion<m>/view<k>/frame_<f>.png             empty placeholders: the reference counts frames here
+        <root>/character<c>/motion<m>/keypoints_view<k>/*_keypoints.json
+
+    Every motion is one `write_mocap_clip` walk (its own seed); every view projects it with its own principal point,
+    pixel noise, confidences and a few low-confidence frames.  Keypoints are rounded to 1e-3 px (confidences to 1e-4), as
+    OpenPose writes a handful of decimals; the files are then the same on any host.  Returns the motion directories."""
+    import os
+    from . import kinopt
+    out = []
+    for c in range(characters):
+        for m in range(motions):
+            mdir = os.path.join(root, "character%02d" % c, "motion%02d" % m)
+            wseed = int(np.random.SeedSequence([seed, c, m]).generate_state(1)[0])
+            _, _, gp, _, fc, _ = _mocap_walk(frames, wseed, 30.0)
+            body = gp[:, kinopt.BACKWARD]
+            os.makedirs(mdir, exist_ok=True)
+            np.save(os.path.join(mdir, "foot_contacts.npy"), fc)
+            for k in range(views):
+                rng = np.random.default_rng([seed, c, m, k])
+                kp = _project_keypoints(body, rng, 1.0, shift=tuple(rng.uniform(-200.0, 200.0, 2)))
+                low = rng.uniform(size=kp.shape[:2]) < 0.03
+                kp[:, :, 2] = np.where(low, kp[:, :, 2] * 0.25, kp[:, :, 2])
+                kp[:, :, :2] = np.round(kp[:, :, :2], 3)
+                kp[:, :, 2] = np.round(kp[:, :, 2], 4)
+                vdir = os.path.join(mdir, "view%d" % k)
+                os.makedirs(vdir, exist_ok=True)
+                for f in range(frames):
+                    open(os.path.join(vdir, "frame_%06d.png" % f), "wb").close()
+                _write_openpose_dir(os.path.join(mdir, "keypoints_view%d" % k), "view%d" % k, kp)
+            out.append(mdir)
+    return out

@@ -182,11 +182,43 @@ int chd_contact_forward_device(chd_contact_net* net, const double* frames_dev, i
  * seq_lens_out [host, optional] V.  Bit identical to the reference's numpy result. */
 int chd_contact_preprocess(chd_contact_net* net, const double* raw, const int32_t* seq_offsets, int32_t V, int32_t dim_w,
                            double* frames_out, int32_t* seq_lens_out);
+/* The same with the two dataset constants as arguments: xy is multiplied by `scale` before the interpolation and divided
+ * by `norm` after it.  chd_contact_preprocess is this with scale = 1280 / dim_w, norm = 200.4160302695367; the synthetic
+ * dataset (OpenPoseDataset, openpose_dataset.py:126-269) uses scale = 1 (exact) and norm = the median MidHip -> LBigToe
+ * distance of its raw keypoints.  Returns -1 for scale or norm not > 0. */
+int chd_contact_preprocess_scaled(chd_contact_net* net, const double* raw, const int32_t* seq_offsets, int32_t V, double scale,
+                                  double norm, double* frames_out, int32_t* seq_lens_out);
 /* test.py --full-video --save-contacts --real-data in one call: raw keypoints in, foot_contacts rows out.
  * labels_out [host] (sum F) x 4 int64 (columns L heel, L toe, R heel, R toe; the rows every video's foot_contacts.npy
  * holds, concatenated).  raw may be page-locked: the upload is asynchronous on the net's stream. */
 int chd_contact_detect(chd_contact_net* net, const double* raw, const int32_t* seq_offsets, int32_t V, int32_t dim_w,
                        int64_t* labels_out, float* min_abs_logit);
+/* Scores the logits of chd_contact_forward_device against ground-truth contacts (test.py:51-152 val_full_video with
+ * labels), one CTA per video, on `stream` after the forward.  logits_dev [device] V x (Fmax-8) x 20 as the forward leaves
+ * them; truth_dev [device] int32 (sum of rows) x 4, video v owning rows truth_offsets_dev[v] .. [v+1]-1
+ * (truth_offsets_dev [device] V+1, non-decreasing); a video's rows are padded with its last row or trimmed to Fmax
+ * (fix_data_len, real_video_dataset.py:165-191), a nonzero entry is a contact, a video without rows has no labels and
+ * gets zeros.  Outputs [device], per video:
+ *   loss_sum_dev    V doubles: sum over windows x 5 frames x 4 contacts of BCE-with-logits (OpenPoseModel.loss), every
+ *                   term in fp32, the sum in fp64;
+ *   conf_frames_dev V x 5 x 4 int64: (tp, fp, fn, tn) of sigmoid(x) > classify_thresh (fp32) for predicted frame p of
+ *                   every window w against truth row w + 2 + p (OpenPoseModel.accuracy, tgt_frame = p);
+ *   conf_merged_dev V x 4 int64: (tp, fp, fn, tn) over all Fmax frames x 4 of the 0.5 vote before trimming to seq_len,
+ *                   against truth row clamp(f, 2, Fmax - 3) (test.py:124-140).
+ * Windows over the padding of shorter videos are counted, as in the reference.  Each video's outputs are bitwise the
+ * same whatever else is in the batch (given the same Fmax).  Returns 0, -1 bad argument, <= -100 CUDA error. */
+int chd_contact_score_device(chd_contact_net* net, const float* logits_dev, int32_t V, int32_t Fmax, const int32_t* truth_dev,
+                             const int32_t* truth_offsets_dev, float classify_thresh, double* loss_sum_dev,
+                             int64_t* conf_frames_dev, int64_t* conf_merged_dev, void* stream);
+/* The labelled counterpart of chd_contact_detect (test.py --full-video with ground truth): one upload of the raw
+ * keypoints and the truth, then preprocessing (chd_contact_preprocess_scaled's scale / norm), forward, vote, score and
+ * pack on the net's stream, then one download.  truth [host] int32 (sum of rows) x 4 (may be NULL when there are no
+ * rows), truth_offsets [host] V+1 starting at 0; labels_out [host] (sum F) x 4 int64 as chd_contact_detect; loss_sum
+ * [host] V, conf_frames [host] V x 5 x 4, conf_merged [host] V x 4 as chd_contact_score_device; min_abs_logit [host,
+ * optional].  Either precision mode.  Returns 0, -1 bad argument, <= -100 CUDA error. */
+int chd_contact_evaluate(chd_contact_net* net, const double* raw, const int32_t* seq_offsets, int32_t V, double scale, double norm,
+                         const int32_t* truth, const int32_t* truth_offsets, float classify_thresh, int64_t* labels_out,
+                         double* loss_sum, int64_t* conf_frames, int64_t* conf_merged, float* min_abs_logit);
 int64_t chd_contact_launch_count(const chd_contact_net* net);
 /* Numerical mode of every later chd_contact_forward / _forward_device / _detect call on this net.
  * FP32 (default): FFMA, labels match the reference's fp32 forward.  TF32X3: the 352-1024-512-128 layers on the
