@@ -5,8 +5,8 @@ Keypoint loading (JSON) happens on the host; the dataset preprocessing (padding,
 interpolation, normalisation: real_video_dataset.py:132-163, openpose_dataset.py:49-121), window construction, the MLP
 and the vote aggregation run in hand-written CUDA behind `chd_contact_*` (include/chd.h).  No CPU fallback.
 With ground truth (test.py --full-video on labelled videos or on the synthetic dataset's test split) `ContactNet.evaluate`
-also scores the windows on the device (`chd_contact_evaluate`); `read_real_videos` / `read_synthetic_videos` read the two
-dataset layouts.
+also scores the windows on the device (`chd_contact_detect` with truth); `read_real_videos` / `read_synthetic_videos`
+read the two dataset layouts.
 """
 from __future__ import annotations
 
@@ -154,7 +154,7 @@ class ContactNet:
         return (labels, logits, float(mabs[0])) if want_logits else (labels, float(mabs[0]))
 
     def preprocess(self, raw: Sequence[np.ndarray], dimensions=(1920, 1080), scale: Optional[float] = None, norm: float = TRAIN_NORMALIZATION):
-        """RealVideoDataset.__init__ on the device (`chd_contact_preprocess_scaled`): list of raw (F_i,25,3) keypoints ->
+        """RealVideoDataset.__init__ on the device (`chd_contact_preprocess`): list of raw (F_i,25,3) keypoints ->
         (frames (V,Fmax,25,3) fp64, seq_lens (V,) int32), bit identical to the reference's numpy result.  `scale`
         (default 1280 / dimensions[0]) and `norm` are the dataset's constants; `SyntheticVideos` carries its own."""
         cat, offs = concat_videos(raw)
@@ -162,29 +162,45 @@ class ContactNet:
         frames = np.zeros((V, Fmax, 25, 3))
         lens = np.zeros(V, dtype=np.int32)
         scale = video_scale(dimensions) if scale is None else scale
-        rc = self.L.chd_contact_preprocess_scaled(self.h, cat.ctypes.data, offs.ctypes.data, V, float(scale), float(norm), frames.ctypes.data,
-                                                  lens.ctypes.data)
+        rc = self.L.chd_contact_preprocess(self.h, cat.ctypes.data, offs.ctypes.data, V, float(scale), float(norm), frames.ctypes.data,
+                                           lens.ctypes.data)
         if rc != 0:
             raise RuntimeError("chd_contact_preprocess failed with code %d" % rc)
         return frames, lens
 
-    def detect(self, raw: Sequence[np.ndarray], dimensions=(1920, 1080), cat=None, offs=None):
-        """raw keypoints -> list of (F_i,4) int64 foot-contact labels (`chd_contact_detect`: preprocessing, windows,
-        network, votes on the device; one upload, one download).  `cat` / `offs` may carry a pre-concatenated (e.g.
-        page-locked) buffer."""
+    def _detect(self, raw, cat, offs, scale, norm, truth=None, classify_thresh=0.5):
+        """One `chd_contact_detect` call on `raw` or the concatenated `cat` / `offs` -> (labels per video, min |logit|, offs,
+        truth offsets, (loss_sum, conf_frames, conf_merged)); without `truth` nothing is scored and those are None."""
         if cat is None:
             cat, offs = concat_videos(raw)
         V = len(offs) - 1
         lab = np.zeros((int(offs[-1]), 4), dtype=np.int64)
         mabs = np.zeros(1, dtype=np.float32)
-        rc = self.L.chd_contact_detect(self.h, cat.ctypes.data, offs.ctypes.data, V, int(dimensions[0]), lab.ctypes.data, mabs.ctypes.data)
+        tcat, toffs, scores = None, None, (None,) * 3
+        if truth is not None:
+            if len(truth) != V:
+                raise ValueError("evaluate: %d videos but %d truth entries" % (V, len(truth)))
+            rows = [np.zeros((0, 4), dtype=np.int32) if t is None else np.asarray(t).reshape(-1, 4) for t in truth]
+            toffs = np.zeros(V + 1, dtype=np.int32)
+            toffs[1:] = np.cumsum([r.shape[0] for r in rows])
+            tcat = np.ascontiguousarray(np.concatenate(rows, axis=0) != 0, dtype=np.int32) if toffs[-1] else np.zeros((1, 4), dtype=np.int32)
+            scores = (np.zeros(V, dtype=np.float64), np.zeros((V, PRED, 4), dtype=np.int64), np.zeros((V, 4), dtype=np.int64))
+        ptr = lambda a: None if a is None else a.ctypes.data
+        rc = self.L.chd_contact_detect(self.h, cat.ctypes.data, offs.ctypes.data, V, float(scale), float(norm), ptr(tcat), ptr(toffs),
+                                       C.c_float(classify_thresh), lab.ctypes.data, *map(ptr, scores), mabs.ctypes.data)
         if rc != 0:
             raise RuntimeError("chd_contact_detect failed with code %d" % rc)
-        return [lab[offs[i]:offs[i + 1]] for i in range(V)], float(mabs[0])
+        return [lab[offs[i]:offs[i + 1]] for i in range(V)], float(mabs[0]), offs, toffs, scores
+
+    def detect(self, raw: Sequence[np.ndarray], dimensions=(1920, 1080), cat=None, offs=None):
+        """raw keypoints -> list of (F_i,4) int64 foot-contact labels (`chd_contact_detect`: preprocessing, windows,
+        network, votes on the device; one upload, one download).  `cat` / `offs` may carry a pre-concatenated (e.g.
+        page-locked) buffer."""
+        return self._detect(raw, cat, offs, video_scale(dimensions), TRAIN_NORMALIZATION)[:2]
 
     def evaluate(self, raw: Sequence[np.ndarray], truth: Sequence[Optional[np.ndarray]], scale: float, norm: float,
                  classify_thresh: float = 0.5, cat=None, offs=None) -> Dict:
-        """test.py --full-video with ground truth (`chd_contact_evaluate`: preprocessing with `scale` / `norm`, windows,
+        """test.py --full-video with ground truth (`chd_contact_detect`: preprocessing with `scale` / `norm`, windows,
         network, votes and scoring on the device; one upload, one download).  truth[i]: (T_i,4) contacts of video i (any
         length: padded with the last row or trimmed to the longest video, as fix_data_len does) or None.  Returns a dict:
           labels       list of (F_i,4) int64, what `detect` returns
@@ -195,30 +211,13 @@ class ContactNet:
           labelled, windows, loss_count: labelled videos, windows per video, terms in the mean loss
           mean_loss    loss_sum.sum() / loss_count (test.py:84-85, 214), None without labelled videos
           min_abs_logit"""
-        if cat is None:
-            cat, offs = concat_videos(raw)
-        V = len(offs) - 1
-        if len(truth) != V:
-            raise ValueError("evaluate: %d videos but %d truth entries" % (V, len(truth)))
-        rows = [np.zeros((0, 4), dtype=np.int32) if t is None else np.asarray(t).reshape(-1, 4) for t in truth]
-        toffs = np.zeros(V + 1, dtype=np.int32)
-        toffs[1:] = np.cumsum([r.shape[0] for r in rows])
-        tcat = np.ascontiguousarray(np.concatenate(rows, axis=0) != 0, dtype=np.int32) if toffs[-1] else np.zeros((1, 4), dtype=np.int32)
-        lab = np.zeros((int(offs[-1]), 4), dtype=np.int64)
-        loss = np.zeros(V, dtype=np.float64)
-        cf = np.zeros((V, PRED, 4), dtype=np.int64)
-        cm = np.zeros((V, 4), dtype=np.int64)
-        mabs = np.zeros(1, dtype=np.float32)
-        rc = self.L.chd_contact_evaluate(self.h, cat.ctypes.data, offs.ctypes.data, V, float(scale), float(norm), tcat.ctypes.data, toffs.ctypes.data,
-                                         C.c_float(classify_thresh), lab.ctypes.data, loss.ctypes.data, cf.ctypes.data, cm.ctypes.data, mabs.ctypes.data)
-        if rc != 0:
-            raise RuntimeError("chd_contact_evaluate failed with code %d" % rc)
+        labels, mabs, offs, toffs, (loss, cf, cm) = self._detect(raw, cat, offs, scale, norm, truth, classify_thresh)
         windows = int(np.diff(offs).max()) - (WINDOW - 1)
         labelled = int((np.diff(toffs) > 0).sum())
         count = PRED * 4 * windows * labelled
-        return dict(labels=[lab[offs[i]:offs[i + 1]] for i in range(V)], loss_sum=loss, conf_frames=cf, conf_merged=cm,
-                    frames_total=cf.sum(0), merged_total=cm.sum(0), labelled=labelled, windows=windows, loss_count=count,
-                    mean_loss=float(loss.sum() / count) if count else None, min_abs_logit=float(mabs[0]))
+        return dict(labels=labels, loss_sum=loss, conf_frames=cf, conf_merged=cm, frames_total=cf.sum(0), merged_total=cm.sum(0),
+                    labelled=labelled, windows=windows, loss_count=count, mean_loss=float(loss.sum() / count) if count else None,
+                    min_abs_logit=mabs)
 
     def launch_count(self) -> int:
         return int(self.L.chd_contact_launch_count(self.h))

@@ -176,31 +176,39 @@ __global__ void __launch_bounds__(256) chd_k_contact_tail(ContactDev net, const 
   }
 }
 
+// The 0.5 vote of frame f, contact c of one video whose window logits are lg [Fmax-8][20] (test.py:88-122); the one
+// rule behind the labels of chd_k_contact_vote and the merged counts of chd_k_contact_score.  mabs, when given, takes
+// the min of the |logit| of every prediction that entered the vote.
+static __device__ __forceinline__ bool ct_vote(const float* __restrict__ lg, int Fmax, int f, int c, float* mabs = nullptr) {
+  const int Wn = Fmax - (CT_WIN - 1), nv = Wn + 2 * (CT_PRED / 2);   // frames that receive votes
+  const int off = (CT_WIN - CT_PRED) / 2;                            // copies padded on each side
+  int fv = f - off;                        // index into the voted array, clamped = repeat first/last row
+  fv = fv < 0 ? 0 : (fv >= nv ? nv - 1 : fv);
+  int votes = 0;
+  for (int p = 0; p < CT_PRED; ++p) {      // window w = fv - p contributes its prediction for offset p
+    const int w = fv - p;
+    if (w < 0 || w >= Wn) continue;
+    const float x = lg[w * 20 + p * 4 + c];
+    const float prob = 1.0f / (1.0f + expf(-x));   // openpose_only.py:75-78: sigmoid(x) > 0.5
+    votes += prob > 0.5f ? 1 : 0;
+    if (mabs) *mabs = fminf(*mabs, fabsf(x));
+  }
+  int thresh = (CT_PRED + 1) / 2;          // test.py:101-104
+  const int e0 = fv, e1 = nv - 1 - fv;
+  if (e0 < CT_PRED - 1) thresh = e0 / 2 + 1;
+  if (e1 < CT_PRED - 1) thresh = e1 / 2 + 1;
+  return votes >= thresh;
+}
+
 // labels [V][Fmax][4] int64; rows >= seq_len are zeroed (the reference trims them, test.py:149-152)
 __global__ void chd_k_contact_vote(const float* __restrict__ logits, int V, int Fmax, const int* __restrict__ seq_lens,
                                    long long* __restrict__ labels, float* __restrict__ min_abs) {
-  const int Wn = Fmax - (CT_WIN - 1), nv = Wn + 2 * (CT_PRED / 2);   // frames that receive votes
-  const int off = (CT_WIN - CT_PRED) / 2;                            // copies padded on each side
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;
   float mabs = 3.4e38f;
   if (idx < V * Fmax * 4) {
     const int c = idx & 3, f = (idx >> 2) % Fmax, v = (idx >> 2) / Fmax;
-    int fv = f - off;                        // index into the voted array, clamped = repeat first/last row
-    fv = fv < 0 ? 0 : (fv >= nv ? nv - 1 : fv);
-    int votes = 0;
-    for (int p = 0; p < CT_PRED; ++p) {      // window w = fv - p contributes its prediction for offset p
-      const int w = fv - p;
-      if (w < 0 || w >= Wn) continue;
-      const float x = logits[((size_t)v * Wn + w) * 20 + p * 4 + c];
-      const float prob = 1.0f / (1.0f + expf(-x));   // openpose_only.py:75-78: sigmoid(x) > 0.5
-      votes += prob > 0.5f ? 1 : 0;
-      mabs = fminf(mabs, fabsf(x));
-    }
-    int thresh = (CT_PRED + 1) / 2;          // test.py:101-104
-    const int e0 = fv, e1 = nv - 1 - fv;
-    if (e0 < CT_PRED - 1) thresh = e0 / 2 + 1;
-    if (e1 < CT_PRED - 1) thresh = e1 / 2 + 1;
-    labels[idx] = f < seq_lens[v] ? (votes >= thresh ? 1 : 0) : 0;
+    const bool vote = ct_vote(logits + (size_t)v * (Fmax - (CT_WIN - 1)) * 20, Fmax, f, c, &mabs);
+    labels[idx] = f < seq_lens[v] ? (vote ? 1 : 0) : 0;
   }
   // block min of |logit|
   for (int o = 16; o > 0; o >>= 1) mabs = fminf(mabs, __shfl_xor_sync(0xffffffffu, mabs, o));
@@ -214,8 +222,8 @@ __global__ void chd_k_contact_vote(const float* __restrict__ logits, int V, int 
 // with their last row or trimmed to Fmax (fix_data_len, real_video_dataset.py:165-191); a video without rows gets zeros.
 //   loss_sum[v]          sum over windows x 5 x 4 of BCE-with-logits (1 - y) x - log_sigmoid(x), fp32 terms, fp64 sum
 //   conf_frames[v][p][.] (tp, fp, fn, tn) of sigmoid(x) > thresh against truth row w + 2 + p of window w
-//   conf_merged[v][.]    (tp, fp, fn, tn) over all Fmax x 4 of the 0.5 vote before trimming (recomputed: the vote kernel
-//                        zeroes rows >= seq_len) against truth row clamp(f, 2, Fmax - 3), test.py:124-140
+//   conf_merged[v][.]    (tp, fp, fn, tn) over all Fmax x 4 of the 0.5 vote before trimming (ct_vote again: the vote
+//                        kernel zeroes rows >= seq_len) against truth row clamp(f, 2, Fmax - 3), test.py:124-140
 // Fixed-order reductions, no atomics: a video's outputs depend only on its own logits, truth and Fmax.
 #define CT_SCORE_THREADS 320
 __global__ void __launch_bounds__(CT_SCORE_THREADS) chd_k_contact_score(const float* __restrict__ logits, int Fmax, const int* __restrict__ truth,
@@ -224,7 +232,7 @@ __global__ void __launch_bounds__(CT_SCORE_THREADS) chd_k_contact_score(const fl
   __shared__ int s_cnt[CT_SCORE_THREADS][4];
   __shared__ double s_loss[CT_SCORE_THREADS / 32];
   const int v = blockIdx.x, tid = threadIdx.x;
-  const int Wn = Fmax - (CT_WIN - 1), nv = Wn + 2 * (CT_PRED / 2), off = (CT_WIN - CT_PRED) / 2;
+  const int Wn = Fmax - (CT_WIN - 1), off = (CT_WIN - CT_PRED) / 2;
   const int t0 = toffs[v], nrow = toffs[v + 1] - t0;
   const float* lg = logits + (size_t)v * Wn * 20;
   auto label = [&](int r, int c) { return truth[(size_t)(t0 + (r < nrow ? r : nrow - 1)) * 4 + c] != 0; };
@@ -264,20 +272,7 @@ __global__ void __launch_bounds__(CT_SCORE_THREADS) chd_k_contact_score(const fl
   if (nrow > 0) {
     for (int i = tid; i < Fmax * 4; i += CT_SCORE_THREADS) {
       const int c = i & 3, f = i >> 2;
-      int fv = f - off;
-      fv = fv < 0 ? 0 : (fv >= nv ? nv - 1 : fv);
-      int votes = 0;
-      for (int p = 0; p < CT_PRED; ++p) {
-        const int w = fv - p;
-        if (w < 0 || w >= Wn) continue;
-        const float x = lg[w * 20 + p * 4 + c];
-        votes += 1.0f / (1.0f + expf(-x)) > 0.5f ? 1 : 0;
-      }
-      int th = (CT_PRED + 1) / 2;
-      const int e0 = fv, e1 = nv - 1 - fv;
-      if (e0 < CT_PRED - 1) th = e0 / 2 + 1;
-      if (e1 < CT_PRED - 1) th = e1 / 2 + 1;
-      const bool pred = votes >= th;
+      const bool pred = ct_vote(lg, Fmax, f, c);
       const bool y = label(f < off ? off : (f > Fmax - 1 - off ? Fmax - 1 - off : f), c);
       ++mc[pred ? (y ? 0 : 1) : (y ? 2 : 3)];
     }
@@ -291,26 +286,24 @@ __global__ void __launch_bounds__(CT_SCORE_THREADS) chd_k_contact_score(const fl
   }
 }
 
+// Grow-only device buffers (ct_reserve): the host entry points' buffers and the slab workspaces of the two modes,
+// IO_WS = A0 [rows][352] | A1 [rows][1024] | A2 [rows][512] | A3 [rows][128] of the FP32 kernels and IO_TC_WS = the
+// tensor-core layers' planes (chd_contact_tc_ws_floats).
+enum { IO_FRAMES, IO_LENS, IO_LABELS, IO_LOGITS, IO_MIN, IO_RAW, IO_OFFS, IO_PACKED, IO_TRUTH, IO_TOFFS, IO_SCORE, IO_WS, IO_TC_WS, IO_COUNT };
+
 struct chd_contact_net {
   std::vector<void*> allocs;
   ContactDev dev;
   cudaStream_t stream = nullptr;
   int64_t launches = 0;
-  float* ws = nullptr;     // activation workspace of one slab: A0 [Mp][352] | A1 [Mp][1024] | A2 [Mp][512] | A3 [Mp][128]
-  int ws_rows = 0;
-  // grow-only device buffers of the host entry points (no allocation per call, nothing to leak on an error path)
-  void* io[11] = {};
-  size_t io_bytes[11] = {};
-  // CHD_CONTACT_TF32X3: split weight planes (one allocation) and the slab workspace of the tensor-core layers
+  // no allocation per call, nothing to leak on an error path
+  void* io[IO_COUNT] = {};
+  size_t io_bytes[IO_COUNT] = {};
+  // CHD_CONTACT_TF32X3: split weight planes (one allocation)
   int precision = CHD_CONTACT_FP32;
   ChdContactTcNet tc = {};
   float* tc_w = nullptr;
-  float* tc_ws = nullptr;
-  int tc_ws_rows = 0;
 };
-enum { IO_FRAMES = 0, IO_LENS = 1, IO_LABELS = 2, IO_LOGITS = 3, IO_MIN = 4, IO_RAW = 5, IO_OFFS = 6, IO_PACKED = 7, IO_TRUTH = 8, IO_TOFFS = 9,
-       IO_SCORE = 10, IO_COUNT = 11 };
-static_assert(sizeof(chd_contact_net::io) / sizeof(void*) == IO_COUNT, "one io slot per IO_* id");
 
 #define CT_CUDA(x)                                                                           \
   do {                                                                                       \
@@ -435,9 +428,7 @@ int chd_contact_create(const float* weights, const float* biases, const float* b
 void chd_contact_destroy(chd_contact_net* net) {
   if (!net) return;
   for (void* p : net->allocs) cudaFree(p);
-  if (net->ws) cudaFree(net->ws);
   if (net->tc_w) cudaFree(net->tc_w);
-  if (net->tc_ws) cudaFree(net->tc_ws);
   for (int q = 0; q < IO_COUNT; ++q)
     if (net->io[q]) cudaFree(net->io[q]);
   if (net->stream) cudaStreamDestroy(net->stream);
@@ -453,17 +444,13 @@ int chd_contact_forward_device(chd_contact_net* net, const double* frames_dev, i
   CT_CUDA(cudaMemcpyAsync(min_abs_dev, &big, sizeof(float), cudaMemcpyHostToDevice, s));
   const int rows = std::min(CT_SLAB, (total + GM - 1) / GM * GM);
   const ContactDev& d = net->dev;
+  int rc;
   if (net->precision == CHD_CONTACT_TF32X3) {
     // per slab: split gather, three tensor-core layers, FFMA tail (chd_contact_tc.cu)
-    if (rows > net->tc_ws_rows) {
-      if (net->tc_ws) cudaFree(net->tc_ws);
-      net->tc_ws = nullptr, net->tc_ws_rows = 0;
-      CT_CUDA(cudaMalloc((void**)&net->tc_ws, chd_contact_tc_ws_floats(rows) * sizeof(float)));
-      net->tc_ws_rows = rows;
-    }
     ChdContactTcPlan plan;
-    int rc = chd_contact_tc_plan(&net->tc, net->tc_ws, net->tc_ws_rows, &plan);
-    if (rc) return rc;
+    if ((rc = ct_reserve(net, IO_TC_WS, chd_contact_tc_ws_floats(rows) * sizeof(float))) ||
+        (rc = chd_contact_tc_plan(&net->tc, (float*)net->io[IO_TC_WS], rows, &plan)))
+      return rc;
     for (int g0 = 0; g0 < total; g0 += CT_SLAB) {
       const int Mp = (std::min(CT_SLAB, total - g0) + GM - 1) / GM * GM;
       if ((rc = chd_contact_tc_layers(plan, frames_dev, V, Fmax, g0, Mp, s))) return rc;
@@ -471,16 +458,11 @@ int chd_contact_forward_device(chd_contact_net* net, const double* frames_dev, i
       net->launches += 5;
     }
   } else {
-    if (rows > net->ws_rows) {
-      if (net->ws) cudaFree(net->ws);
-      net->ws = nullptr, net->ws_rows = 0;
-      CT_CUDA(cudaMalloc((void**)&net->ws, (size_t)rows * (CT_K0 + 1024 + 512 + 128) * sizeof(float)));
-      net->ws_rows = rows;
-    }
-    float* A0 = net->ws;
-    float* A1 = A0 + (size_t)net->ws_rows * CT_K0;
-    float* A2 = A1 + (size_t)net->ws_rows * 1024;
-    float* A3 = A2 + (size_t)net->ws_rows * 512;
+    if ((rc = ct_reserve(net, IO_WS, (size_t)rows * (CT_K0 + 1024 + 512 + 128) * sizeof(float)))) return rc;
+    float* A0 = (float*)net->io[IO_WS];
+    float* A1 = A0 + (size_t)rows * CT_K0;
+    float* A2 = A1 + (size_t)rows * 1024;
+    float* A3 = A2 + (size_t)rows * 512;
     for (int g0 = 0; g0 < total; g0 += CT_SLAB) {
       const int Mp = (std::min(CT_SLAB, total - g0) + GM - 1) / GM * GM;
       chd_k_contact_gather<<<(unsigned)(((size_t)Mp * CT_K0 + 255) / 256), 256, 0, s>>>(frames_dev, V, Fmax, g0, Mp, A0);
@@ -521,7 +503,7 @@ int chd_contact_forward(chd_contact_net* net, const double* frames, int32_t V, i
   return 0;
 }
 
-// raw OpenPose keypoints -> preprocessed frames on the device (shared by the preprocess / detect / evaluate entries):
+// raw OpenPose keypoints -> preprocessed frames on the device (shared by chd_contact_preprocess / _detect):
 // xy multiplied by `scale`, gaps interpolated, xy divided by `norm`
 static int ct_prep_device(chd_contact_net* net, const double* raw, const int32_t* offs, int32_t V, double scale, double norm, int* Fmax_out) {
   int Fmax = 0, total = offs[V];
@@ -544,60 +526,14 @@ static int ct_prep_device(chd_contact_net* net, const double* raw, const int32_t
   return 0;
 }
 
-// the real-video preprocessing: TRAIN_DIM[0] / dimensions[0] and the training normalisation, real_video_dataset.py:17-18,149-161
-static double ct_video_scale(int32_t dim_w) { return 1280.0 / dim_w; }
-static const double CT_TRAIN_NORMALIZATION = 200.4160302695367;
-
-int chd_contact_preprocess_scaled(chd_contact_net* net, const double* raw, const int32_t* seq_offsets, int32_t V, double scale, double norm,
-                                  double* frames_out, int32_t* seq_lens_out) {
+int chd_contact_preprocess(chd_contact_net* net, const double* raw, const int32_t* seq_offsets, int32_t V, double scale, double norm,
+                           double* frames_out, int32_t* seq_lens_out) {
   if (!net || !raw || !seq_offsets || V <= 0 || !(scale > 0) || !(norm > 0) || !frames_out) return -1;
   int Fmax = 0;
   int rc = ct_prep_device(net, raw, seq_offsets, V, scale, norm, &Fmax);
   if (rc) return rc;
   CT_CUDA(cudaMemcpyAsync(frames_out, net->io[IO_FRAMES], (size_t)V * Fmax * 75 * sizeof(double), cudaMemcpyDeviceToHost, net->stream));
   if (seq_lens_out) CT_CUDA(cudaMemcpyAsync(seq_lens_out, net->io[IO_LENS], V * sizeof(int), cudaMemcpyDeviceToHost, net->stream));
-  CT_CUDA(cudaStreamSynchronize(net->stream));
-  return 0;
-}
-
-int chd_contact_preprocess(chd_contact_net* net, const double* raw, const int32_t* seq_offsets, int32_t V, int32_t dim_w, double* frames_out,
-                           int32_t* seq_lens_out) {
-  if (dim_w <= 0) return -1;
-  return chd_contact_preprocess_scaled(net, raw, seq_offsets, V, ct_video_scale(dim_w), CT_TRAIN_NORMALIZATION, frames_out, seq_lens_out);
-}
-
-// prep + forward + vote of chd_contact_detect / chd_contact_evaluate on the net's stream; *Fmax_out = longest video
-static int ct_detect_device(chd_contact_net* net, const double* raw, const int32_t* seq_offsets, int32_t V, double scale, double norm, int* Fmax_out) {
-  int Fmax = 0;
-  int rc = ct_prep_device(net, raw, seq_offsets, V, scale, norm, &Fmax);
-  if (rc) return rc;
-  const size_t total = seq_offsets[V], Wn = Fmax - (CT_WIN - 1), nlog = (size_t)V * Wn * 20, nlab = (size_t)V * Fmax * 4;
-  if ((rc = ct_reserve(net, IO_LABELS, nlab * sizeof(long long))) || (rc = ct_reserve(net, IO_LOGITS, nlog * sizeof(float))) ||
-      (rc = ct_reserve(net, IO_MIN, sizeof(float))) || (rc = ct_reserve(net, IO_PACKED, total * 4 * sizeof(long long))))
-    return rc;
-  *Fmax_out = Fmax;
-  return chd_contact_forward_device(net, (const double*)net->io[IO_FRAMES], V, Fmax, (const int*)net->io[IO_LENS], (int64_t*)net->io[IO_LABELS],
-                                    (float*)net->io[IO_LOGITS], (float*)net->io[IO_MIN], net->stream);
-}
-
-// (V, Fmax, 4) labels -> the packed rows on the device, then their download (and min |logit|) on the net's stream
-static int ct_pack_download(chd_contact_net* net, const int32_t* seq_offsets, int32_t V, int Fmax, int64_t* labels_out, float* min_abs_logit) {
-  const size_t total = seq_offsets[V];
-  chd_k_contact_pack<<<dim3(4, V), 256, 0, net->stream>>>((const long long*)net->io[IO_LABELS], (const int*)net->io[IO_OFFS], V, Fmax,
-                                                          (long long*)net->io[IO_PACKED]);
-  net->launches += 1;
-  CT_CUDA(cudaGetLastError());
-  CT_CUDA(cudaMemcpyAsync(labels_out, net->io[IO_PACKED], total * 4 * sizeof(long long), cudaMemcpyDeviceToHost, net->stream));
-  if (min_abs_logit) CT_CUDA(cudaMemcpyAsync(min_abs_logit, net->io[IO_MIN], sizeof(float), cudaMemcpyDeviceToHost, net->stream));
-  return 0;
-}
-
-int chd_contact_detect(chd_contact_net* net, const double* raw, const int32_t* seq_offsets, int32_t V, int32_t dim_w, int64_t* labels_out,
-                       float* min_abs_logit) {
-  if (!net || !raw || !seq_offsets || V <= 0 || dim_w <= 0 || !labels_out) return -1;
-  int Fmax = 0, rc;
-  if ((rc = ct_detect_device(net, raw, seq_offsets, V, ct_video_scale(dim_w), CT_TRAIN_NORMALIZATION, &Fmax))) return rc;
-  if ((rc = ct_pack_download(net, seq_offsets, V, Fmax, labels_out, min_abs_logit))) return rc;
   CT_CUDA(cudaStreamSynchronize(net->stream));
   return 0;
 }
@@ -614,36 +550,52 @@ int chd_contact_score_device(chd_contact_net* net, const float* logits_dev, int3
   return 0;
 }
 
-int chd_contact_evaluate(chd_contact_net* net, const double* raw, const int32_t* seq_offsets, int32_t V, double scale, double norm,
-                         const int32_t* truth, const int32_t* truth_offsets, float classify_thresh, int64_t* labels_out, double* loss_sum,
-                         int64_t* conf_frames, int64_t* conf_merged, float* min_abs_logit) {
-  if (!net || !raw || !seq_offsets || V <= 0 || !(scale > 0) || !(norm > 0) || !truth_offsets || !labels_out || !loss_sum || !conf_frames ||
-      !conf_merged)
-    return -1;
-  if (truth_offsets[0] != 0) return -1;
-  for (int v = 0; v < V; ++v)
-    if (truth_offsets[v + 1] < truth_offsets[v]) return -1;
-  const size_t nrows = truth_offsets[V];
-  if (nrows > 0 && !truth) return -1;
+int chd_contact_detect(chd_contact_net* net, const double* raw, const int32_t* seq_offsets, int32_t V, double scale, double norm,
+                       const int32_t* truth, const int32_t* truth_offsets, float classify_thresh, int64_t* labels_out, double* loss_sum,
+                       int64_t* conf_frames, int64_t* conf_merged, float* min_abs_logit) {
+  if (!net || !raw || !seq_offsets || V <= 0 || !(scale > 0) || !(norm > 0) || !labels_out) return -1;
+  const bool scored = truth_offsets != nullptr;
+  double* d_loss = nullptr;          // IO_SCORE: loss_sum [V] | conf_frames [V][20] | conf_merged [V][4]
+  int64_t *d_frames = nullptr, *d_merged = nullptr;
   int rc;
-  // the truth goes up first: the prep / forward reservations below do not touch these slots
-  if ((rc = ct_reserve(net, IO_TRUTH, std::max<size_t>(nrows, 1) * 4 * sizeof(int))) || (rc = ct_reserve(net, IO_TOFFS, (V + 1) * sizeof(int))) ||
-      (rc = ct_reserve(net, IO_SCORE, (size_t)V * (1 + 20 + 4) * 8)))
-    return rc;
-  if (nrows) CT_CUDA(cudaMemcpyAsync(net->io[IO_TRUTH], truth, nrows * 4 * sizeof(int), cudaMemcpyHostToDevice, net->stream));
-  CT_CUDA(cudaMemcpyAsync(net->io[IO_TOFFS], truth_offsets, (V + 1) * sizeof(int), cudaMemcpyHostToDevice, net->stream));
+  if (scored) {
+    if (!loss_sum || !conf_frames || !conf_merged || truth_offsets[0] != 0) return -1;
+    for (int v = 0; v < V; ++v)
+      if (truth_offsets[v + 1] < truth_offsets[v]) return -1;
+    const size_t nrows = truth_offsets[V];
+    if (nrows > 0 && !truth) return -1;
+    // the truth goes up first: the prep / forward reservations below do not touch these slots
+    if ((rc = ct_reserve(net, IO_TRUTH, std::max<size_t>(nrows, 1) * 4 * sizeof(int))) || (rc = ct_reserve(net, IO_TOFFS, (V + 1) * sizeof(int))) ||
+        (rc = ct_reserve(net, IO_SCORE, (size_t)V * (1 + 20 + 4) * 8)))
+      return rc;
+    d_loss = (double*)net->io[IO_SCORE], d_frames = (int64_t*)(d_loss + V), d_merged = d_frames + (size_t)V * 20;
+    if (nrows) CT_CUDA(cudaMemcpyAsync(net->io[IO_TRUTH], truth, nrows * 4 * sizeof(int), cudaMemcpyHostToDevice, net->stream));
+    CT_CUDA(cudaMemcpyAsync(net->io[IO_TOFFS], truth_offsets, (V + 1) * sizeof(int), cudaMemcpyHostToDevice, net->stream));
+  }
   int Fmax = 0;
-  if ((rc = ct_detect_device(net, raw, seq_offsets, V, scale, norm, &Fmax))) return rc;
-  double* d_loss = (double*)net->io[IO_SCORE];
-  int64_t* d_frames = (int64_t*)(d_loss + V);
-  int64_t* d_merged = d_frames + (size_t)V * 20;
-  if ((rc = chd_contact_score_device(net, (const float*)net->io[IO_LOGITS], V, Fmax, (const int*)net->io[IO_TRUTH], (const int*)net->io[IO_TOFFS],
-                                     classify_thresh, d_loss, d_frames, d_merged, net->stream)))
+  if ((rc = ct_prep_device(net, raw, seq_offsets, V, scale, norm, &Fmax))) return rc;
+  const size_t total = seq_offsets[V], Wn = Fmax - (CT_WIN - 1), nlog = (size_t)V * Wn * 20, nlab = (size_t)V * Fmax * 4;
+  if ((rc = ct_reserve(net, IO_LABELS, nlab * sizeof(long long))) || (rc = ct_reserve(net, IO_LOGITS, nlog * sizeof(float))) ||
+      (rc = ct_reserve(net, IO_MIN, sizeof(float))) || (rc = ct_reserve(net, IO_PACKED, total * 4 * sizeof(long long))))
     return rc;
-  if ((rc = ct_pack_download(net, seq_offsets, V, Fmax, labels_out, min_abs_logit))) return rc;
-  CT_CUDA(cudaMemcpyAsync(loss_sum, d_loss, V * sizeof(double), cudaMemcpyDeviceToHost, net->stream));
-  CT_CUDA(cudaMemcpyAsync(conf_frames, d_frames, (size_t)V * 20 * sizeof(int64_t), cudaMemcpyDeviceToHost, net->stream));
-  CT_CUDA(cudaMemcpyAsync(conf_merged, d_merged, (size_t)V * 4 * sizeof(int64_t), cudaMemcpyDeviceToHost, net->stream));
+  if ((rc = chd_contact_forward_device(net, (const double*)net->io[IO_FRAMES], V, Fmax, (const int*)net->io[IO_LENS], (int64_t*)net->io[IO_LABELS],
+                                       (float*)net->io[IO_LOGITS], (float*)net->io[IO_MIN], net->stream)))
+    return rc;
+  if (scored && (rc = chd_contact_score_device(net, (const float*)net->io[IO_LOGITS], V, Fmax, (const int*)net->io[IO_TRUTH],
+                                               (const int*)net->io[IO_TOFFS], classify_thresh, d_loss, d_frames, d_merged, net->stream)))
+    return rc;
+  // (V, Fmax, 4) labels -> the rows foot_contacts.npy keeps, then one download
+  chd_k_contact_pack<<<dim3(4, V), 256, 0, net->stream>>>((const long long*)net->io[IO_LABELS], (const int*)net->io[IO_OFFS], V, Fmax,
+                                                          (long long*)net->io[IO_PACKED]);
+  net->launches += 1;
+  CT_CUDA(cudaGetLastError());
+  CT_CUDA(cudaMemcpyAsync(labels_out, net->io[IO_PACKED], total * 4 * sizeof(long long), cudaMemcpyDeviceToHost, net->stream));
+  if (min_abs_logit) CT_CUDA(cudaMemcpyAsync(min_abs_logit, net->io[IO_MIN], sizeof(float), cudaMemcpyDeviceToHost, net->stream));
+  if (scored) {
+    CT_CUDA(cudaMemcpyAsync(loss_sum, d_loss, V * sizeof(double), cudaMemcpyDeviceToHost, net->stream));
+    CT_CUDA(cudaMemcpyAsync(conf_frames, d_frames, (size_t)V * 20 * sizeof(int64_t), cudaMemcpyDeviceToHost, net->stream));
+    CT_CUDA(cudaMemcpyAsync(conf_merged, d_merged, (size_t)V * 4 * sizeof(int64_t), cudaMemcpyDeviceToHost, net->stream));
+  }
   CT_CUDA(cudaStreamSynchronize(net->stream));
   return 0;
 }
@@ -654,8 +606,8 @@ int chd_contact_set_precision(chd_contact_net* net, int32_t precision) {
   if (!net || (precision != CHD_CONTACT_FP32 && precision != CHD_CONTACT_TF32X3)) return -1;
   if (precision == CHD_CONTACT_FP32) {             // the FP32 kernels never read the fast mode's buffers
     if (net->tc_w) cudaFree(net->tc_w);
-    if (net->tc_ws) cudaFree(net->tc_ws);
-    net->tc_w = nullptr, net->tc_ws = nullptr, net->tc_ws_rows = 0, net->tc = ChdContactTcNet{};
+    if (net->io[IO_TC_WS]) cudaFree(net->io[IO_TC_WS]);
+    net->tc_w = nullptr, net->io[IO_TC_WS] = nullptr, net->io_bytes[IO_TC_WS] = 0, net->tc = ChdContactTcNet{};
   } else if (!net->tc_w) {                         // split the weights of the three large layers once
     const int K[3] = {CT_K0, 1024, 512}, N[3] = {1024, 512, 128};
     size_t n = 0;

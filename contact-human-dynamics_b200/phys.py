@@ -82,11 +82,9 @@ SIGNATURES = {
     "chd_contact_destroy": (None, [_vp]),
     "chd_contact_forward": (_int, [_vp, _vp, _i32, _i32, _vp, _vp, _vp, _vp]),
     "chd_contact_forward_device": (_int, [_vp, _vp, _i32, _i32, _vp, _vp, _vp, _vp, _vp]),
-    "chd_contact_preprocess": (_int, [_vp, _vp, _vp, _i32, _i32, _vp, _vp]),
-    "chd_contact_preprocess_scaled": (_int, [_vp, _vp, _vp, _i32, _f64, _f64, _vp, _vp]),
-    "chd_contact_detect": (_int, [_vp, _vp, _vp, _i32, _i32, _vp, _vp]),
+    "chd_contact_preprocess": (_int, [_vp, _vp, _vp, _i32, _f64, _f64, _vp, _vp]),
     "chd_contact_score_device": (_int, [_vp, _vp, _i32, _i32, _vp, _vp, C.c_float, _vp, _vp, _vp, _vp]),
-    "chd_contact_evaluate": (_int, [_vp, _vp, _vp, _i32, _f64, _f64, _vp, _vp, C.c_float, _vp, _vp, _vp, _vp, _vp]),
+    "chd_contact_detect": (_int, [_vp, _vp, _vp, _i32, _f64, _f64, _vp, _vp, C.c_float, _vp, _vp, _vp, _vp, _vp]),
     "chd_contact_launch_count": (_i64, [_vp]),
     "chd_contact_set_precision": (_int, [_vp, _i32]),
     "chd_openpose_load": (_int, [C.POINTER(C.c_char_p), _i32, _i32, _vp, _i32]),

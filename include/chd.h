@@ -175,24 +175,17 @@ int chd_contact_forward(chd_contact_net* net, const double* frames, int32_t V, i
 int chd_contact_forward_device(chd_contact_net* net, const double* frames_dev, int32_t V, int32_t Fmax,
                                const int32_t* seq_lens_dev, int64_t* labels_dev, float* logits_dev, float* min_abs_dev,
                                void* stream);
-/* Dataset preprocessing on the device (RealVideoDataset.__init__, real_video_dataset.py:132-163, and
- * process_openpose_data, openpose_dataset.py:49-121): raw [host] = concatenated OpenPose keypoints (sum F) x 25 x 3
- * doubles [x, y, confidence] as load_keypoint_dir returns them, seq_offsets [host] V+1 frame offsets, dim_w = width of
- * the source video (reference default 1920).  frames_out [host] V x Fmax x 25 x 3 (Fmax = longest video),
- * seq_lens_out [host, optional] V.  Bit identical to the reference's numpy result. */
-int chd_contact_preprocess(chd_contact_net* net, const double* raw, const int32_t* seq_offsets, int32_t V, int32_t dim_w,
-                           double* frames_out, int32_t* seq_lens_out);
-/* The same with the two dataset constants as arguments: xy is multiplied by `scale` before the interpolation and divided
- * by `norm` after it.  chd_contact_preprocess is this with scale = 1280 / dim_w, norm = 200.4160302695367; the synthetic
- * dataset (OpenPoseDataset, openpose_dataset.py:126-269) uses scale = 1 (exact) and norm = the median MidHip -> LBigToe
- * distance of its raw keypoints.  Returns -1 for scale or norm not > 0. */
-int chd_contact_preprocess_scaled(chd_contact_net* net, const double* raw, const int32_t* seq_offsets, int32_t V, double scale,
-                                  double norm, double* frames_out, int32_t* seq_lens_out);
-/* test.py --full-video --save-contacts --real-data in one call: raw keypoints in, foot_contacts rows out.
- * labels_out [host] (sum F) x 4 int64 (columns L heel, L toe, R heel, R toe; the rows every video's foot_contacts.npy
- * holds, concatenated).  raw may be page-locked: the upload is asynchronous on the net's stream. */
-int chd_contact_detect(chd_contact_net* net, const double* raw, const int32_t* seq_offsets, int32_t V, int32_t dim_w,
-                       int64_t* labels_out, float* min_abs_logit);
+/* Dataset preprocessing on the device (RealVideoDataset.__init__, real_video_dataset.py:132-163, OpenPoseDataset,
+ * openpose_dataset.py:126-269, and process_openpose_data, openpose_dataset.py:49-121): raw [host] = concatenated
+ * OpenPose keypoints (sum F) x 25 x 3 doubles [x, y, confidence] as load_keypoint_dir returns them, seq_offsets [host]
+ * V+1 frame offsets.  Videos are padded to the longest one, xy is multiplied by `scale` before the low-confidence
+ * interpolation and divided by `norm` after it.  Real videos use scale = 1280.0 / width of the source video (reference
+ * default 1920) and norm = 200.4160302695367, both in double; the synthetic dataset uses scale = 1 (exact) and norm =
+ * the median MidHip -> LBigToe distance of its raw keypoints.  frames_out [host] V x Fmax x 25 x 3 (Fmax = longest
+ * video), seq_lens_out [host, optional] V.  Bit identical to the reference's numpy result.  Returns -1 for scale or
+ * norm not > 0. */
+int chd_contact_preprocess(chd_contact_net* net, const double* raw, const int32_t* seq_offsets, int32_t V, double scale,
+                           double norm, double* frames_out, int32_t* seq_lens_out);
 /* Scores the logits of chd_contact_forward_device against ground-truth contacts (test.py:51-152 val_full_video with
  * labels), one CTA per video, on `stream` after the forward.  logits_dev [device] V x (Fmax-8) x 20 as the forward leaves
  * them; truth_dev [device] int32 (sum of rows) x 4, video v owning rows truth_offsets_dev[v] .. [v+1]-1
@@ -210,15 +203,20 @@ int chd_contact_detect(chd_contact_net* net, const double* raw, const int32_t* s
 int chd_contact_score_device(chd_contact_net* net, const float* logits_dev, int32_t V, int32_t Fmax, const int32_t* truth_dev,
                              const int32_t* truth_offsets_dev, float classify_thresh, double* loss_sum_dev,
                              int64_t* conf_frames_dev, int64_t* conf_merged_dev, void* stream);
-/* The labelled counterpart of chd_contact_detect (test.py --full-video with ground truth): one upload of the raw
- * keypoints and the truth, then preprocessing (chd_contact_preprocess_scaled's scale / norm), forward, vote, score and
- * pack on the net's stream, then one download.  truth [host] int32 (sum of rows) x 4 (may be NULL when there are no
- * rows), truth_offsets [host] V+1 starting at 0; labels_out [host] (sum F) x 4 int64 as chd_contact_detect; loss_sum
- * [host] V, conf_frames [host] V x 5 x 4, conf_merged [host] V x 4 as chd_contact_score_device; min_abs_logit [host,
- * optional].  Either precision mode.  Returns 0, -1 bad argument, <= -100 CUDA error. */
-int chd_contact_evaluate(chd_contact_net* net, const double* raw, const int32_t* seq_offsets, int32_t V, double scale, double norm,
-                         const int32_t* truth, const int32_t* truth_offsets, float classify_thresh, int64_t* labels_out,
-                         double* loss_sum, int64_t* conf_frames, int64_t* conf_merged, float* min_abs_logit);
+/* test.py --full-video in one call: raw keypoints in, foot_contacts rows out, and with ground truth also the scores.
+ * One upload of the raw keypoints (and the truth), then preprocessing (chd_contact_preprocess's scale / norm), forward,
+ * vote, (score) and pack on the net's stream, then one download.  raw may be page-locked: the copies are asynchronous.
+ * labels_out [host] (sum F) x 4 int64 (columns L heel, L toe, R heel, R toe; the rows every video's foot_contacts.npy
+ * holds, concatenated); min_abs_logit [host, optional].
+ *   Unlabelled (test.py --save-contacts --real-data): truth_offsets = NULL.  Nothing is scored; truth, classify_thresh,
+ *   loss_sum, conf_frames and conf_merged are ignored and may be NULL.
+ *   Labelled: truth [host] int32 (sum of rows) x 4 (may be NULL when there are no rows), truth_offsets [host] V+1
+ *   starting at 0, non-decreasing; loss_sum [host] V, conf_frames [host] V x 5 x 4, conf_merged [host] V x 4 as
+ *   chd_contact_score_device writes them for classify_thresh.
+ * Either precision mode.  Returns 0, -1 bad argument, <= -100 CUDA error. */
+int chd_contact_detect(chd_contact_net* net, const double* raw, const int32_t* seq_offsets, int32_t V, double scale, double norm,
+                       const int32_t* truth, const int32_t* truth_offsets, float classify_thresh, int64_t* labels_out,
+                       double* loss_sum, int64_t* conf_frames, int64_t* conf_merged, float* min_abs_logit);
 int64_t chd_contact_launch_count(const chd_contact_net* net);
 /* Numerical mode of every later chd_contact_forward / _forward_device / _detect call on this net.
  * FP32 (default): FFMA, labels match the reference's fp32 forward.  TF32X3: the 352-1024-512-128 layers on the

@@ -50,21 +50,22 @@ def interpolate_low_confidence(seq, thresh=0.2):
     return seq
 
 
-def preprocess_videos(raw, dimensions=(1920, 1080)):
+def preprocess_videos(raw, dimensions=(1920, 1080), scale=None, norm=TRAIN_NORMALIZATION):
     """RealVideoDataset.__init__ (real_video_dataset.py:132-163): pad every video to the longest by repeating the last
-    frame, scale xy by 1280/width, interpolate low-confidence joints, divide xy by the training normalisation.
+    frame, scale xy by `scale` (default 1280/width), interpolate low-confidence joints, divide xy by `norm` (default the
+    training normalisation; the synthetic dataset passes scale 1 and its median).
     Returns (frames (V,Fmax,25,3) fp64, seq_lens (V,) int32)."""
     seq_lens = np.array([r.shape[0] for r in raw], dtype=np.int32)
     Fmax = int(seq_lens.max())
     out = np.zeros((len(raw), Fmax, 25, 3))
-    scale = float(TRAIN_DIM[0]) / dimensions[0]
+    scale = float(TRAIN_DIM[0]) / dimensions[0] if scale is None else scale
     for i, r in enumerate(raw):
         a = np.array(r, dtype=np.float64)
         if a.shape[0] < Fmax:
             a = np.concatenate([a, np.repeat(a[-1:], Fmax - a.shape[0], axis=0)], axis=0)
         a[:, :, :2] *= scale
         a = interpolate_low_confidence(a, 0.2)
-        a[:, :, :2] /= TRAIN_NORMALIZATION
+        a[:, :, :2] /= norm
         out[i] = a
     return out, seq_lens
 

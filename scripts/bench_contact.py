@@ -11,6 +11,7 @@ e2e   : windows/s through the public host call `ContactNet.detect` (`chd_contact
 import argparse
 import json
 import os
+import subprocess
 import sys
 import time
 
@@ -29,6 +30,19 @@ def make_raw(n):
     rng = np.random.default_rng(0)
     base = [synth_keypoints(i, F) for i in range(8)]
     return [base[i % 8] + rng.normal(0, 0.5, base[0].shape) * np.array([1, 1, 0]) for i in range(n)]
+
+
+def card():
+    """Name, power limit and maximum SM clock of cuda:0, to state beside numbers measured in the same run."""
+    import torch
+    out = {"name": torch.cuda.get_device_name(0), "power_limit_w": None, "max_sm_clock_mhz": None}
+    try:
+        q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader,nounits", "-i", "0"],
+                           capture_output=True, text=True, timeout=30).stdout.strip().split(",")
+        out["power_limit_w"], out["max_sm_clock_mhz"] = float(q[0]), float(q[1])
+    except Exception as e:                                     # reported, not guessed
+        out["query_error"] = repr(e)
+    return out
 
 
 def cpu_arm(raw, sd, threads):

@@ -9,24 +9,24 @@ device_resident     : windows/s of forward + vote + score and of forward + vote,
 e2e                 : windows/s of ContactNet.evaluate from page-locked raw keypoints (upload, prep, forward, vote,
                       score, pack, download)
 cpu_baseline        : the oracle arm (numpy preprocessing, torch fp32 CPU forward, numpy scoring) on --cpu-videos videos
-gpu                 : card name and power limit, read in the same run
+gpu                 : card name, power limit and max SM clock, read in the same run
 
     python scripts/bench_contact_eval.py --steps 30 --warmup 5
 """
 import argparse
 import json
 import os
-import subprocess
 import sys
 import tempfile
 import time
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "scripts"))
 sys.path.insert(0, os.path.join(ROOT, "tests", "golden"))
 import numpy as np
 
-V, F = 1000, 108
+from bench_contact import F, V, card
 
 
 def make_videos(chd):
@@ -40,30 +40,14 @@ def make_videos(chd):
     return raw, truth, s.scale, s.norm
 
 
-def gpu_info():
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True, timeout=30)
-        name, power = [x.strip() for x in q.stdout.strip().splitlines()[0].split(",")]
-        return {"name": name, "power_limit": power}
-    except Exception as e:     # the number is still the card's; say that the limit could not be read
-        import torch
-        return {"name": torch.cuda.get_device_name(0), "power_limit": "not read (%s)" % type(e).__name__}
-
-
 def cpu_arm(raw, truth, scale, norm, sd, threads):
     import torch
     from oracle import contact as oc
     from oracle.contact_eval import score
     torch.set_num_threads(threads)
     t0 = time.perf_counter()
-    frames = []
-    for r in raw:
-        a = np.array(r, dtype=np.float64)
-        a[:, :, :2] *= scale
-        a = oc.interpolate_low_confidence(a, 0.2)
-        a[:, :, :2] /= norm
-        frames.append(a)
-    logits = oc.forward_torch(sd, oc.windows_from_frames(np.stack(frames)))
+    frames, _ = oc.preprocess_videos(raw, scale=scale, norm=norm)
+    logits = oc.forward_torch(sd, oc.windows_from_frames(frames))
     res = [score(logits[i], truth[i]) for i in range(len(raw))]
     return time.perf_counter() - t0, res
 
@@ -158,7 +142,7 @@ def main():
                       "mean_loss": res["mean_loss"], "min_abs_logit": res["min_abs_logit"],
                       "cpu_baseline": {"value": ns * (F - 8) / cpu_t, "unit": "windows/s", "threads": cores, "videos": ns, "seconds": cpu_t,
                                        "counts_equal_frac_vs_gpu": agree},
-                      "gpu": gpu_info()}))
+                      "gpu": card()}))
 
 
 if __name__ == "__main__":

@@ -14,7 +14,6 @@ and the smallest |fp32 logit| of each video whose labels differ.
 import argparse
 import json
 import os
-import subprocess
 import sys
 import time
 
@@ -24,23 +23,11 @@ sys.path.insert(0, os.path.join(ROOT, "scripts"))
 sys.path.insert(0, os.path.join(ROOT, "tests", "golden"))
 import numpy as np
 
-from bench_contact import CONFIG, F, V, make_raw
+from bench_contact import CONFIG, F, V, card, make_raw
 
 FLOP_PER_WINDOW = 2 * 953984                                   # all five layers, as counted by bench_contact.py
 TC_MAC_PER_WINDOW = 352 * 1024 + 1024 * 512 + 512 * 128        # the three tensor-core layers (K of layer 0 padded to 352)
 MODES = ("fp32", "tf32x3")
-
-
-def card():
-    import torch
-    out = {"name": torch.cuda.get_device_name(0), "power_limit_w": None, "max_sm_clock_mhz": None}
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader,nounits", "-i", "0"],
-                           capture_output=True, text=True, timeout=30).stdout.strip().split(",")
-        out["power_limit_w"], out["max_sm_clock_mhz"] = float(q[0]), float(q[1])
-    except Exception as e:                                     # reported, not guessed
-        out["query_error"] = repr(e)
-    return out
 
 
 def stats(ts):

@@ -1,5 +1,5 @@
-"""Labelled evaluation of the contact classifier on the GPU (`chd_contact_evaluate`, `chd_k_contact_score`) against the
-counts and loss the reference's own val_full_video produced (tests/golden/make_contact_eval_golden.py)."""
+"""Labelled evaluation of the contact classifier on the GPU (`chd_contact_detect` with truth, `chd_k_contact_score`)
+against the counts and loss the reference's own val_full_video produced (tests/golden/make_contact_eval_golden.py)."""
 import json
 import os
 import subprocess
