@@ -160,15 +160,15 @@ int run_schedule(chd_phys_batch* b) {
     {
       Timer t(b, KT_INIT);
       chd_k_hess_zero<<<dim3(8, B), 256, 0, b->stream>>>(b->D);
-      chd_k_hess_base<<<dim3(8, B), CHD_THREADS, 0, b->stream>>>(b->D);
+      chd_k_hess_base<<<dim3(16, B), 256, 0, b->stream>>>(b->D);
       chd_k_hess_fin<<<B, 128, 0, b->stream>>>(b->D, 0);
       b->launches += 2;
     }
-    if (it > 0) {
-      CHD_CUDA(cudaStreamWaitEvent(b->stream, b->ev_copy, 0));   // Kwork refreshed by the side stream
-      chd_k_asm<<<dim3(8, B), 256, 0, b->stream>>>(b->D);     // matrix entries of the sequences that continue in their stage
-      b->launches++;
-    }
+    // Kwork refreshed by the side stream (iteration 0: the event has not been recorded yet and the wait is a no-op; the
+    // sequences that begin a stage had Kwork prepared by the chd_k_hess_* kernels above)
+    CHD_CUDA(cudaStreamWaitEvent(b->stream, b->ev_copy, 0));
+    chd_k_asm<<<dim3(8, B), 256, 0, b->stream>>>(b->D);
+    b->launches++;
     {
       Timer t(b, KT_KKT);
       if (b->D.win_smem) chd_k_kkt<<<B, CHD_KKT_THREADS, b->smem_kkt, b->stream>>>(b->D);
@@ -351,6 +351,8 @@ static int batch_create_impl(const chd_phys_problem* problems, int32_t batch, co
   const size_t kkt_fixed = (CHD_KKT_THREADS + nbp8 * nbp8 + (size_t)D.pan_doubles + 16) * sizeof(double);
   const size_t kkt_win = ((size_t)D.win_tiles * 64 + (size_t)D.Q * D.nbt * 64) * sizeof(double);
   CHD_CUDA(cudaDeviceGetAttribute(&smem_max, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+  // (+ 3072: chd_k_kkt's former distance-row curvature scratch; it guards nothing now, but dropping it would move
+  // borderline batches from chd_k_kkt_gwin onto chd_k_kkt)
   const bool vectors_fit = (size_t)D.win_tiles * 64 + (size_t)D.Q * D.nbt * 64 >= n_even + xs_len + 2 * (size_t)D.Q * 64 + 3072;
   if (vectors_fit && kkt_fixed + kkt_win + kkt_static + 256 <= (size_t)smem_max) {
     D.win_smem = 1;
@@ -554,7 +556,7 @@ int chd_phys_solve_stage(chd_phys_batch* b, int32_t stage, int32_t max_iter, int
       double* s = stats + 8 * i;
       s[0] = I.f, s[1] = I.E0, s[2] = I.viol_u, s[3] = I.dual_u, s[4] = I.compl_u, s[5] = I.mu, s[6] = I.delta_w, s[7] = I.ls_fail;
     }
-    if (i == 0 && getenv("CHD_PROF")) fprintf(stderr, "chd prof (Mcycles) seq0 stage %d: err %.2f jasm %.2f hasm %.2f factor %.2f border %.2f back %.2f rec %.2f\n", stage, I.prof[0]/1e6, I.prof[1]/1e6, I.prof[2]/1e6, I.prof[3]/1e6, I.prof[4]/1e6, I.prof[5]/1e6, I.prof[6]/1e6);
+    if (i == 0 && getenv("CHD_PROF")) fprintf(stderr, "chd prof (Mcycles) seq0 stage %d: err %.2f asm %.2f factor %.2f border %.2f back %.2f rec %.2f\n", stage, I.prof[0]/1e6, I.prof[1]/1e6, I.prof[2]/1e6, I.prof[3]/1e6, I.prof[4]/1e6, I.prof[5]/1e6);
   }
   return 0;
 }

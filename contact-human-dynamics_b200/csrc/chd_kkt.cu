@@ -1,15 +1,16 @@
 // KKT kernels of the batched interior-point solver (product code, sm_90a).
 //
 //   chd_k_hess_base : once per stage -- Gauss-Newton Hessian of the (quadratic, fixed-duration) cost terms
-//                     of data_cost.cpp / vel_smooth_cost.cpp, scaled by the objective scaling, in tile format (Kbase)
+//                     of data_cost.cpp / vel_smooth_cost.cpp, scaled by the objective scaling, in tile format (Kbase);
+//                     with chd_k_hess_zero it also prepares Kwork of the stage's first iteration
 //   chd_k_kcopy     : per iteration, side stream -- Kwork <- Kbase for the sequences that continue in their stage
 //   chd_k_curv      : per iteration, side stream, after the line search -- y+ Jd^T Jd of the squared-distance rows
 //   chd_k_asm       : per iteration, right before chd_k_kkt -- Jacobian dependent matrix entries and the right-hand
 //                     side as rhs0 + mu * rhs1 (several CTAs per sequence: the cost is the L2 reductions)
-//   chd_k_kkt       : per iteration, one CTA per sequence -- IPOPT error measures + barrier update, (first iteration
-//                     of a stage: the whole assembly), tiled band LDL^T with dense border (shared-memory window or,
-//                     for wide bands, in place on Kwork; panel, trailing and corner updates on the FP64 tensor
-//                     core), triangular solves, step recovery and fraction-to-the-boundary rule
+//   chd_k_kkt       : per iteration, one CTA per sequence -- IPOPT error measures + barrier update, tiled band LDL^T
+//                     with dense border (shared-memory window or, for wide bands, in place on Kwork; panel, trailing
+//                     and corner updates on the FP64 tensor core), triangular solves, step recovery and
+//                     fraction-to-the-boundary rule
 //   chd_k_fp64_peak : DFMA / DMMA throughput probe for the roofline denominators of bench.py
 // Replaces IPOPT's per-iteration MA57 factorisation (phys_optim.cpp:573) for the block-banded systems this NLP
 // produces.
@@ -122,18 +123,12 @@ __device__ void chd_hess_clear(const ChdDev& D, int b, double* base, int part, i
   double2* dst = reinterpret_cast<double2*>(base);
   for (size_t i = lo + threadIdx.x; i < hi; i += blockDim.x) dst[i] = make_double2(0.0, 0.0);
 }
+// zero fill of the right-hand-side accumulators of chd_k_asm of sequence b, by one CTA
+__device__ void chd_rhs_clear(const ChdDev& D, int b) {
+  const size_t go = (size_t)b * (D.Na_max + D.nb_max);
+  for (int i = threadIdx.x; i < D.Na_max + D.nb_max; i += blockDim.x) D.rhs0[go + i] = 0.0, D.rhs1[go + i] = 0.0;
+}
 
-// stage begin, grid (G, B): Kbase <- 0, then the cost Hessian, then (one CTA per sequence) the flags + BEGIN -> RUN
-__global__ void __launch_bounds__(256) chd_k_hess_zero(ChdDev D) {
-  const int b = blockIdx.y;
-  if (D.ipm[b].phase != CHD_PH_BEGIN) return;
-  chd_hess_clear(D, b, D.Kbase + (size_t)b * D.kstride, blockIdx.x, gridDim.x);
-}
-__global__ void __launch_bounds__(CHD_THREADS) chd_k_hess_base(ChdDev D) {
-  const int b = blockIdx.y;
-  if (D.ipm[b].phase != CHD_PH_BEGIN) return;
-  chd_hess_build(D, b, D.stages[D.ipm[b].stage], D.Kbase + (size_t)b * D.kstride, blockIdx.x, gridDim.x);
-}
 // stage 3, every iteration after the line search (side stream, grid (G, B)): the cost Hessian at the accepted iterate
 // goes straight into Kwork, which chd_k_kcopy has zeroed for the sequences of that stage
 __global__ void __launch_bounds__(CHD_THREADS) chd_k_hess_dur(ChdDev D) {
@@ -178,8 +173,8 @@ __global__ void __launch_bounds__(128) chd_k_hess_fin(ChdDev D, int mode) {
 
 // y^+ * Jd^T Jd of the squared-distance rows (leg length, toe-heel distance) of sequence b added into K: one warp
 // per active row, rows dealt round-robin to `nw` warps of which this is number `wid`.  ws: 192 doubles of per-warp
-// scratch, slot -> (kkt index, weight, 3-vector column of Jd).  Called from chd_k_kkt (first iteration of a stage)
-// and from chd_k_curv (all later iterations, side stream).
+// scratch, slot -> (kkt index, weight, 3-vector column of Jd).  Called from chd_k_hess_base (first iteration of a
+// stage) and from chd_k_curv (all later iterations, side stream).
 __device__ __forceinline__ void chd_curv_rows(const ChdDev& D, int b, const ChdKT& K, const ChdStageDev& sg, int wid, int nw, int lane,
                                               double* ws) {
   const ChdSeq* h = D.seq + b;
@@ -269,16 +264,46 @@ __device__ __forceinline__ void chd_curv_rows(const ChdDev& D, int b, const ChdK
   }
 }
 
-// Assembly of the condensed KKT system of sequence b by threads t0, t0 + tstep, ...: matrix entries (do_mat; global
-// reductions into K) and / or right-hand side (rhs_s != nullptr; shared-memory atomics, [0, Np) band unknowns,
-// [8*nbc_max, +nb) border unknowns).  Narrow inequality rows (<= 12 slots: terrain, friction pyramid, height) are
-// condensed into the primal block (J^T Sigma J); wide ones (leg length) keep their multiplier as an unknown with
-// diagonal -1/Sigma, which needs 36 instead of 666 matrix updates per row.
-// (A per-column gather of the right-hand side, as in section A, was measured slower than the shared-memory atomics.)
-// g0 / g1 (global, chd_k_asm): the right-hand side split as rhs = g0 + mu * g1 -- every term is affine in the barrier
-// parameter, which is only decided inside chd_k_kkt -- accumulated with global reductions.
-__device__ __forceinline__ void chd_assemble(const ChdDev& D, int b, const ChdKT& K, double delta_w, double mu, double sf, double* rhs_s,
-                                             bool do_mat, int t0, int tstep, double* g0 = nullptr, double* g1 = nullptr) {
+// Stage begin, grid (G, B), sequences in CHD_PH_BEGIN: what chd_k_kcopy, chd_k_hess_dur and chd_k_curv prepare for
+// every later iteration, so that chd_k_asm and chd_k_kkt see the first iteration of a stage like any other --
+// Kbase, Kwork, rhs0, rhs1 <- 0 (chd_k_hess_zero); the distance-row curvature at the initial point (x, y, scaling
+// are final after chd_k_init; y != 0 in a warm-started stage 3) into Kwork, then the cost Hessian into Kbase and
+// Kwork (chd_k_hess_base; this order spills less); the flags and BEGIN -> RUN (chd_k_hess_fin, mode 0).
+// kw_req stays 0 here: the side-stream kernels of the previous iteration may still be running, and they leave the
+// Kwork / rhs0 / rhs1 of a sequence whose stage just ended alone only because chd_stage_advance cleared its kw_req
+// before they were launched.
+__global__ void __launch_bounds__(256) chd_k_hess_zero(ChdDev D) {
+  const int b = blockIdx.y;
+  if (D.ipm[b].phase != CHD_PH_BEGIN) return;
+  chd_hess_clear(D, b, D.Kbase + (size_t)b * D.kstride, blockIdx.x, gridDim.x);
+  chd_hess_clear(D, b, D.Kwork + (size_t)b * D.kstride, blockIdx.x, gridDim.x);
+  if (blockIdx.x == 0) chd_rhs_clear(D, b);
+}
+// (256 threads, two CTAs per SM, grid (16, B): launched every iteration, its CTAs exit at once for the sequences that
+// do not begin a stage, but each needs its registers free before it starts -- with 512 threads at 128 registers that
+// is a whole SM, so they would wait for the side-stream kernels of the previous iteration to drain)
+__global__ void __launch_bounds__(256, 2) chd_k_hess_base(ChdDev D) {
+  __shared__ double s_ws[8][192];
+  const int b = blockIdx.y;
+  if (D.ipm[b].phase != CHD_PH_BEGIN) return;
+  const ChdStageDev sg = D.stages[D.ipm[b].stage];
+  ChdKT K;
+  chd_kt_init(D, D.seq + b, D.Kwork + (size_t)b * D.kstride, K);
+  K.ovf = &D.ipm[b].band_ovf;
+  const int warp = threadIdx.x >> 5, nwarp = blockDim.x >> 5;
+  chd_curv_rows(D, b, K, sg, blockIdx.x * nwarp + warp, gridDim.x * nwarp, threadIdx.x & 31, s_ws[warp]);
+  chd_hess_build(D, b, sg, D.Kbase + (size_t)b * D.kstride, blockIdx.x, gridDim.x);
+  chd_hess_build(D, b, sg, D.Kwork + (size_t)b * D.kstride, blockIdx.x, gridDim.x);
+}
+
+// Jacobian-dependent part of the condensed KKT system of sequence b by threads t0, t0 + tstep, ...: matrix entries
+// (global reductions into K) and the right-hand side split as rhs = g0 + mu * g1 -- every term is affine in the
+// barrier parameter, which is only decided inside chd_k_kkt -- accumulated with global reductions.  Narrow inequality
+// rows (<= 12 slots: terrain, friction pyramid, height) are condensed into the primal block (J^T Sigma J); wide ones
+// (leg length) keep their multiplier as an unknown with diagonal -1/Sigma, which needs 36 instead of 666 matrix
+// updates per row.
+__device__ __forceinline__ void chd_assemble(const ChdDev& D, int b, const ChdKT& K, double delta_w, double sf, int t0, int tstep,
+                                             double* g0, double* g1) {
   const ChdSeq* h = D.seq + b;
   const int n = D.stages[D.ipm[b].stage].opt_dur ? h->n : h->n - h->n_dur;   // the durations are unknowns in stage 3 only
   const int m = h->m, Na = K.Na;
@@ -290,14 +315,10 @@ __device__ __forceinline__ void chd_assemble(const ChdDev& D, int b, const ChdKT
   const int* ec = D.ent_col + (size_t)b * D.slots_max;
   const double* Jv = D.Jv + (size_t)b * D.slots_max;
   const double* grad = D.grad + vo;
-  auto rhs_add = [&](int kk, double v) { if (rhs_s) atomicAdd(rhs_s + (kk < Na ? kk : 8 * D.nbc_max + (kk - Na)), v); };
-  auto mat_add = [&](int i, int j, double v) { if (do_mat) chd_kadd(K, i, j, v); };
   auto gidx = [&](int kk) { return kk < Na ? kk : D.Na_max + (kk - Na); };
   auto g_add = [&](int kk, double v0, double v1) {
-    if (g0) {
-      atomicAdd(g0 + gidx(kk), v0);
-      if (v1 != 0.0) atomicAdd(g1 + gidx(kk), v1);
-    }
+    atomicAdd(g0 + gidx(kk), v0);
+    if (v1 != 0.0) atomicAdd(g1 + gidx(kk), v1);
   };
   // foot-motion node values that no cost sample sees (polynomials shorter than a frame): without curvature of their own
   // the Newton step uses them as free slack and they drift by orders of magnitude, which stage 3 (where the sample
@@ -307,38 +328,33 @@ __device__ __forceinline__ void chd_assemble(const ChdDev& D, int b, const ChdKT
   for (int i = t0; i < n; i += tstep) {
     const int k = vk[i];
     if (k < 0) continue;
-    if (do_mat && unobs[i]) mat_add(k, k, CHD_DW_UNOBS);
-    mat_add(k, k, delta_w);
-    rhs_add(k, -sf * grad[i]);
+    if (unobs[i]) chd_kadd(K, k, k, CHD_DW_UNOBS);
+    chd_kadd(K, k, k, delta_w);
     g_add(k, -sf * grad[i], 0.0);
   }
   for (int r = t0; r < m; r += tstep) {
     const int f = rf[r];
     const int k = rk[r];
     if (!(f & CHD_ROW_ACTIVE)) {
-      if (k >= 0) mat_add(k, k, -1.0);   // row of an inactive set: decoupled dummy unknown
+      if (k >= 0) chd_kadd(K, k, k, -1.0);   // row of an inactive set: decoupled dummy unknown
       continue;
     }
     const double sc = D.sc[ro + r];
     const int e0 = ep[r], e1 = ep[r + 1];
     if (k >= 0) {
       // explicit row: equality, or wide inequality with its slack eliminated
-      double diag = -CHD_DELTA_C, rr, rr0, rr1 = 0.0;
+      double diag = -CHD_DELTA_C, rr0, rr1 = 0.0;
       if (f & CHD_ROW_EQ) {
-        rr = -(sc * D.g[ro + r] - D.dL[ro + r]);
-        rr0 = rr;
+        rr0 = -(sc * D.g[ro + r] - D.dL[ro + r]);
       } else {
         const double s = D.s[ro + r];
         const double gapL = (f & CHD_ROW_HASL) ? s - D.dL[ro + r] : 1.0, gapU = (f & CHD_ROW_HASU) ? D.dU[ro + r] - s : 1.0;
         const double Sig = ((f & CHD_ROW_HASL) ? D.zL[ro + r] / gapL : 0.0) + ((f & CHD_ROW_HASU) ? D.zU[ro + r] / gapU : 0.0);
-        const double bvec = ((f & CHD_ROW_HASL) ? mu / gapL : 0.0) - ((f & CHD_ROW_HASU) ? mu / gapU : 0.0);
         diag -= 1.0 / Sig;
-        rr = -(sc * D.g[ro + r] - s) + (D.y[ro + r] + bvec) / Sig;
         rr0 = -(sc * D.g[ro + r] - s) + D.y[ro + r] / Sig;
         rr1 = (((f & CHD_ROW_HASL) ? 1.0 / gapL : 0.0) - ((f & CHD_ROW_HASU) ? 1.0 / gapU : 0.0)) / Sig;
       }
-      mat_add(k, k, diag);
-      rhs_add(k, rr);
+      chd_kadd(K, k, k, diag);
       g_add(k, rr0, rr1);
       const double ys = sc * D.y[ro + r];
       for (int e = e0; e < e1; ++e) {
@@ -348,8 +364,7 @@ __device__ __forceinline__ void chd_assemble(const ChdDev& D, int b, const ChdKT
         if (kc < 0) continue;
         const double jv = Jv[e];
         if (jv == 0.0) continue;
-        mat_add(k, kc, sc * jv);
-        rhs_add(kc, -ys * jv);
+        chd_kadd(K, k, kc, sc * jv);
         g_add(kc, -ys * jv, 0.0);
       }
     } else {
@@ -357,8 +372,6 @@ __device__ __forceinline__ void chd_assemble(const ChdDev& D, int b, const ChdKT
       const double s = D.s[ro + r];
       const double gapL = (f & CHD_ROW_HASL) ? s - D.dL[ro + r] : 1.0, gapU = (f & CHD_ROW_HASU) ? D.dU[ro + r] - s : 1.0;
       const double Sig = ((f & CHD_ROW_HASL) ? D.zL[ro + r] / gapL : 0.0) + ((f & CHD_ROW_HASU) ? D.zU[ro + r] / gapU : 0.0);
-      const double bvec = ((f & CHD_ROW_HASL) ? mu / gapL : 0.0) - ((f & CHD_ROW_HASU) ? mu / gapU : 0.0);
-      const double coef = Sig * (sc * D.g[ro + r] - s) - bvec;
       const double coef0 = Sig * (sc * D.g[ro + r] - s);
       const double beta = ((f & CHD_ROW_HASL) ? 1.0 / gapL : 0.0) - ((f & CHD_ROW_HASU) ? 1.0 / gapU : 0.0);
       for (int ea = e0; ea < e1; ++ea) {
@@ -368,32 +381,18 @@ __device__ __forceinline__ void chd_assemble(const ChdDev& D, int b, const ChdKT
         if (ka < 0) continue;
         const double va = sc * Jv[ea];
         if (va == 0.0) continue;
-        rhs_add(ka, -va * coef);
         g_add(ka, -va * coef0, va * beta);
-        if (do_mat)
         for (int eb = e0; eb < e1; ++eb) {
           const int cb = ec[eb];
           if (cb < 0) continue;
           const int kb = vk[cb];
           if (kb < 0 || ka < kb) continue;
           const double vb = sc * Jv[eb];
-          if (vb != 0.0) mat_add(ka, kb, Sig * va * vb);
+          if (vb != 0.0) chd_kadd(K, ka, kb, Sig * va * vb);
         }
       }
     }
   }
-}
-
-// Kwork <- Kbase of sequence b: double2 elements i, i + nt, ... below hi (four independent 16-byte loads in flight per
-// thread).  Whole matrix inside chd_k_kkt on the first iteration of a stage, one slice per CTA in chd_k_kcopy.
-__device__ __forceinline__ void chd_kwork_copy(const ChdDev& D, int b, size_t i, size_t hi, size_t nt) {
-  const double2* src = reinterpret_cast<const double2*>(D.Kbase + (size_t)b * D.kstride);
-  double2* dst = reinterpret_cast<double2*>(D.Kwork + (size_t)b * D.kstride);
-  for (; i + 3 * nt < hi; i += 4 * nt) {
-    const double2 v0 = src[i], v1 = src[i + nt], v2 = src[i + 2 * nt], v3 = src[i + 3 * nt];
-    dst[i] = v0, dst[i + nt] = v1, dst[i + 2 * nt] = v2, dst[i + 3 * nt] = v3;
-  }
-  for (; i < hi; i += nt) dst[i] = src[i];
 }
 
 // What every phase of chd_k_kkt sees of its sequence: the thread's place in the CTA, the sequence's arrays and KKT
@@ -405,7 +404,6 @@ __device__ __forceinline__ void chd_kwork_copy(const ChdDev& D, int b, size_t i,
 struct ChdKktCtx {
   int b, tid, nt, lane, warp, nwarp;
   ChdIpm* I;
-  int pre_refreshed;   // Kwork = Kbase + distance-row curvature already prepared on the side stream
   ChdStageDev sg;
   const ChdSeq* h;
   int n, m, n_act, Qs, Q, nbt, nbp8, nbl, nbc, NBR, nbt_s;
@@ -423,7 +421,6 @@ __device__ __forceinline__ void chd_kkt_ctx_init(const ChdDev& D, ChdIpm& I, Chd
   extern __shared__ double sm[];
   const int b = blockIdx.x;
   c.b = b, c.I = &I;
-  c.pre_refreshed = I.kw_req;
   c.sg = D.stages[I.stage];
   const ChdSeq* h = c.h = D.seq + b;
   c.n = h->n, c.m = h->m, c.tid = threadIdx.x, c.nt = blockDim.x;
@@ -456,9 +453,8 @@ __device__ __forceinline__ void chd_kkt_ctx_init(const ChdDev& D, ChdIpm& I, Chd
   c.ypan = c.cc + c.nbp8 * c.nbp8;
   c.xpan = c.ypan + (c.Q + c.nbt) * 64;
   c.dinv = c.ypan + D.pan_doubles;
-  // WS: the per-unknown vectors vecn (step recovery) and xs (right-hand side before, solution after the factorisation)
-  // alias the tail of the window region, which is dead whenever they are live (the right-hand side moves into the border
-  // storage before the window is loaded; the back-substitution stages its tiles in the front part only)
+  // WS: the per-unknown vectors vecn (step recovery) and xs (solution after the factorisation) alias the tail of the
+  // window region, which is dead whenever they are live (the back-substitution stages its tiles in the front part only)
   c.win_region = (size_t)D.win_tiles * 64 + (size_t)c.Qs * c.nbt * 64;
   c.win = WS ? c.dinv + 16 : gs + c.n_even + c.xs_len + 8 * (size_t)D.nbc_max;
   c.bwin = c.win + (size_t)D.win_tiles * 64;
@@ -588,41 +584,25 @@ __device__ __forceinline__ bool chd_kkt_errors(const ChdDev& D, ChdKktCtx& c, in
   return false;
 }
 
-// B. assembly of the KKT system (the distance-row curvature terms follow separately, see chd_kkt_body).
-// Narrow inequality rows (<= 12 slots: terrain, friction pyramid, height) are condensed into the primal block
-// (J^T Sigma J); wide ones (leg length) keep their multiplier as an unknown with diagonal
-// -1/Sigma, which needs 36 instead of 666 matrix updates per row.  The right-hand side is accumulated in
-// shared memory (xs) and written out once.
+// B. what this iteration's barrier parameter and step rule decide of the KKT system, which chd_k_asm has assembled
+// otherwise: a feasibility-polish step tops up the adaptive weight chd_k_asm put on the diagonal, and the right-hand
+// side rhs0 + mu * rhs1 goes into border row NBR (band unknowns) and corner row NBR (border unknowns).
 __device__ __forceinline__ void chd_kkt_assemble(const ChdDev& D, const ChdKktCtx& c) {
   const ChdIpm& I = *c.I;
   const ChdKT& K = c.K;
-  const int b = c.b, tid = c.tid, nt = c.nt, n_act = c.n_act, nbl = c.nbl, nbt = c.nbt, nbp8 = c.nbp8, NBR = c.NBR;
+  const int tid = c.tid, nt = c.nt, n_act = c.n_act, nbl = c.nbl, nbt = c.nbt, nbp8 = c.nbp8, NBR = c.NBR, Na = K.Na;
   const int* vk = c.vk;
   const double mu = c.mu;
-  if (!c.pre_refreshed) chd_kwork_copy(D, b, tid, D.kstride / 2, nt);   // first iteration of a stage; afterwards chd_k_kcopy refreshes Kwork on the side stream
-  const int Na = K.Na;
-  double* rhs_s = c.xs;   // [0, Np) band unknowns, [8*nbc_max, +nb) border unknowns
-  for (int i = tid; i < 8 * D.nbc_max + nbp8; i += nt) rhs_s[i] = 0.0;
-  __syncthreads();
-  // matrix entries do not depend on the barrier parameter: for sequences that continue in their stage they were
-  // added by chd_k_asm (8 CTAs per sequence) before this kernel; the right-hand side (shared-memory atomics) is
-  // always assembled here
-  if (c.pre_refreshed && c.polish) {   // chd_k_asm put the adaptive weight on the diagonal: top it up
+  if (c.polish) {
     const double extra = c.delta_w - I.delta_w;
     for (int i = tid; i < n_act; i += nt)
       if (vk[i] >= 0) chd_kadd(K, vk[i], vk[i], extra);
   }
-  if (c.pre_refreshed) {
-    const double* r0 = D.rhs0 + (size_t)b * (D.Na_max + D.nb_max);
-    const double* r1 = D.rhs1 + (size_t)b * (D.Na_max + D.nb_max);
-    for (int i = tid; i < Na; i += nt) rhs_s[i] = r0[i] + mu * r1[i];
-    for (int i = tid; i < nbl; i += nt) rhs_s[8 * D.nbc_max + i] = r0[D.Na_max + i] + mu * r1[D.Na_max + i];
-  } else {
-    chd_assemble(D, b, K, c.delta_w, mu, c.sf, rhs_s, true, tid, nt);
-  }
-  __syncthreads();
-  for (int i = tid; i < K.Np; i += nt) K.bord[((size_t)(i >> 3) * nbt + (NBR >> 3)) * 64 + (NBR & 7) * 8 + (i & 7)] = i < Na ? rhs_s[i] : 0.0;
-  for (int i = tid; i < nbl; i += nt) K.corn[(size_t)NBR * nbp8 + i] = rhs_s[8 * D.nbc_max + i];
+  const double* r0 = D.rhs0 + (size_t)c.b * (D.Na_max + D.nb_max);
+  const double* r1 = D.rhs1 + (size_t)c.b * (D.Na_max + D.nb_max);
+  for (int i = tid; i < K.Np; i += nt)
+    K.bord[((size_t)(i >> 3) * nbt + (NBR >> 3)) * 64 + (NBR & 7) * 8 + (i & 7)] = i < Na ? r0[i] + mu * r1[i] : 0.0;
+  for (int i = tid; i < nbl; i += nt) K.corn[(size_t)NBR * nbp8 + i] = r0[D.Na_max + i] + mu * r1[D.Na_max + i];
 }
 
 // Trailing updates C -= X Y^T of one block column by the warps 1 .. nwarp-1, for at most 64 panel groups (every
@@ -1128,23 +1108,18 @@ __device__ __forceinline__ void chd_kkt_body(const ChdDev& D) {
   if (chd_kkt_errors(D, c, s_fail)) return;
   CHD_PROF(0);
   chd_kkt_assemble(D, c);
-  CHD_PROF(1);
-  // y^+ * Jd^T Jd of the squared-distance rows: in-kernel only on the first iteration of a stage, afterwards
-  // chd_k_curv has already added them on the side stream (many CTAs per sequence: the atomics are the cost)
-  if (!c.pre_refreshed) chd_curv_rows(D, c.b, c.K, c.sg, c.warp, c.nwarp, c.lane, c.win + c.warp * 192);
-  __threadfence_block();
   __syncthreads();
-  CHD_PROF(2);
+  CHD_PROF(1);
   chd_kkt_factor<WS>(c, s_fail);
-  CHD_PROF(3);
+  CHD_PROF(2);
   chd_kkt_border(D, c, s_fail);
-  CHD_PROF(4);
+  CHD_PROF(3);
   chd_kkt_backsub<WS>(D, c);
-  CHD_PROF(5);
+  CHD_PROF(4);
   if (chd_kkt_no_step(D, c, s_fail)) return;
   __syncthreads();
   chd_kkt_recover(D, c);
-  CHD_PROF(6);
+  CHD_PROF(5);
 }
 #undef CHD_PROF
 
@@ -1153,10 +1128,7 @@ __device__ __forceinline__ void chd_kkt_body(const ChdDev& D) {
 __global__ void __launch_bounds__(256) chd_k_kcopy(ChdDev D) {
   const int b = blockIdx.y;
   if (!D.ipm[b].kw_req) return;
-  if (blockIdx.x == 0) {   // right-hand side accumulators of chd_k_asm
-    const size_t go = (size_t)b * (D.Na_max + D.nb_max);
-    for (int i = threadIdx.x; i < D.Na_max + D.nb_max; i += blockDim.x) D.rhs0[go + i] = 0.0, D.rhs1[go + i] = 0.0;
-  }
+  if (blockIdx.x == 0) chd_rhs_clear(D, b);
   if (D.stages[D.ipm[b].stage].opt_dur && D.ipm[b].phase == CHD_PH_RUN) {
     // stage 3: the cost Hessian moves with the durations; chd_k_hess_dur rebuilds it into a cleared Kwork after the line search
     chd_hess_clear(D, b, D.Kwork + (size_t)b * D.kstride, blockIdx.x, gridDim.x);
@@ -1164,7 +1136,15 @@ __global__ void __launch_bounds__(256) chd_k_kcopy(ChdDev D) {
   }
   const size_t cnt2 = D.kstride / 2, per = (cnt2 + gridDim.x - 1) / gridDim.x;
   const size_t lo = (size_t)blockIdx.x * per, hi = lo + per < cnt2 ? lo + per : cnt2;
-  chd_kwork_copy(D, b, lo + threadIdx.x, hi, blockDim.x);
+  const double2* src = reinterpret_cast<const double2*>(D.Kbase + (size_t)b * D.kstride);
+  double2* dst = reinterpret_cast<double2*>(D.Kwork + (size_t)b * D.kstride);
+  const size_t nt = blockDim.x;
+  size_t i = lo + threadIdx.x;
+  for (; i + 3 * nt < hi; i += 4 * nt) {   // four independent 16-byte loads in flight per thread
+    const double2 v0 = src[i], v1 = src[i + nt], v2 = src[i + 2 * nt], v3 = src[i + 3 * nt];
+    dst[i] = v0, dst[i + nt] = v1, dst[i + 2 * nt] = v2, dst[i + 3 * nt] = v3;
+  }
+  for (; i < hi; i += nt) dst[i] = src[i];
 }
 
 // distance-row curvature terms of the next iteration (needs the iterate the line search just accepted); side stream,
@@ -1181,18 +1161,23 @@ __global__ void __launch_bounds__(256) chd_k_curv(ChdDev D) {
   chd_curv_rows(D, b, K, D.stages[I.stage], blockIdx.x * 8 + warp, gridDim.x * 8, lane, s_ws + warp * 192);
 }
 
-// matrix part of the assembly for the sequences that continue in their stage (Kwork already refreshed by chd_k_kcopy
-// and chd_k_curv): grid (G, B), launched right before chd_k_kkt.  The reductions into L2 are the cost, so G CTAs per
-// sequence on the SMs the one-CTA-per-sequence kernels leave idle take 1/G of the time.
+// Jacobian-dependent matrix entries and right-hand side of every running sequence, on a Kwork that holds the cost
+// Hessian and the distance-row curvature (chd_k_hess_zero / chd_k_hess_base on the first iteration of a stage,
+// chd_k_kcopy / chd_k_hess_dur / chd_k_curv afterwards) and zeroed rhs0 / rhs1: grid (G, B), launched right before
+// chd_k_kkt.  The reductions into L2 are the cost, so G CTAs per sequence on the SMs the one-CTA-per-sequence kernels
+// leave idle take 1/G of the time.
 __global__ void __launch_bounds__(256) chd_k_asm(ChdDev D) {
   const int b = blockIdx.y;
   const ChdIpm& I = D.ipm[b];
-  if (!I.kw_req || I.phase != CHD_PH_RUN) return;
+  if (I.phase != CHD_PH_RUN) return;
   ChdKT K;
   chd_kt_init(D, D.seq + b, D.Kwork + (size_t)b * D.kstride, K);
   K.ovf = &D.ipm[b].band_ovf;
+  // the band chd_k_kkt factors in a fixed-duration stage: a Jacobian coupling outside it (stage 4 on the durations a
+  // failed stage 3 left behind) fails the stage instead of being left out of the factorisation
+  if (!D.stages[I.stage].opt_dur) K.q = D.Qfix - 1;
   const size_t go = (size_t)b * (D.Na_max + D.nb_max);
-  chd_assemble(D, b, K, I.delta_w, I.mu, I.sf, nullptr, true, blockIdx.x * blockDim.x + threadIdx.x, gridDim.x * blockDim.x, D.rhs0 + go, D.rhs1 + go);
+  chd_assemble(D, b, K, I.delta_w, I.sf, blockIdx.x * blockDim.x + threadIdx.x, gridDim.x * blockDim.x, D.rhs0 + go, D.rhs1 + go);
 }
 
 // fp64 throughput probe for the roofline denominators: mode 0 = DFMA chains, mode 1 = DMMA (mma.sync m8n8k4 f64)
