@@ -322,68 +322,40 @@ static int batch_create_impl(const chd_phys_problem* problems, int32_t batch, co
 #define AL(field, cnt) if ((rc = dev_alloc(b, (cnt), &D.field))) return rc;
   AL(x, nm) AL(xt, nm) AL(jty, nm) AL(unobs, nm) AL(dx, nm) AL(grad, nm) AL(g, mm) AL(gt, mm) AL(Jv, B * hb.slots_max) AL(rflag, mm)
   AL(sc, mm) AL(dL, mm) AL(dU, mm) AL(s, mm) AL(y, mm) AL(zL, mm) AL(zU, mm) AL(ds, mm) AL(dy, mm) AL(dzL, mm) AL(dzU, mm)
-  D.nbc_max = (hb.Na_max + 7) / 8;
-  D.Q = (hb.w_max + 7) / 8 + 1;
-  D.Qfix = (hb.w_fix_max + 7) / 8 + 1;   // band tiles the fixed-duration stages work with (storage strides follow Q)
-  D.nbt = (hb.nb_max + 1 + 7) / 8;
-  D.win_tiles = std::max(D.Q * (D.Q + 1) / 2, 2 * D.Q);
-  D.kstride = (size_t)D.nbc_max * D.Q * 64 + (size_t)D.nbc_max * D.nbt * 64 + (size_t)64 * D.nbt * D.nbt;
   int dev = 0, sms = 0, smem_max = 0;
   CHD_CUDA(cudaGetDevice(&dev));
   CHD_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  CHD_CUDA(cudaDeviceGetAttribute(&smem_max, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+  cudaFuncAttributes fa_kkt, fa_gwin;
+  CHD_CUDA(cudaFuncGetAttributes(&fa_kkt, chd_k_kkt));
+  CHD_CUDA(cudaFuncGetAttributes(&fa_gwin, chd_k_kkt_gwin));
+  const ChdKktPlan P = chd_kkt_plan(hb.Na_max, hb.nb_max, hb.w_max, hb.w_fix_max, hb.n_max, fa_kkt.sharedSizeBytes,
+                                    fa_gwin.sharedSizeBytes, (size_t)smem_max);
+  D.win_smem = P.win_smem, D.nbc_max = P.nbc_max, D.Q = P.Q, D.Qfix = P.Qfix, D.nbt = P.nbt, D.win_tiles = P.win_tiles;
+  D.pan_doubles = P.pan_doubles, D.kstride = P.kstride, D.scratch_stride = P.scratch_stride;
+  b->smem_kkt = P.smem_bytes;
   // CTAs per sequence: enough for four per SM over the whole batch, and at least one per 128 KB of band storage
-  b->kcopy_blocks = (int)std::min<size_t>(512, std::max<size_t>(std::max<size_t>(1, 4 * (size_t)sms / B), D.kstride * sizeof(double) / 131072));
-  AL(cost, B * 2) AL(Kwork, B * D.kstride) AL(Kbase, B * D.kstride) AL(sol, B * (size_t)(hb.Na_max + hb.nb_max)) AL(ipm, B)
+  b->kcopy_blocks = (int)std::min<size_t>(512, std::max<size_t>(std::max<size_t>(1, 4 * (size_t)sms / B), P.kstride * sizeof(double) / 131072));
+  AL(cost, B * 2) AL(Kwork, B * P.kstride) AL(Kbase, B * P.kstride) AL(sol, B * (size_t)(hb.Na_max + hb.nb_max)) AL(ipm, B)
   AL(rhs0, B * (size_t)(hb.Na_max + hb.nb_max)) AL(rhs1, B * (size_t)(hb.Na_max + hb.nb_max))
+  if (P.scratch_stride) AL(scratch, B * P.scratch_stride)
 #undef AL
   if ((rc = dev_upload(b, hb.x0, (const double**)&b->d_x0))) return rc;
   CHD_CUDA(cudaMemcpyAsync(D.x, b->d_x0, nm * sizeof(double), cudaMemcpyDeviceToDevice, b->stream));
   // shared-memory budgets
-  const size_t nbp8 = 8 * (size_t)D.nbt;
   b->smem_eval = (2 * (size_t)hb.n_max + CHD_THREADS) * sizeof(double);
   b->smem_ls = ((size_t)hb.n_max + CHD_THREADS) * sizeof(double);
-  D.pan_doubles = std::max(2 * (D.Q + D.nbt) * 64, 8 * D.nbc_max);
-  cudaFuncAttributes fa;
-  CHD_CUDA(cudaFuncGetAttributes(&fa, chd_k_kkt));
-  const size_t kkt_static = fa.sharedSizeBytes;
-  const size_t n_even = (size_t)((hb.n_max + 1) & ~1), xs_len = 8 * (size_t)D.nbc_max + nbp8;
-  // the per-unknown vectors alias the tail of the window region (chd_kkt_body)
-  const size_t kkt_fixed = (CHD_KKT_THREADS + nbp8 * nbp8 + (size_t)D.pan_doubles + 16) * sizeof(double);
-  const size_t kkt_win = ((size_t)D.win_tiles * 64 + (size_t)D.Q * D.nbt * 64) * sizeof(double);
-  CHD_CUDA(cudaDeviceGetAttribute(&smem_max, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
-  // (+ 3072: chd_k_kkt's former distance-row curvature scratch; it guards nothing now, but dropping it would move
-  // borderline batches from chd_k_kkt_gwin onto chd_k_kkt)
-  const bool vectors_fit = (size_t)D.win_tiles * 64 + (size_t)D.Q * D.nbt * 64 >= n_even + xs_len + 2 * (size_t)D.Q * 64 + 3072;
-  if (vectors_fit && kkt_fixed + kkt_win + kkt_static + 256 <= (size_t)smem_max) {
-    D.win_smem = 1;
-    b->smem_kkt = kkt_fixed + kkt_win;
-    // chd_k_kkt compacts at most 64 panel groups (band + border tiles) for its trailing updates and has no other update
-    // loop for the shared-memory window; any window that fits is well below that (Q + nbt <= 30 at 227 KB)
-    if (D.Q - 1 + D.nbt > 64) {
-      fprintf(stderr, "libchd: band + border too wide for the compacted update loop (Q=%d nbt=%d)\n", D.Q, D.nbt);
-      return -5;
-    }
-  } else {
-    // long horizons / wide bands: vectors and window in a global scratch area (chd_k_kkt_gwin)
-    D.win_smem = 0;
-    D.pan_doubles = 2 * (D.Q + D.nbt) * 64;
-    b->smem_kkt = chd_kkt_gwin_smem(D.Q, D.nbt);
-    D.scratch_stride = n_even + xs_len + 8 * (size_t)D.nbc_max + (size_t)D.win_tiles * 64 + (size_t)D.Q * D.nbt * 64;
-    if ((rc = dev_alloc(b, B * D.scratch_stride, &D.scratch))) return rc;
-    if (D.Q - 1 + D.nbt > CHD_KKT_GROUPS_MAX) {
-      fprintf(stderr, "libchd: band + border too wide for the pair tables (Q=%d nbt=%d)\n", D.Q, D.nbt);
-      return -5;
-    }
+  if (P.status == CHD_KKT_TOO_WIDE_COMPACT || P.status == CHD_KKT_TOO_WIDE_PAIRS) {
+    fprintf(stderr, "libchd: band + border too wide for the %s (Q=%d nbt=%d)\n",
+            P.status == CHD_KKT_TOO_WIDE_COMPACT ? "compacted update loop" : "pair tables", P.Q, P.nbt);
+    return -5;
   }
-  // (the global-window kernel has more static shared memory than chd_k_kkt: its pair table holds up to 96 panel groups)
-  CHD_CUDA(cudaFuncGetAttributes(&fa, chd_k_kkt_gwin));
-  const size_t kkt_static_used = D.win_smem ? kkt_static : fa.sharedSizeBytes;
-  if (b->smem_eval + 1024 > (size_t)smem_max || b->smem_kkt + kkt_static_used + 256 > (size_t)smem_max) {
+  if (P.status == CHD_KKT_TOO_LARGE || b->smem_eval + 1024 > (size_t)smem_max) {
     fprintf(stderr, "libchd: problem too large for the shared-memory staged kernels (n_max=%d)\n", hb.n_max);
     return -5;
   }
   CHD_CUDA(cudaFuncSetAttribute(chd_k_eval, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)b->smem_eval));
-  CHD_CUDA(cudaFuncSetAttribute(D.win_smem ? chd_k_kkt : chd_k_kkt_gwin, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)b->smem_kkt));
+  CHD_CUDA(cudaFuncSetAttribute(P.win_smem ? chd_k_kkt : chd_k_kkt_gwin, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)b->smem_kkt));
   CHD_CUDA(cudaFuncSetAttribute(chd_k_linesearch, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)b->smem_ls));
   const size_t stride = 6 + 7 * (size_t)hb.n_ee_max;
   CHD_CUDA(cudaMallocAsync((void**)&b->d_samples, B * hb.fo_max * stride * sizeof(double), b->stream));

@@ -1,20 +1,11 @@
 // Device-side views of a phys-optim batch (product code).
 #pragma once
 #include "chd_core.h"
+#include "chd_kkt_plan.h"
 #include "chd_layout.h"
 
 #define CHD_FILT_MAX 24
 #define CHD_THREADS 512
-#define CHD_KKT_THREADS 512
-#define CHD_KKT_GROUPS_MAX 96          /* panel groups (band tiles below the diagonal + border tiles) chd_k_kkt_gwin's pair table holds */
-#define CHD_SMEM_OPTIN 232448          /* shared memory per block an sm_90 kernel may opt in to (227 KB) */
-#define CHD_KKT_GWIN_STATIC_MAX 16384  /* bound on chd_k_kkt_gwin's static shared memory (ptxas: 12144 B) */
-// dynamic shared memory of chd_k_kkt_gwin for Q band tiles per block column and nbt border tiles: reduction buffer,
-// corner (incl. the right-hand-side row), panel buffers, diagonal inverses
-inline size_t chd_kkt_gwin_smem(int Q, int nbt) {
-  const size_t nbp8 = 8 * (size_t)nbt;
-  return (CHD_KKT_THREADS + nbp8 * nbp8 + 2 * (size_t)(Q + nbt) * 64 + 16) * sizeof(double);
-}
 #define CHD_NL_GUARD 1.0    /* stage 3 line search: trial refused while theta_t - (1-alpha) theta > CHD_NL_GUARD * max(alpha theta, CHD_NL_FLOOR max(1, theta_ref)) */
 #define CHD_NL_FLOOR 1e-4
 #define CHD_UNOBS_EPS 1e-14 /* "sees": diagonal of the scaled cost Hessian above this (a sample sitting exactly on a node gives weights of 1e-17) */
@@ -69,6 +60,7 @@ struct ChdDev {
   int B, S, Pmax, n_max, m_max, slots_max, sets_max, tab_max, F_max, Kd_max, Kr_max, Na_max, nb_max, w_max, par_stride,
       n_ee_max, fo_max, Ph_max, win_smem, nbc_max, Q, Qfix, nbt, win_tiles, pan_doubles;
   size_t kstride;                             // doubles per sequence of a tile-format KKT buffer (band | bord | corn)
+                                              // (win_smem .. pan_doubles, kstride, scratch_stride: ChdKktPlan)
   // ---- static layout ----
   const ChdSeq* seq;
   // poly_T / poly_tend / phase_tend / ent_col are rewritten on the device once stage 3 moves the durations

@@ -96,12 +96,9 @@ __device__ void chd_hess_build(const ChdDev& D, int b, const ChdStageDev& sg, do
     }
   }
   if (part == 0)
-    for (int i = K.Na + tid; i < K.Np; i += nt) K.band[((size_t)(i >> 3) * K.Q) * 64 + (i & 7) * 9] = 1.0;  // identity padding of the band
+    for (int i = K.Na + tid; i < K.Np; i += nt) *chd_kdiag(K, i, true) = 1.0;  // identity padding of the band
   if (part == 0 && !sg.opt_dur && h->dur_band)   // banded switch times outside stage 3: decoupled unknowns, unit diagonal
-    for (int i = tid; i < h->n_dur; i += nt) {
-      const int k = vk[h->dur_xoff[0] + i];   // the duration variables of all feet are contiguous in x
-      K.band[((size_t)(k >> 3) * K.Q) * 64 + (k & 7) * 9] = 1.0;
-    }
+    for (int i = tid; i < h->n_dur; i += nt) *chd_kdiag(K, vk[h->dur_xoff[0] + i], true) = 1.0;   // the duration variables of all feet are contiguous in x
   if (part == 0 && sg.opt_dur && sg.w_dur != 0.0) {   // duration_cost.cpp: w I in the durations = w D^T D in the switch times
     for (int ee = 0; ee < n_ee; ++ee)
       for (int k = tid; k < h->n_phases[ee] - 1; k += nt) {
@@ -145,7 +142,7 @@ __global__ void __launch_bounds__(CHD_THREADS) chd_k_hess_dur(ChdDev D) {
 __global__ void __launch_bounds__(128) chd_k_hess_fin(ChdDev D, int mode) {
   const int b = blockIdx.x;
   ChdIpm& I = D.ipm[b];
-  const double* base;
+  double* base;
   if (mode == 0) {
     if (I.phase != CHD_PH_BEGIN) return;
     base = D.Kbase + (size_t)b * D.kstride;
@@ -155,17 +152,13 @@ __global__ void __launch_bounds__(128) chd_k_hess_fin(ChdDev D, int mode) {
   }
   const ChdSeq* h = D.seq + b;
   const int* vk = D.var_kkt + (size_t)b * D.n_max;
-  const double* corn = base + (size_t)D.nbc_max * D.Q * 64 + (size_t)D.nbc_max * D.nbt * 64;
+  ChdKT K;
+  chd_kt_init(D, h, base, K);
   unsigned char* un = D.unobs + (size_t)b * D.n_max;
-  const int mot_lo = h->sp_xoff[2], mot_hi = h->sp_xoff[2 + h->n_ee], Na = h->Na;
+  const int mot_lo = h->sp_xoff[2], mot_hi = h->sp_xoff[2 + h->n_ee];
   for (int i = mot_lo + threadIdx.x; i < mot_hi; i += blockDim.x) {
     const int k = vk[i];
-    unsigned char f = 0;
-    if (k >= 0) {
-      const double hd = k < Na ? base[((size_t)(k >> 3) * D.Q) * 64 + (k & 7) * 9] : corn[(size_t)(k - Na) * 8 * D.nbt + (k - Na)];
-      f = hd <= CHD_UNOBS_EPS;
-    }
-    un[i] = f;
+    un[i] = k >= 0 && *chd_kdiag(K, k) <= CHD_UNOBS_EPS;
   }
   __syncthreads();
   if (mode == 0 && threadIdx.x == 0) I.phase = CHD_PH_RUN;

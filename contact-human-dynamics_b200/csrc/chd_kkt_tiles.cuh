@@ -53,6 +53,12 @@ __device__ __forceinline__ void chd_kadd(const ChdKT& K, int i, int j, double v)
     atomicAdd(K.corn + (size_t)(i - K.Na) * K.nbp8 + (j - K.Na), v);
   }
 }
+// diagonal element (k, k), unknown index as in chd_kadd (k >= Na: border); band = true addresses the band for any
+// k < Np, the identity padding rows Na .. Np-1 included
+__device__ __forceinline__ double* chd_kdiag(const ChdKT& K, int k, bool band = false) {
+  if (band || k < K.Na) return K.band + ((size_t)(k >> 3) * K.Q) * 64 + (k & 7) * 9;
+  return K.corn + (size_t)(k - K.Na) * (K.nbp8 + 1);
+}
 
 // D(8x8) = C - X * Y^T for row-major 8x8 tiles X, Y (fp64 tensor core, two k-steps of m8n8k4).
 // Fragment layout (PTX ISA, mma.m8n8k4 f64): A[row = lane>>2][k = lane&3], B[k = lane&3][col = lane>>2],

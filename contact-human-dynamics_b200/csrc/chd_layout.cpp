@@ -94,8 +94,7 @@ std::vector<double> discretize(double T, double dt) {
 // wide run in: its pair table (panel groups) and its shared memory.  Checked for the whole batch, whose strides come
 // from the widest band and the largest border of possibly different sequences.
 bool kkt_fits(int w_max, int nb_max) {
-  const int Q = (w_max + 7) / 8 + 1, nbt = (nb_max + 1 + 7) / 8;
-  return Q - 1 + nbt <= CHD_KKT_GROUPS_MAX && chd_kkt_gwin_smem(Q, nbt) + CHD_KKT_GWIN_STATIC_MAX <= CHD_SMEM_OPTIN;
+  return chd_kkt_gwin_status(w_max, nb_max, CHD_KKT_GWIN_STATIC_MAX, CHD_SMEM_OPTIN) == CHD_KKT_FITS;
 }
 
 // Returns 0, a negative code for malformed input, or 1 when banded switch times would make the band too wide for the

@@ -1,7 +1,7 @@
 // TEST INFRASTRUCTURE ONLY -- host build of the product's work-item evaluators (csrc/chd_eval.cuh) for the CPU test
 // suite: the same source the CUDA kernels include, compiled with a one-thread shim of the CUDA built-ins, so the
 // stage-3 evaluation logic (run-time polynomial location, switch-time columns, table rebuilds) can be checked
-// against the oracle without a GPU.  Never loaded by the product.
+// against the oracle without a GPU, and of the KKT plan (csrc/chd_kkt_plan.h).  Never loaded by the product.
 #include <cmath>
 #include <cstring>
 #include <vector>
@@ -61,4 +61,11 @@ extern "C" int chd_emu_eval(const chd_phys_problem* prob, const chd_phys_weights
   if (Jv) std::memcpy(Jv, jv.data(), sizeof(double) * h.nslots);
   if (ent_col) std::memcpy(ent_col, hb.ent_col.data(), sizeof(int) * h.nslots);
   return 0;
+}
+
+// The KKT plan batch creation computes for these batch strides, kernel static shared-memory sizes and opt-in limit.
+extern "C" int chd_emu_kkt_plan(int Na_max, int nb_max, int w_max, int w_fix_max, int n_max, long long kkt_static,
+                                long long gwin_static, long long smem_optin, ChdKktPlan* out) {
+  *out = chd_kkt_plan(Na_max, nb_max, w_max, w_fix_max, n_max, kkt_static, gwin_static, smem_optin);
+  return (int)sizeof(ChdKktPlan);
 }
