@@ -241,8 +241,8 @@ int chd_measure_fp64_peak(double* dfma_gflops, double* dmma_gflops) {
       CHD_CUDA(cudaEventElapsedTime(&ms, e0, e1));
       if (rep > 0 && ms < best) best = ms;
     }
-    // mode 0: 8 independent FMA chains per thread; mode 1: 4 independent m8n8k4 accumulators per warp (512 flop each)
-    const double flop = mode == 0 ? (double)blocks * threads * iters * 8 * 2 : (double)blocks * (threads / 32) * iters * 4 * 512;
+    // mode 0: 8 independent FMA chains per thread; mode 1: 4 independent m16n8k8 accumulators per warp (2048 flop each)
+    const double flop = mode == 0 ? (double)blocks * threads * iters * 8 * 2 : (double)blocks * (threads / 32) * iters * 4 * 2048;
     double* out = mode == 0 ? dfma_gflops : dmma_gflops;
     if (out) *out = flop / (best * 1e-3) / 1e9;
   }
@@ -528,7 +528,7 @@ int chd_phys_solve_stage(chd_phys_batch* b, int32_t stage, int32_t max_iter, int
       double* s = stats + 8 * i;
       s[0] = I.f, s[1] = I.E0, s[2] = I.viol_u, s[3] = I.dual_u, s[4] = I.compl_u, s[5] = I.mu, s[6] = I.delta_w, s[7] = I.ls_fail;
     }
-    if (i == 0 && getenv("CHD_PROF")) fprintf(stderr, "chd prof (Mcycles) seq0 stage %d: err %.2f asm %.2f factor %.2f border %.2f back %.2f rec %.2f\n", stage, I.prof[0]/1e6, I.prof[1]/1e6, I.prof[2]/1e6, I.prof[3]/1e6, I.prof[4]/1e6, I.prof[5]/1e6);
+    if (i == 0 && getenv("CHD_PROF")) fprintf(stderr, "chd prof (Mcycles) seq0 stage %d: err %.2f asm %.2f factor %.2f border %.2f back %.2f rec %.2f | factor (c): diag %.2f upd %.2f\n", stage, I.prof[0]/1e6, I.prof[1]/1e6, I.prof[2]/1e6, I.prof[3]/1e6, I.prof[4]/1e6, I.prof[5]/1e6, I.prof[6]/1e6, I.prof[7]/1e6);
   }
   return 0;
 }

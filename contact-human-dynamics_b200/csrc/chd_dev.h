@@ -45,7 +45,7 @@ struct ChdIpm {
   double theta_ref;                               // theta at the first iteration of the stage (nonlinearity guard of stage 3)
   double filt[2 * CHD_FILT_MAX];
   double st_stat[6][4];                           // per stage at its end: f, E0 (scaled NLP error), unscaled constraint violation, unscaled dual infeasibility
-  double prof[8];   // clock64 cycles per phase of chd_k_kkt (0 errors, 1 assembly, 2 factor, 3 border, 4 back-subst, 5 step recovery)
+  double prof[8];   // clock64 cycles per phase of chd_k_kkt (0 errors, 1 assembly, 2 factor, 3 border, 4 back-subst, 5 step recovery; inside 2: 6 warp 0's next diagonal tile, 7 the trailing updates)
 };
 
 struct ChdStageDev {

@@ -598,16 +598,55 @@ __device__ __forceinline__ void chd_kkt_assemble(const ChdDev& D, const ChdKktCt
   for (int i = tid; i < nbl; i += nt) K.corn[(size_t)NBR * nbp8 + i] = r0[D.Na_max + i] + mu * r1[D.Na_max + i];
 }
 
-// Trailing updates C -= X Y^T of one block column by the warps 1 .. nwarp-1, for at most 64 panel groups (every
-// shared-memory window; global windows of narrower bands).  2 x 2 register blocking over the compacted list of the groups
-// with a non-zero X tile: one trip loads the operand fragments of two panel rows (X) and two panel columns (Y) once and
+// One 2 x 2 block of the trailing update C -= X Y^T: panel rows gi[0], gi[1] (X) against panel columns gj[0], gj[1] (Y)
+// of the panel buffers, vi / vj = which of them take part.  The operand fragments of the block are loaded once and every
+// target tile's C is loaded before the first product; one m16n8k8 per panel column (the two row tiles stacked).
+// Targets that are not updated here (the upper tile of a diagonal block, a row or column that takes no part, warp 0's
+// next diagonal tile) are computed from a zero C and not stored.
+template <class BandTile, class BordTile>
+__device__ __forceinline__ void chd_kkt_update_block(const ChdKktCtx& c, const int* gi, const int* gj, const bool* vi, const bool* vj, bool diag,
+                                                     int GB, const BandTile& band_tile, const BordTile& bord_tile) {
+  const int lane = c.lane;
+  const double2 z = make_double2(0.0, 0.0);
+  double2 xf[2], yf[2];
+#pragma unroll
+  for (int a = 0; a < 2; ++a) {
+    xf[a] = vi[a] ? *reinterpret_cast<const double2*>(c.xpan + gi[a] * 64 + 2 * lane) : z;
+    yf[a] = vj[a] ? *reinterpret_cast<const double2*>(c.ypan + gj[a] * 64 + 2 * lane) : z;
+  }
+  double* Cp[4];
+  double2 cv[4];
+#pragma unroll
+  for (int t = 0; t < 4; ++t) {
+    const int a = t & 1, cl = t >> 1;          // tile (row a, column cl) of the block
+    bool ok = vi[a] && vj[cl] && !(diag && a == 0 && cl == 1);
+    ok = ok && !(gi[a] == 0 && gj[cl] == 0);   // the next diagonal tile is updated by warp 0
+    // this lane's (row g, columns 2t, 2t+1) of the target: band tile, border tile or corner block (row stride nbp8)
+    Cp[t] = nullptr;
+    if (ok) {
+      if (gi[a] < GB) Cp[t] = band_tile(gi[a], gj[cl]) + (lane >> 2) * 8 + 2 * (lane & 3);
+      else if (gj[cl] < GB) Cp[t] = bord_tile(gi[a] - GB, gj[cl]) + (lane >> 2) * 8 + 2 * (lane & 3);
+      else Cp[t] = c.cc + (size_t)((gi[a] - GB) * 8 + (lane >> 2)) * c.nbp8 + (gj[cl] - GB) * 8 + 2 * (lane & 3);
+    }
+    cv[t] = ok ? *reinterpret_cast<const double2*>(Cp[t]) : z;
+  }
+  const double2 xt = make_double2(-xf[0].x, -xf[0].y), xb = make_double2(-xf[1].x, -xf[1].y);
+#pragma unroll
+  for (int cl = 0; cl < 2; ++cl) chd_mma_16x8x8(cv[2 * cl], cv[2 * cl + 1], xt, xb, yf[cl]);
+#pragma unroll
+  for (int t = 0; t < 4; ++t)
+    if (Cp[t]) *reinterpret_cast<double2*>(Cp[t]) = cv[t];
+}
+
+// Trailing updates of one block column by the warps 1 .. nwarp-1, for at most 64 panel groups (every shared-memory
+// window; global windows of narrower bands).  2 x 2 register blocking over the compacted list of the groups with a
+// non-zero X tile: one trip loads the operand fragments of two panel rows (X) and two panel columns (Y) once and
 // updates up to four target tiles with them -- the loop is shared-memory bandwidth bound, this cuts the bytes per tile
 // update from 2 KB to 1.5 KB and the index work 4x.  cmp: this warp's rank -> group table.
 template <class BandTile, class BordTile>
 __device__ __forceinline__ void chd_kkt_update_compact(const ChdKktCtx& c, const unsigned short* s_pairs, unsigned char* cmp, const int* gnz,
                                                        int GB, int Gm, int tq, const BandTile& band_tile, const BordTile& bord_tile) {
-  const int lane = c.lane, warp = c.warp, nbp8 = c.nbp8;
-  const double *xpan = c.xpan, *ypan = c.ypan;
+  const int lane = c.lane, warp = c.warp;
   // compact list of the groups with a non-zero X tile (every warp builds it redundantly: no extra barrier).
   // the pair table enumerates (i >= j) row by row, so its first na(na+1)/2 entries pair the first na entries.
   int na;
@@ -624,111 +663,31 @@ __device__ __forceinline__ void chd_kkt_update_compact(const ChdKktCtx& c, const
     if (act1) cmp[n0 + __popc(m1 & below)] = (unsigned char)g1;
     __syncwarp();
   }
-  auto corner = [&](const double* X, const double* Y, int bi, int bj) {   // corner block: same tensor-core update, row stride nbp8
-    double* Cc = c.cc + (size_t)(bi * 8 + (lane >> 2)) * nbp8 + bj * 8 + 2 * (lane & 3);
-    double c0 = Cc[0], c1 = Cc[1];
-    chd_tile_mma(c0, c1, X, Y, lane);
-    Cc[0] = c0, Cc[1] = c1;
-  };
-  const int step = c.nwarp - 1, r8 = (lane >> 2) * 8 + 2 * (lane & 3);
+  const int step = c.nwarp - 1;
   const int nb2 = (na + 1) >> 1, nblk = nb2 * (nb2 + 1) / 2;
   for (int p = warp - 1; p < nblk; p += step) {
     const int bi = s_pairs[p] >> 8, bj = s_pairs[p] & 255;
     const int i1 = 2 * bi + 1, j1 = 2 * bj + 1;
-    const bool vi1 = i1 < na, vj1 = j1 < na;
-    int gi[2], gj[2];
-    gi[0] = cmp[2 * bi], gi[1] = cmp[i1 & 63];
-    gj[0] = cmp[2 * bj], gj[1] = cmp[j1 & 63];
-    double2 xf[2], yf[2];
-    xf[0] = *reinterpret_cast<const double2*>(xpan + gi[0] * 64 + 2 * lane);
-    yf[0] = *reinterpret_cast<const double2*>(ypan + gj[0] * 64 + 2 * lane);
-    xf[1] = vi1 ? *reinterpret_cast<const double2*>(xpan + gi[1] * 64 + 2 * lane) : make_double2(0.0, 0.0);
-    yf[1] = vj1 ? *reinterpret_cast<const double2*>(ypan + gj[1] * 64 + 2 * lane) : make_double2(0.0, 0.0);
-    double* Cp[4];
-    double2 cv[4];
-#pragma unroll
-    for (int t = 0; t < 4; ++t) {
-      const int a = t & 1, cl = t >> 1;          // tile (row a, column cl) of the block
-      bool ok = (a == 0 || vi1) && (cl == 0 || vj1) && !(bi == bj && a == 0 && cl == 1);
-      const int g_i = gi[a], g_j = gj[cl];
-      ok = ok && !(g_i == 0 && g_j == 0);       // the next diagonal tile is updated by warp 0
-      Cp[t] = nullptr;
-      if (ok) {
-        if (g_i < GB) Cp[t] = band_tile(g_i, g_j);
-        else if (g_j < GB) Cp[t] = bord_tile(g_i - GB, g_j);
-        else corner(xpan + g_i * 64, ypan + g_j * 64, g_i - GB, g_j - GB);
-      }
-      if (Cp[t]) cv[t] = *reinterpret_cast<const double2*>(Cp[t] + r8);
-    }
-#pragma unroll
-    for (int t = 0; t < 4; ++t)
-      if (Cp[t]) {
-        const double2 xa = xf[t & 1], yb = yf[t >> 1];
-        asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};"
-                     : "+d"(cv[t].x), "+d"(cv[t].y)
-                     : "d"(-xa.x), "d"(yb.x));
-      }
-#pragma unroll
-    for (int t = 0; t < 4; ++t)
-      if (Cp[t]) {
-        const double2 xa = xf[t & 1], yb = yf[t >> 1];
-        asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};"
-                     : "+d"(cv[t].x), "+d"(cv[t].y)
-                     : "d"(-xa.y), "d"(yb.y));
-        *reinterpret_cast<double2*>(Cp[t] + r8) = cv[t];
-      }
+    const int gi[2] = {cmp[2 * bi], cmp[i1 & 63]}, gj[2] = {cmp[2 * bj], cmp[j1 & 63]};
+    const bool vi[2] = {true, i1 < na}, vj[2] = {true, j1 < na};
+    chd_kkt_update_block(c, gi, gj, vi, vj, bi == bj, GB, band_tile, bord_tile);
   }
 }
 
 // Trailing updates of one block column by the warps 1 .. nwarp-1 with more than 64 panel groups (window in global (L2)
-// memory): each warp collects up to four target tiles from the full pair table, issues all their loads, and only then
-// runs the tensor-core updates and the stores.  (With the window in shared memory the simple loop was faster on the
-// benchmark batch.)
+// memory): the same 2 x 2 blocks over the groups themselves (the per-warp compacted list holds 64 groups); blocks
+// without a live target are skipped.
 template <class BandTile, class BordTile>
-__device__ __forceinline__ void chd_kkt_update_wide(const ChdKktCtx& c, const unsigned short* s_pairs, const int* gnz, int GB, int npairs,
+__device__ __forceinline__ void chd_kkt_update_wide(const ChdKktCtx& c, const unsigned short* s_pairs, const int* gnz, int GB, int Gm,
                                                     int tq, const BandTile& band_tile, const BordTile& bord_tile) {
-  const int lane = c.lane, nwarp = c.nwarp, nbp8 = c.nbp8;
-  const double *xpan = c.xpan, *ypan = c.ypan;
-  double* cc = c.cc;
-  const int r8 = (lane >> 2) * 8 + 2 * (lane & 3);
-  int p = c.warp - 1;
-  while (p < npairs) {
-    // target tiles and their operands; one array of structs, not three pointer arrays: an array of the compact loop's
-    // type double*[4] gets merged with its Cp when both loops are inlined, which puts that one in local memory as well
-    struct { double* C; const double *X, *Y; } tl[4];
-    int nq = 0;
-    while (nq < 4 && p < npairs) {
-      const int gi = s_pairs[p] >> 8, gj = s_pairs[p] & 255;
-      p += nwarp - 1;
-      if ((gi < GB && gi >= tq) || (gj < GB && gj >= tq) || !gnz[gi] || !gnz[gj]) continue;
-      if (gi == 0 && gj == 0) continue;
-      const double* X = xpan + gi * 64;
-      const double* Y = ypan + gj * 64;
-      if (gi < GB) {
-        tl[nq].C = band_tile(gi, gj), tl[nq].X = X, tl[nq].Y = Y, ++nq;
-      } else if (gj < GB) {
-        tl[nq].C = bord_tile(gi - GB, gj), tl[nq].X = X, tl[nq].Y = Y, ++nq;
-      } else {
-        const int bi = gi - GB, bj = gj - GB;
-        for (int e = lane; e < 64; e += 32) {
-          const int r = e >> 3, cq = e & 7;
-          double acc = 0.0;
-#pragma unroll
-          for (int kk = 0; kk < 8; ++kk) acc += X[r * 8 + kk] * Y[cq * 8 + kk];
-          cc[(bi * 8 + r) * nbp8 + bj * 8 + cq] -= acc;
-        }
-      }
-    }
-    double c0[4], c1[4];
-#pragma unroll
-    for (int i = 0; i < 4; ++i)
-      if (i < nq) c0[i] = tl[i].C[r8], c1[i] = tl[i].C[r8 + 1];
-#pragma unroll
-    for (int i = 0; i < 4; ++i)
-      if (i < nq) {
-        chd_tile_mma(c0[i], c1[i], tl[i].X, tl[i].Y, lane);
-        tl[i].C[r8] = c0[i], tl[i].C[r8 + 1] = c1[i];
-      }
+  auto live = [&](int g) { return g < Gm && (g >= GB || g < tq) && gnz[g]; };
+  const int nb2 = (Gm + 1) >> 1, nblk = nb2 * (nb2 + 1) / 2;
+  for (int p = c.warp - 1; p < nblk; p += c.nwarp - 1) {
+    const int bi = s_pairs[p] >> 8, bj = s_pairs[p] & 255;
+    const int gi[2] = {2 * bi, 2 * bi + 1}, gj[2] = {2 * bj, 2 * bj + 1};
+    const bool vi[2] = {live(gi[0]), live(gi[1])}, vj[2] = {live(gj[0]), live(gj[1])};
+    if (!(vi[0] || vi[1]) || !(vj[0] || vj[1])) continue;
+    chd_kkt_update_block(c, gi, gj, vi, vj, bi == bj, GB, band_tile, bord_tile);
   }
 }
 
@@ -754,17 +713,27 @@ __device__ __forceinline__ void chd_kkt_factor(const ChdKktCtx& c, int& s_fail) 
     }
   }
   __syncthreads();
-  // index tables: pair list (gi >= gj) over band groups 0..q-1 and border groups q..q+nbt-1 (built once),
-  // window slot of every band group of the current block column (double buffered, no integer division)
+  // index tables: pair list of the 2 x 2 blocks of the trailing update (built once; panel groups = band groups 0..q-1,
+  // border groups q..q+nbt-1), window slot of every band group of the current block column (double buffered, no
+  // integer division)
   __shared__ int s_rs[2][96];
   __shared__ int s_gnz[2][96];   // per panel group: any non-zero entry in the X tile (zero tiles skip their trailing updates)
   // pair table: at most 64 panel groups with the shared-memory window, 96 with the global one (its static shared memory
-  // is not needed for a window)
+  // is not needed for a window).  The 2 x 2 blocks use the first (Gm+1)/2 * ((Gm+1)/2 + 1) / 2 entries; the sizes are
+  // the static shared memory the KKT plan budgets for each kernel.
   constexpr int kPairs = WS ? 3000 : CHD_KKT_GROUPS_MAX * (CHD_KKT_GROUPS_MAX + 1) / 2;
   __shared__ unsigned short s_pairs[kPairs];
   __shared__ unsigned char s_cmp[CHD_KKT_THREADS / 32][64];   // per warp: rank -> id of the non-zero panel groups
   __shared__ __align__(16) double s_winv[2][64];   // inverse of the current / next diagonal tile factor, fragment order
-  const int GB = K.q, Gm = K.q + nbt_s, npairs = Gm * (Gm + 1) / 2;
+#ifdef CHD_PROFILE
+  // phase (c) of every block column: warp 0's update and LDL^T of the next diagonal tile (prof[6]), and the time until the
+  // last update warp is done (prof[7]) -- the larger of the two bounds the block column
+  __shared__ unsigned long long s_upd_end;
+  double prof_diag = 0.0, prof_upd = 0.0;
+  if (tid == 0) s_upd_end = 0;
+#endif
+  // block pairs (bi >= bj) of the 2 x 2 blocks of the trailing update, row by row
+  const int GB = K.q, Gm = K.q + nbt_s, nb2 = (Gm + 1) >> 1, npairs = nb2 * (nb2 + 1) / 2;
   for (int p = tid; p < npairs && p < kPairs; p += nt) {
     int gi = (int)((sqrt(8.0 * p + 1.0) - 1.0) * 0.5);
     while (gi * (gi + 1) / 2 > p) --gi;
@@ -794,33 +763,38 @@ __device__ __forceinline__ void chd_kkt_factor(const ChdKktCtx& c, int& s_fail) 
     double* Bk = WS ? bwin + (size_t)kslot * nbt * 64 : K.bord + (size_t)Kc * nbt * 64;
     const double* dv = dinv + 8 * cur;
     // (b) panel: Y = A L0^-T = A W^T (W = L0^-1 from the diagonal-tile factorisation) as one tensor-core product per
-    //     8x8 panel tile, X = Y D^-1; both go to the panel buffers in fragment order, X also to global (final L);
-    //     the diagonal tile goes to global as well
+    //     pair of 8x8 panel tiles (stacked rows of an m16n8k8), X = Y D^-1; both go to the panel buffers in fragment
+    //     order, X also to global (final L); the diagonal tile goes to global as well
     {
       const double* wv = s_winv[cur];
-      const int r = lane >> 2, k = lane & 3;
+      const int r = lane >> 2, k = lane & 3, ng = tq + nbt_s;
       const double2 wf = *reinterpret_cast<const double2*>(wv + 2 * lane);
       const double d0 = dv[2 * k], d1 = dv[2 * k + 1];
       const int f0 = r * 8 + chd_frag_col(2 * k), f1 = r * 8 + chd_frag_col(2 * k + 1);
-      for (int g = warp; g < tq + nbt_s; g += nwarp) {
-        const bool band_t = g < tq;
-        const int pg = band_t ? g : GB + (g - tq);                   // group id inside the panel buffers
-        const double* A = band_t ? (WS ? win + (size_t)tri(rs[g], kslot) * 64 : K.band + ((size_t)Kc * Qs + 1 + g) * 64) : Bk + (g - tq) * 64;
-        const double ax = A[r * 8 + k], ay = A[r * 8 + k + 4];
-        double c0 = 0.0, c1 = 0.0;
-        asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};"
-                     : "+d"(c0), "+d"(c1)
-                     : "d"(ax), "d"(wf.x));
-        asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};"
-                     : "+d"(c0), "+d"(c1)
-                     : "d"(ay), "d"(wf.y));
-        const double x0 = c0 * d0, x1 = c1 * d1;
-        ypan[pg * 64 + f0] = c0, ypan[pg * 64 + f1] = c1;
-        xpan[pg * 64 + f0] = x0, xpan[pg * 64 + f1] = x1;
-        double* G = band_t ? K.band + ((size_t)Kc * Qs + 1 + g) * 64 : K.bord + ((size_t)Kc * nbt + (g - tq)) * 64;
-        *reinterpret_cast<double2*>(G + r * 8 + 2 * k) = make_double2(x0, x1);
-        const bool nz = __any_sync(0xffffffffu, x0 != 0.0 || x1 != 0.0);
-        if (lane == 0 && nz) s_gnz[cur][pg] = 1;
+      for (int g0 = 2 * warp; g0 < ng; g0 += 2 * nwarp) {
+        double2 a[2], y[2];
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int g = g0 + h;
+          const double* A = g < tq ? (WS ? win + (size_t)tri(rs[g], kslot) * 64 : K.band + ((size_t)Kc * Qs + 1 + g) * 64) : Bk + (g - tq) * 64;
+          a[h] = g < ng ? make_double2(A[r * 8 + k], A[r * 8 + k + 4]) : make_double2(0.0, 0.0);
+          y[h] = make_double2(0.0, 0.0);
+        }
+        chd_mma_16x8x8(y[0], y[1], a[0], a[1], wf);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int g = g0 + h;
+          if (g >= ng) break;
+          const bool band_t = g < tq;
+          const int pg = band_t ? g : GB + (g - tq);                   // group id inside the panel buffers
+          const double x0 = y[h].x * d0, x1 = y[h].y * d1;
+          ypan[pg * 64 + f0] = y[h].x, ypan[pg * 64 + f1] = y[h].y;
+          xpan[pg * 64 + f0] = x0, xpan[pg * 64 + f1] = x1;
+          double* G = band_t ? K.band + ((size_t)Kc * Qs + 1 + g) * 64 : K.bord + ((size_t)Kc * nbt + (g - tq)) * 64;
+          *reinterpret_cast<double2*>(G + r * 8 + 2 * k) = make_double2(x0, x1);
+          const bool nz = __any_sync(0xffffffffu, x0 != 0.0 || x1 != 0.0);
+          if (lane == 0 && nz) s_gnz[cur][pg] = 1;
+        }
       }
     }
     if (WS)
@@ -829,6 +803,9 @@ __device__ __forceinline__ void chd_kkt_factor(const ChdKktCtx& c, int& s_fail) 
     // (c) stream in block row Kc + Q (its slots are dead now), trailing updates on the fp64 tensor core;
     //     warp 0 takes the pair that completes the next diagonal tile and factors it right away
     const int In = Kc + Q;
+#ifdef CHD_PROFILE
+    const long long tc0 = clock64();
+#endif
     if (WS && In < nbc) {
       // 16-byte cp.async chunks by the warps 1..15; warp 0 goes straight to the diagonal tile.  (A TMA producer warp, bulk
       // copies issued by a lane of an updating warp and dynamically dealt update blocks were slower: DESIGN.md section 9)
@@ -852,6 +829,9 @@ __device__ __forceinline__ void chd_kkt_factor(const ChdKktCtx& c, int& s_fail) 
         const bool ok = chd_tile_ldl(Tn, dinv + 8 * (cur ^ 1), s_winv[cur ^ 1], lane);
         if (!ok && lane == 0) s_fail = 1;
       }
+#ifdef CHD_PROFILE
+      if (lane == 0) prof_diag += (double)(clock64() - tc0);
+#endif
     } else {
       if (warp == 1) {
         for (int g = lane; g < GB; g += 32) {   // slot table of the next block column
@@ -862,13 +842,22 @@ __device__ __forceinline__ void chd_kkt_factor(const ChdKktCtx& c, int& s_fail) 
         for (int g = lane; g < Gm; g += 32) s_gnz[cur ^ 1][g] = 0;
       }
       // every shared-memory window has Gm <= 64 (batch creation checks Q - 1 + nbt <= 64)
-      if (!WS && Gm > 64) chd_kkt_update_wide(c, s_pairs, s_gnz[cur], GB, npairs, tq, band_tile, bord_tile);
+      if (!WS && Gm > 64) chd_kkt_update_wide(c, s_pairs, s_gnz[cur], GB, Gm, tq, band_tile, bord_tile);
       else chd_kkt_update_compact(c, s_pairs, s_cmp[warp], s_gnz[cur], GB, Gm, tq, band_tile, bord_tile);
+#ifdef CHD_PROFILE
+      if (lane == 0) atomicMax(&s_upd_end, (unsigned long long)clock64());
+#endif
     }
     chd_copy_wait(WS);
     __syncthreads();
+#ifdef CHD_PROFILE
+    if (tid == 0) prof_upd += (double)((long long)s_upd_end - tc0);
+#endif
     kslot = kslot + 1 == Q ? 0 : kslot + 1;
   }
+#ifdef CHD_PROFILE
+  if (tid == 0) c.I->prof[6] += prof_diag, c.I->prof[7] += prof_upd;
+#endif
 }
 
 // dense LDL^T of the border Schur complement S = cc[0..nbl)^2 and solve S xb = rb (rb = row NBR of cc); xb goes to
@@ -1173,30 +1162,28 @@ __global__ void __launch_bounds__(256) chd_k_asm(ChdDev D) {
   chd_assemble(D, b, K, I.delta_w, I.sf, blockIdx.x * blockDim.x + threadIdx.x, gridDim.x * blockDim.x, D.rhs0 + go, D.rhs1 + go);
 }
 
-// fp64 throughput probe for the roofline denominators: mode 0 = DFMA chains, mode 1 = DMMA (mma.sync m8n8k4 f64)
+// fp64 throughput probe for the roofline denominators: mode 0 = DFMA chains, mode 1 = DMMA in the shape of the KKT
+// factorisation's panel and trailing updates (mma.sync m16n8k8 f64, DMMA.16x8x8)
 __global__ void __launch_bounds__(256) chd_k_fp64_peak(int mode, int iters, double* sink) {
   const double s = 1.0 + 1e-9 * threadIdx.x;
-  double a[8];
+  double2 a[8];
 #pragma unroll
-  for (int i = 0; i < 8; ++i) a[i] = 0.5 + i;
+  for (int i = 0; i < 8; ++i) a[i] = make_double2(0.5 + i, 1.5 + i);
   if (mode == 0) {
     for (int it = 0; it < iters; ++it) {
 #pragma unroll
-      for (int i = 0; i < 8; ++i) a[i] = fma(a[i], s, 1e-3);
+      for (int i = 0; i < 8; ++i) a[i].x = fma(a[i].x, s, 1e-3);
     }
   } else {
-    const double x = s, y = 1.0 - 1e-9 * threadIdx.x;
+    const double2 x = make_double2(s, s), y = make_double2(1.0 - 1e-9 * threadIdx.x, 1.0);
     for (int it = 0; it < iters; ++it) {
 #pragma unroll
-      for (int i = 0; i < 4; ++i)
-        asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};"
-                     : "+d"(a[2 * i]), "+d"(a[2 * i + 1])
-                     : "d"(x), "d"(y));
+      for (int i = 0; i < 4; ++i) chd_mma_16x8x8(a[2 * i], a[2 * i + 1], x, x, y);
     }
   }
   double t = 0;
 #pragma unroll
-  for (int i = 0; i < 8; ++i) t += a[i];
+  for (int i = 0; i < 8; ++i) t += a[i].x + a[i].y;
   if (t == 123.456) sink[threadIdx.x] = t;
 }
 

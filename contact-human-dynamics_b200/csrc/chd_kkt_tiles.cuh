@@ -11,8 +11,10 @@
 // The right-hand side is stored as the border row right behind the border unknowns of the stage (chd_k_kkt).
 // The factorisation is an unpivoted block LDL^T (the matrix is quasi-definite by construction, DESIGN.md):
 // per block column: 8x8 diagonal LDL^T (warp shuffles) that also yields the inverse of its unit factor, the panel as one
-// FP64 tensor-core (mma.sync m8n8k4) product per tile, and rank-8 tensor-core trailing updates of the elimination window
-// (shared memory, or in place in global memory for wide bands).
+// FP64 tensor-core product per pair of panel tiles, and rank-8 tensor-core trailing updates of the elimination window
+// (shared memory, or in place in global memory for wide bands), two target tiles per instruction.  Both use Hopper's
+// mma.sync m16n8k8 f64 (SASS DMMA.16x8x8), which runs at twice the rate of the Ampere shape m8n8k4; only the single
+// next diagonal tile (chd_tile_sub_xyT) still takes two m8n8k4.
 #pragma once
 #include "chd_dev.h"
 
@@ -60,15 +62,29 @@ __device__ __forceinline__ double* chd_kdiag(const ChdKT& K, int k, bool band = 
   return K.corn + (size_t)(k - K.Na) * (K.nbp8 + 1);
 }
 
-// D(8x8) = C - X * Y^T for row-major 8x8 tiles X, Y (fp64 tensor core, two k-steps of m8n8k4).
-// Fragment layout (PTX ISA, mma.m8n8k4 f64): A[row = lane>>2][k = lane&3], B[k = lane&3][col = lane>>2],
-// C/D[row = lane>>2][col = 2*(lane&3) + {0,1}].
-// accumulator form: (c0, c1) -= (X Y^T)[r][2k, 2k+1].
-// X and Y are panel tiles in *fragment order*: element (row r, column c) of the 8x8 tile sits at
-// r*8 + chd_frag_col(c), so that lane (r = lane>>2, k = lane&3) finds its two operands {c = k, c = k+4} of both
-// k-steps in one aligned 16-byte word at [2*lane] -- a conflict-free LDS.128 instead of two 4-way bank-conflicted
-// 8-byte loads per operand (the trailing updates were shared-memory bound on exactly those conflicts).
+// Fragment layouts (PTX ISA), lane = 4 g + t:
+//   m8n8k4 f64 : A[row g][k t], B[k t][col g], C/D[row g][col 2t + {0,1}]
+//   m16n8k8 f64: A {a0, a1, a2, a3} = A[g][t], A[g+8][t], A[g][t+4], A[g+8][t+4]; B {b0, b1} = B[t][g], B[t+4][g];
+//                C/D {c0, c1} = C[g][2t + {0,1}], {c2, c3} = C[g+8][2t + {0,1}]
+// Panel tiles are kept in *fragment order*: element (row r, column c) of the 8x8 tile sits at r*8 + chd_frag_col(c),
+// so that lane (g, t) finds its two operands (c = t, c = t+4) in one aligned 16-byte word at [2*lane] -- a
+// conflict-free LDS.128 instead of two 4-way bank-conflicted 8-byte loads per operand (the trailing updates were
+// shared-memory bound on exactly those conflicts).  That word is both k-steps of an m8n8k4 pair, and one 8x8 half of
+// the A operand (or all of B) of an m16n8k8.
 __device__ __forceinline__ int chd_frag_col(int c) { return ((c & 3) << 1) | (c >> 2); }
+
+// Two stacked 8x8 products on the fp64 tensor core, one m16n8k8 (DMMA.16x8x8):
+//   [ct; cb] += [Xt; Xb] Y^T,   ct, cb = this lane's (row g, columns 2t, 2t+1) of the top / bottom target tile,
+// xt, xb, y = this lane's (row g, columns t, t+4) of the 8x8 tiles Xt, Xb, Y (the fragment-order word above).
+__device__ __forceinline__ void chd_mma_16x8x8(double2& ct, double2& cb, double2 xt, double2 xb, double2 y) {
+  asm volatile("mma.sync.aligned.m16n8k8.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+               : "+d"(ct.x), "+d"(ct.y), "+d"(cb.x), "+d"(cb.y)
+               : "d"(xt.x), "d"(xb.x), "d"(xt.y), "d"(xb.y), "d"(y.x), "d"(y.y));
+}
+
+// D(8x8) = C - X * Y^T for single 8x8 tiles X, Y in fragment order (two k-steps of m8n8k4): warp 0's update of the
+// next diagonal tile, which has no partner tile, and the kinematic solver's tile products (chd_kin.cu).
+// accumulator form: (c0, c1) -= (X Y^T)[g][2t, 2t+1].
 __device__ __forceinline__ void chd_tile_mma(double& c0, double& c1, const double* X, const double* Y, int lane) {
   const double2 xa = *reinterpret_cast<const double2*>(X + 2 * lane);
   const double2 yb = *reinterpret_cast<const double2*>(Y + 2 * lane);

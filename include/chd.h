@@ -279,7 +279,7 @@ int64_t chd_ik_work_bytes(int32_t F_total, int32_t J, int32_t T);
 const char* chd_version(void);
 
 /* Measurement helper (no reference counterpart): sustained fp64 throughput of the current device in GFLOP/s, for the
- * scalar FMA pipe (DFMA) and for the fp64 tensor-core instruction the KKT kernel uses (mma.sync m8n8k4, DMMA);
+ * scalar FMA pipe (DFMA) and for the fp64 tensor-core instruction the KKT kernel uses (mma.sync m16n8k8, DMMA);
  * MEASURED_PEAKS.json carries no fp64 figure (SURVEY 8(d)).  Either output may be NULL. */
 int chd_measure_fp64_peak(double* dfma_gflops, double* dmma_gflops);
 
