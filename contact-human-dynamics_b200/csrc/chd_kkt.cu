@@ -620,7 +620,9 @@ __device__ __forceinline__ void chd_kkt_update_block(const ChdKktCtx& c, const i
   for (int t = 0; t < 4; ++t) {
     const int a = t & 1, cl = t >> 1;          // tile (row a, column cl) of the block
     bool ok = vi[a] && vj[cl] && !(diag && a == 0 && cl == 1);
-    ok = ok && !(gi[a] == 0 && gj[cl] == 0);   // the next diagonal tile is updated by warp 0
+    // the next diagonal tile is updated by warp 0.  With a single band tile per block column (GB = 0) group 0 is the
+    // first border tile, whose corner block is updated here like every other
+    ok = ok && !(GB > 0 && gi[a] == 0 && gj[cl] == 0);
     // this lane's (row g, columns 2t, 2t+1) of the target: band tile, border tile or corner block (row stride nbp8)
     Cp[t] = nullptr;
     if (ok) {
@@ -762,6 +764,15 @@ __device__ __forceinline__ void chd_kkt_factor(const ChdKktCtx& c, int& s_fail) 
     double* Tkk = WS ? win + (size_t)tri(kslot, kslot) * 64 : K.band + (size_t)Kc * Qs * 64;
     double* Bk = WS ? bwin + (size_t)kslot * nbt * 64 : K.bord + (size_t)Kc * nbt * 64;
     const double* dv = dinv + 8 * cur;
+    // with a single band tile per block column (half bandwidth 0) no trailing update reaches the next diagonal tile, so
+    // warp 0 does not factor it in (c): it is factored here, once the previous block column has streamed it in
+    if (GB == 0 && Kc > 0) {
+      if (warp == 0) {
+        const bool ok = chd_tile_ldl(Tkk, dinv + 8 * cur, s_winv[cur], lane);
+        if (!ok && lane == 0) s_fail = 1;
+      }
+      __syncthreads();
+    }
     // (b) panel: Y = A L0^-T = A W^T (W = L0^-1 from the diagonal-tile factorisation) as one tensor-core product per
     //     pair of 8x8 panel tiles (stacked rows of an m16n8k8), X = Y D^-1; both go to the panel buffers in fragment
     //     order, X also to global (final L); the diagonal tile goes to global as well
