@@ -128,6 +128,34 @@ struct ChdDev {
 #define CHD_INF 1e19
 
 #if defined(__CUDACC__) || defined(CHD_HOST_EMU)
+// Interior-point terms of one constraint row with flags f, defined once for the assembly, the KKT kernel's error
+// measures and step recovery, and the line search: theta and phi at the current iterate and at a trial point are the
+// same functions.  Bounds and multipliers are taken by reference so that a row without the bound never reads them.
+struct ChdGaps { double L, U; };   // s - dL and dU - s; 1.0 for a bound the row does not have
+__device__ __forceinline__ ChdGaps chd_row_gaps(int f, double s, const double& dL, const double& dU) {
+  return {(f & CHD_ROW_HASL) ? s - dL : 1.0, (f & CHD_ROW_HASU) ? dU - s : 1.0};
+}
+struct ChdSigma {   // zL / gapL and zU / gapU (0.0 for a bound the row does not have); their sum is the barrier weight
+  double L, U;
+  __device__ __forceinline__ double sum() const { return L + U; }
+};
+__device__ __forceinline__ ChdSigma chd_row_sigma(int f, ChdGaps gap, const double& zL, const double& zU) {
+  return {(f & CHD_ROW_HASL) ? zL / gap.L : 0.0, (f & CHD_ROW_HASU) ? zU / gap.U : 0.0};
+}
+// coefficient of the barrier parameter in the row's right-hand side
+__device__ __forceinline__ double chd_row_mu_coef(int f, ChdGaps gap) {
+  return ((f & CHD_ROW_HASL) ? 1.0 / gap.L : 0.0) - ((f & CHD_ROW_HASU) ? 1.0 / gap.U : 0.0);
+}
+// primal residual of the scaled constraint value d (theta sums its magnitude, the constraint violation takes the largest)
+__device__ __forceinline__ double chd_row_res(int f, double d, const double& dL, const double& s) {
+  return (f & CHD_ROW_EQ) ? d - dL : d - s;
+}
+// barrier term: acc - mu log gapL - mu log gapU, over the bounds the row has
+__device__ __forceinline__ void chd_row_barrier(int f, double mu, ChdGaps gap, double& acc) {
+  if (f & CHD_ROW_HASL) acc -= mu * log(gap.L);
+  if (f & CHD_ROW_HASU) acc -= mu * log(gap.U);
+}
+
 // a stage ended for this sequence: record its outcome, request the snapshot, move on in the schedule
 // (phys_optim.cpp:709-749: stage 4 only runs when stage 3 did not succeed)
 __device__ __forceinline__ void chd_stage_advance(const ChdDev& D, ChdIpm& I, int status, int snap_after) {

@@ -242,14 +242,10 @@ __global__ void __launch_bounds__(CHD_THREADS) chd_k_linesearch(ChdDev D) {
     for (int r = tid; r < m; r += nt) {
       const int f = rf[r];
       if (!(f & CHD_ROW_ACTIVE)) continue;
-      const double d = D.sc[ro + r] * gt[r];
-      if (f & CHD_ROW_EQ) a_th += fabs(d - D.dL[ro + r]);
-      else {
-        const double st = D.s[ro + r] + alpha * D.ds[ro + r];
-        a_th += fabs(d - st);
-        if (f & CHD_ROW_HASL) a_bar -= mu * log(st - D.dL[ro + r]);
-        if (f & CHD_ROW_HASU) a_bar -= mu * log(D.dU[ro + r] - st);
-      }
+      const bool eq = f & CHD_ROW_EQ;
+      const double st = eq ? 0.0 : D.s[ro + r] + alpha * D.ds[ro + r];   // trial slack (an equality row has none)
+      a_th += fabs(chd_row_res(f, D.sc[ro + r] * gt[r], D.dL[ro + r], st));
+      if (!eq) chd_row_barrier(f, mu, chd_row_gaps(f, st, D.dL[ro + r], D.dU[ro + r]), a_bar);
     }
     const double theta_t = chd_block_sum(a_th, red);
     const double bar_t = chd_block_sum(a_bar, red);
@@ -300,16 +296,15 @@ __global__ void __launch_bounds__(CHD_THREADS) chd_k_linesearch(ChdDev D) {
     if (f & CHD_ROW_EQ) continue;
     const double s = D.s[ro + r] + alpha * D.ds[ro + r];
     D.s[ro + r] = s;
+    const ChdGaps gap = chd_row_gaps(f, s, D.dL[ro + r], D.dU[ro + r]);
     if (f & CHD_ROW_HASL) {
-      const double gap = s - D.dL[ro + r];
       double z = D.zL[ro + r] + a_du * D.dzL[ro + r];
-      z = fmin(fmax(z, mu / (CHD_KAPPA_SIGMA * gap)), CHD_KAPPA_SIGMA * mu / gap);
+      z = fmin(fmax(z, mu / (CHD_KAPPA_SIGMA * gap.L)), CHD_KAPPA_SIGMA * mu / gap.L);
       D.zL[ro + r] = z;
     }
     if (f & CHD_ROW_HASU) {
-      const double gap = D.dU[ro + r] - s;
       double z = D.zU[ro + r] + a_du * D.dzU[ro + r];
-      z = fmin(fmax(z, mu / (CHD_KAPPA_SIGMA * gap)), CHD_KAPPA_SIGMA * mu / gap);
+      z = fmin(fmax(z, mu / (CHD_KAPPA_SIGMA * gap.U)), CHD_KAPPA_SIGMA * mu / gap.U);
       D.zU[ro + r] = z;
     }
   }

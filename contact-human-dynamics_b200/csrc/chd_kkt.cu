@@ -336,16 +336,13 @@ __device__ __forceinline__ void chd_assemble(const ChdDev& D, int b, const ChdKT
     const int e0 = ep[r], e1 = ep[r + 1];
     if (k >= 0) {
       // explicit row: equality, or wide inequality with its slack eliminated
-      double diag = -CHD_DELTA_C, rr0, rr1 = 0.0;
-      if (f & CHD_ROW_EQ) {
-        rr0 = -(sc * D.g[ro + r] - D.dL[ro + r]);
-      } else {
-        const double s = D.s[ro + r];
-        const double gapL = (f & CHD_ROW_HASL) ? s - D.dL[ro + r] : 1.0, gapU = (f & CHD_ROW_HASU) ? D.dU[ro + r] - s : 1.0;
-        const double Sig = ((f & CHD_ROW_HASL) ? D.zL[ro + r] / gapL : 0.0) + ((f & CHD_ROW_HASU) ? D.zU[ro + r] / gapU : 0.0);
+      double diag = -CHD_DELTA_C, rr0 = -chd_row_res(f, sc * D.g[ro + r], D.dL[ro + r], D.s[ro + r]), rr1 = 0.0;
+      if (!(f & CHD_ROW_EQ)) {
+        const ChdGaps gap = chd_row_gaps(f, D.s[ro + r], D.dL[ro + r], D.dU[ro + r]);
+        const double Sig = chd_row_sigma(f, gap, D.zL[ro + r], D.zU[ro + r]).sum();
         diag -= 1.0 / Sig;
-        rr0 = -(sc * D.g[ro + r] - s) + D.y[ro + r] / Sig;
-        rr1 = (((f & CHD_ROW_HASL) ? 1.0 / gapL : 0.0) - ((f & CHD_ROW_HASU) ? 1.0 / gapU : 0.0)) / Sig;
+        rr0 += D.y[ro + r] / Sig;
+        rr1 = chd_row_mu_coef(f, gap) / Sig;
       }
       chd_kadd(K, k, k, diag);
       g_add(k, rr0, rr1);
@@ -363,10 +360,10 @@ __device__ __forceinline__ void chd_assemble(const ChdDev& D, int b, const ChdKT
     } else {
       // condensed narrow inequality row
       const double s = D.s[ro + r];
-      const double gapL = (f & CHD_ROW_HASL) ? s - D.dL[ro + r] : 1.0, gapU = (f & CHD_ROW_HASU) ? D.dU[ro + r] - s : 1.0;
-      const double Sig = ((f & CHD_ROW_HASL) ? D.zL[ro + r] / gapL : 0.0) + ((f & CHD_ROW_HASU) ? D.zU[ro + r] / gapU : 0.0);
-      const double coef0 = Sig * (sc * D.g[ro + r] - s);
-      const double beta = ((f & CHD_ROW_HASL) ? 1.0 / gapL : 0.0) - ((f & CHD_ROW_HASU) ? 1.0 / gapU : 0.0);
+      const ChdGaps gap = chd_row_gaps(f, s, D.dL[ro + r], D.dU[ro + r]);
+      const double Sig = chd_row_sigma(f, gap, D.zL[ro + r], D.zU[ro + r]).sum();
+      const double coef0 = Sig * chd_row_res(f, sc * D.g[ro + r], D.dL[ro + r], s);
+      const double beta = chd_row_mu_coef(f, gap);
       for (int ea = e0; ea < e1; ++ea) {
         const int ca = ec[ea];
         if (ca < 0) continue;
@@ -484,18 +481,16 @@ __device__ __forceinline__ bool chd_kkt_errors(const ChdDev& D, ChdKktCtx& c, in
     a_ysum += fabs(y);
     a_violu = fmax(a_violu, fmax(D.row_lo[ro + r] - gval, gval - D.row_hi[ro + r]));
     rowv[r] = sc * y;
-    if (f & CHD_ROW_EQ) {
-      const double re = d - D.dL[ro + r];
-      a_cviol = fmax(a_cviol, fabs(re));
-      a_theta += fabs(re);
-    } else {
-      const double s = D.s[ro + r], ri = d - s, zL = D.zL[ro + r], zU = D.zU[ro + r];
-      a_cviol = fmax(a_cviol, fabs(ri));
-      a_theta += fabs(ri);
+    const double rp = chd_row_res(f, d, D.dL[ro + r], D.s[ro + r]);
+    a_cviol = fmax(a_cviol, fabs(rp));
+    a_theta += fabs(rp);
+    if (!(f & CHD_ROW_EQ)) {
+      const double zL = D.zL[ro + r], zU = D.zU[ro + r];
+      const ChdGaps gap = chd_row_gaps(f, D.s[ro + r], D.dL[ro + r], D.dU[ro + r]);
       a_rs = fmax(a_rs, fabs(-y - zL + zU));
       a_zsum += zL + zU;
-      if (f & CHD_ROW_HASL) { const double cp = (s - D.dL[ro + r]) * zL; a_cmax = fmax(a_cmax, cp); a_cmin = fmin(a_cmin, cp); }
-      if (f & CHD_ROW_HASU) { const double cp = (D.dU[ro + r] - s) * zU; a_cmax = fmax(a_cmax, cp); a_cmin = fmin(a_cmin, cp); }
+      if (f & CHD_ROW_HASL) { const double cp = gap.L * zL; a_cmax = fmax(a_cmax, cp); a_cmin = fmin(a_cmin, cp); }
+      if (f & CHD_ROW_HASU) { const double cp = gap.U * zU; a_cmax = fmax(a_cmax, cp); a_cmin = fmin(a_cmin, cp); }
     }
   }
   __syncthreads();
@@ -1053,23 +1048,24 @@ __device__ __forceinline__ void chd_kkt_recover(const ChdDev& D, const ChdKktCtx
       const int col = ec[e];
       if (col >= 0) Jdx += Jv[e] * vecn[col];
     }
-    const double riq = sc * D.g[ro + r] - s;
+    const double riq = chd_row_res(f, sc * D.g[ro + r], D.dL[ro + r], s);
     const double ds = sc * Jdx + riq;
     const bool hl = f & CHD_ROW_HASL, hu = f & CHD_ROW_HASU;
-    const double gapL = hl ? s - D.dL[ro + r] : 1.0, gapU = hu ? D.dU[ro + r] - s : 1.0;
+    const ChdGaps gap = chd_row_gaps(f, s, D.dL[ro + r], D.dU[ro + r]);
     const double zL = D.zL[ro + r], zU = D.zU[ro + r];
-    const double sigL = hl ? zL / gapL : 0.0, sigU = hu ? zU / gapU : 0.0;
-    const double bvec = (hl ? mu / gapL : 0.0) - (hu ? mu / gapU : 0.0);
-    const double dy = (sigL + sigU) * ds - D.y[ro + r] - bvec;
-    const double dzL = hl ? mu / gapL - zL - sigL * ds : 0.0;
-    const double dzU = hu ? mu / gapU - zU + sigU * ds : 0.0;
+    const ChdSigma sig = chd_row_sigma(f, gap, zL, zU);
+    const double bvec = (hl ? mu / gap.L : 0.0) - (hu ? mu / gap.U : 0.0);   // mu times chd_row_mu_coef, rounded per bound
+    const double dy = sig.sum() * ds - D.y[ro + r] - bvec;
+    const double dzL = hl ? mu / gap.L - zL - sig.L * ds : 0.0;
+    const double dzU = hu ? mu / gap.U - zU + sig.U * ds : 0.0;
     D.ds[ro + r] = ds, D.dy[ro + r] = dy, D.dzL[ro + r] = dzL, D.dzU[ro + r] = dzU;
-    if (hl && ds < 0) a_pr = fmin(a_pr, -tau * gapL / ds);
-    if (hu && ds > 0) a_pr = fmin(a_pr, tau * gapU / ds);
+    if (hl && ds < 0) a_pr = fmin(a_pr, -tau * gap.L / ds);
+    if (hu && ds > 0) a_pr = fmin(a_pr, tau * gap.U / ds);
     if (hl && dzL < 0) a_du = fmin(a_du, -tau * zL / dzL);
     if (hu && dzU < 0) a_du = fmin(a_du, -tau * zU / dzU);
-    if (hl) a_dphi -= mu * ds / gapL, a_phi -= mu * log(gapL);
-    if (hu) a_dphi += mu * ds / gapU, a_phi -= mu * log(gapU);
+    if (hl) a_dphi -= mu * ds / gap.L;
+    if (hu) a_dphi += mu * ds / gap.U;
+    chd_row_barrier(f, mu, gap, a_phi);
   }
   a_pr = chd_block_min(a_pr, red);
   a_du = chd_block_min(a_du, red);
