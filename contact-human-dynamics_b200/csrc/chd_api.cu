@@ -11,6 +11,7 @@
 
 // kernels (chd_kernels.cu)
 __global__ void chd_k_stage_begin(ChdDev D);
+template <bool GLOBAL>
 __global__ void chd_k_eval(ChdDev D);
 __global__ void chd_k_init(ChdDev D);
 __global__ void chd_k_kkt(ChdDev D);
@@ -25,6 +26,7 @@ __global__ void chd_k_hess_zero(ChdDev D);
 __global__ void chd_k_hess_fin(ChdDev D, int mode);
 __global__ void chd_k_tables(ChdDev D);
 __global__ void chd_k_clear_dyn(ChdDev D);
+template <bool GLOBAL>
 __global__ void chd_k_linesearch(ChdDev D);
 __global__ void chd_k_sample(ChdDev D, double* out, int* frames_out);
 __global__ void chd_k_snapshot(ChdDev D, int* frames_out);
@@ -41,6 +43,22 @@ __global__ void chd_k_sched_reset(ChdDev D);
 
 enum { KT_EVAL = 0, KT_KKT = 1, KT_LS = 2, KT_INIT = 3, KT_SAMPLE = 4, KT_N = 8 };
 
+// Form of the evaluation and line-search kernels for a batch: with the iterate (and the gradient) in shared memory
+// when twice the longest sequence's iterate fits the opt-in limit, otherwise with both in global memory (D.x / D.grad /
+// D.xt) and only the block-reduction buffer in shared memory.  The input size decides; batch creation picks it once.
+struct ChdIterForm {
+  void (*eval)(ChdDev);
+  void (*linesearch)(ChdDev);
+  size_t smem_eval, smem_ls;   // dynamic shared memory per CTA
+};
+static ChdIterForm chd_iter_form(int n_max, int smem_optin) {
+  const size_t red = CHD_THREADS * sizeof(double);
+  if ((2 * (size_t)n_max + CHD_THREADS) * sizeof(double) + 1024 <= (size_t)smem_optin)
+    return {chd_k_eval<false>, chd_k_linesearch<false>, 2 * (size_t)n_max * sizeof(double) + red,
+            (size_t)n_max * sizeof(double) + red};
+  return {chd_k_eval<true>, chd_k_linesearch<true>, red, red};
+}
+
 struct chd_phys_batch {
   ChdHostBatch hb;
   ChdDev D;
@@ -55,7 +73,8 @@ struct chd_phys_batch {
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
   int* d_frames = nullptr;
   double* d_samples = nullptr;
-  size_t smem_eval = 0, smem_kkt = 0, smem_ls = 0;
+  ChdIterForm iter = {};   // evaluation / line-search kernels and their shared memory (chd_iter_form)
+  size_t smem_kkt = 0;
   int kcopy_blocks = 1;
   ChdIpm* h_ipm = nullptr;  // host copy of the per-sequence solver state
   double* d_x0 = nullptr;
@@ -123,7 +142,7 @@ struct Timer {
 
 void launch_eval(chd_phys_batch* b) {
   Timer t(b, KT_EVAL);
-  chd_k_eval<<<b->hb.B, CHD_THREADS, b->smem_eval, b->stream>>>(b->D);
+  b->iter.eval<<<b->hb.B, CHD_THREADS, b->iter.smem_eval, b->stream>>>(b->D);
 }
 
 // uploads the stage table (optionally with an iteration-cap override for one stage) and the schedule
@@ -182,7 +201,7 @@ int run_schedule(chd_phys_batch* b) {
     b->launches++;
     {
       Timer t(b, KT_LS);
-      chd_k_linesearch<<<B, CHD_THREADS, b->smem_ls, b->stream>>>(b->D);
+      b->iter.linesearch<<<B, CHD_THREADS, b->iter.smem_ls, b->stream>>>(b->D);
     }
     // distance-row curvature of the next iteration needs the accepted iterate: after the line search, on the side stream
     CHD_CUDA(cudaEventRecord(b->ev_ls, b->stream));
@@ -342,21 +361,19 @@ static int batch_create_impl(const chd_phys_problem* problems, int32_t batch, co
 #undef AL
   if ((rc = dev_upload(b, hb.x0, (const double**)&b->d_x0))) return rc;
   CHD_CUDA(cudaMemcpyAsync(D.x, b->d_x0, nm * sizeof(double), cudaMemcpyDeviceToDevice, b->stream));
-  // shared-memory budgets
-  b->smem_eval = (2 * (size_t)hb.n_max + CHD_THREADS) * sizeof(double);
-  b->smem_ls = ((size_t)hb.n_max + CHD_THREADS) * sizeof(double);
+  b->iter = chd_iter_form(hb.n_max, smem_max);
   if (P.status == CHD_KKT_TOO_WIDE_COMPACT || P.status == CHD_KKT_TOO_WIDE_PAIRS) {
     fprintf(stderr, "libchd: band + border too wide for the %s (Q=%d nbt=%d)\n",
             P.status == CHD_KKT_TOO_WIDE_COMPACT ? "compacted update loop" : "pair tables", P.Q, P.nbt);
     return -5;
   }
-  if (P.status == CHD_KKT_TOO_LARGE || b->smem_eval + 1024 > (size_t)smem_max) {
-    fprintf(stderr, "libchd: problem too large for the shared-memory staged kernels (n_max=%d)\n", hb.n_max);
+  if (P.status == CHD_KKT_TOO_LARGE) {
+    fprintf(stderr, "libchd: KKT band + border too large for the shared memory of the factorisation (n_max=%d)\n", hb.n_max);
     return -5;
   }
-  CHD_CUDA(cudaFuncSetAttribute(chd_k_eval, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)b->smem_eval));
+  CHD_CUDA(cudaFuncSetAttribute(b->iter.eval, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)b->iter.smem_eval));
   CHD_CUDA(cudaFuncSetAttribute(P.win_smem ? chd_k_kkt : chd_k_kkt_gwin, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)b->smem_kkt));
-  CHD_CUDA(cudaFuncSetAttribute(chd_k_linesearch, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)b->smem_ls));
+  CHD_CUDA(cudaFuncSetAttribute(b->iter.linesearch, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)b->iter.smem_ls));
   const size_t stride = 6 + 7 * (size_t)hb.n_ee_max;
   CHD_CUDA(cudaMallocAsync((void**)&b->d_samples, B * hb.fo_max * stride * sizeof(double), b->stream));
   CHD_CUDA(cudaMallocAsync((void**)&b->d_frames, B * sizeof(int), b->stream));

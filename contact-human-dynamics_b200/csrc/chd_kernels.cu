@@ -6,7 +6,8 @@
 //   chd_k_init        : gradient-based scaling, relaxed bounds, slack / multiplier initialisation
 //   chd_k_kkt         : error measures + barrier update, condensed KKT assembly (band + border),
 //                       unpivoted band LDL^T with dense border, triangular solves, step recovery
-//   chd_k_linesearch  : filter backtracking line search (trial evaluations in shared memory), update
+//   chd_k_linesearch  : filter backtracking line search (trial point in shared memory, or in global memory when the
+//                       iterate is too long for it), update
 //   chd_k_sample      : SaveSolution sampling (phys_optim.cpp:63-143)
 #include <cuda_runtime.h>
 
@@ -79,26 +80,44 @@ __global__ void chd_k_stage_begin(ChdDev D) {
 
 // ------------------------------------------------------------------ evaluation --------------------
 // dynamic shared memory: x[n_max] | grad[n_max] | red[CHD_THREADS]
+// GLOBAL (iterates too long for shared memory, chd_iter_form in chd_api.cu): red[CHD_THREADS] only; x is read from
+// D.x and the gradient accumulates in the sequence's row of D.grad (fp64 global atomics: this CTA is the row's only
+// writer, and the barrier after the zeroing orders it before every addition)
+template <bool GLOBAL>
 __global__ void __launch_bounds__(CHD_THREADS) chd_k_eval(ChdDev D) {
   extern __shared__ double sm[];
   const int b = blockIdx.x;
   if (D.ipm[b].phase != CHD_PH_BEGIN && D.ipm[b].phase != CHD_PH_RUN) return;
   const ChdStageDev sg = D.stages[D.ipm[b].stage];
   const ChdSeq* h = D.seq + b;
-  double* xs = sm;
-  double* gs = sm + D.n_max;
-  double* red = sm + 2 * D.n_max;
-  const double* x = D.x + (size_t)b * D.n_max;
-  for (int i = threadIdx.x; i < h->n; i += blockDim.x) xs[i] = x[i], gs[i] = 0.0;
+  const double* xs;
+  double *gs, *red;
+  if (GLOBAL) {
+    xs = D.x + (size_t)b * D.n_max;
+    gs = D.grad + (size_t)b * D.n_max;
+    red = sm;
+    for (int i = threadIdx.x; i < h->n; i += blockDim.x) gs[i] = 0.0;
+  } else {
+    double* xsm = sm;
+    gs = sm + D.n_max;
+    red = sm + 2 * D.n_max;
+    const double* x = D.x + (size_t)b * D.n_max;
+    for (int i = threadIdx.x; i < h->n; i += blockDim.x) xsm[i] = x[i], gs[i] = 0.0;
+    xs = xsm;
+  }
   __syncthreads();
   ChdCtx c;
   chd_make_ctx(D, b, xs, c);
   c.dyn = D.ipm[b].dyn;
   c.opt_dur = sg.opt_dur;
   chd_eval_all<true>(c, sg, D.g + (size_t)b * D.m_max, D.Jv + (size_t)b * D.slots_max, gs, D.cost + 2 * b, red);
-  double* grad = D.grad + (size_t)b * D.n_max;
-  for (int i = threadIdx.x; i < h->n; i += blockDim.x) grad[i] = gs[i];
+  if (!GLOBAL) {
+    double* grad = D.grad + (size_t)b * D.n_max;
+    for (int i = threadIdx.x; i < h->n; i += blockDim.x) grad[i] = gs[i];
+  }
 }
+template __global__ void chd_k_eval<false>(ChdDev D);
+template __global__ void chd_k_eval<true>(ChdDev D);
 
 // ------------------------------------------------------------------ init --------------------------
 // IPOPT gradient-based scaling (nlp_scaling_max_gradient 100), relaxed bounds, slack push, z = 1, y = 0.
@@ -176,6 +195,9 @@ __global__ void __launch_bounds__(CHD_THREADS) chd_k_init(ChdDev D) {
 
 // ------------------------------------------------------------------ line search -------------------
 // dynamic shared memory: xt[n_max] | red[CHD_THREADS]
+// GLOBAL (iterates too long for shared memory, chd_iter_form in chd_api.cu): red[CHD_THREADS] only; the trial point is
+// built in the sequence's row of D.xt
+template <bool GLOBAL>
 __global__ void __launch_bounds__(CHD_THREADS) chd_k_linesearch(ChdDev D) {
   extern __shared__ double sm[];
   __shared__ int s_ok, s_ftype, s_trust;
@@ -188,8 +210,8 @@ __global__ void __launch_bounds__(CHD_THREADS) chd_k_linesearch(ChdDev D) {
   const int n = h->n, m = h->m, tid = threadIdx.x, nt = blockDim.x;
   const size_t ro = (size_t)b * D.m_max, vo = (size_t)b * D.n_max;
   const int* rf = D.rflag + ro;
-  double* xt = sm;
-  double* red = sm + D.n_max;
+  double* xt = GLOBAL ? D.xt + vo : sm;
+  double* red = GLOBAL ? sm : sm + D.n_max;
   const double* x = D.x + vo;
   const double* dx = D.dx + vo;
   double* gt = D.gt + ro;
@@ -338,6 +360,8 @@ __global__ void __launch_bounds__(CHD_THREADS) chd_k_linesearch(ChdDev D) {
     I.step_ready = 0;
   }
 }
+template __global__ void chd_k_linesearch<false>(ChdDev D);
+template __global__ void chd_k_linesearch<true>(ChdDev D);
 
 // ------------------------------------------------------------------ sampling ----------------------
 // SaveSolution (phys_optim.cpp:63-143): t accumulates dt while t <= T + 1e-5.

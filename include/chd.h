@@ -68,7 +68,8 @@ typedef struct chd_phys_options {
 } chd_phys_options;
 /* Builds the NLP layouts of `batch` sequences on the host and uploads them to the current CUDA device.
  * device < 0 keeps the current device.  weights and opt may be NULL: the defaults.  Returns -1 for a bad argument or an
- * option out of range. */
+ * option out of range, -5 when the batch's KKT band + border does not fit the factorisation kernels.  The length of a
+ * sequence is not limited otherwise: iterates too long for shared memory are evaluated from global memory. */
 int chd_phys_batch_create(const chd_phys_problem* problems, int32_t batch, const chd_phys_weights* weights,
                           int32_t device, const chd_phys_options* opt, chd_phys_batch** out);
 void chd_phys_batch_destroy(chd_phys_batch* b);

@@ -1,6 +1,9 @@
 #!/usr/bin/env python
 """Long-horizon configuration of BASELINE.json (600-frame sequences, 4 end-effectors, dense contact switches):
-solve a batch on cuda:0 and report per-stage status / iterations / residuals and the wall time.
+solve a batch on cuda:0 and report per-stage status / iterations / residuals, the wall time, the evaluation and
+line-search kernel time per launch and the card's name and power limit.  Clips of any length run: past about 14 200
+variables per sequence (e.g. --frames 1200 --sparse, or --frames 900) the evaluation and line-search kernels keep the
+iterate in global memory instead of shared memory.
 
 --stage3-long runs stage 3 on these sequences too (switch times as band unknowns, `PhysBatch(stage3_band_above=96)`);
 --stage-times N then solves the stages once more, one by one for the whole batch with at most N iterations each, and
@@ -8,12 +11,23 @@ reports the KKT kernel time per launch of every stage."""
 import argparse
 import json
 import os
+import subprocess
 import sys
 import time
 
 import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+
+
+def gpu_card():
+    """name and power limit [W] of cuda:0 (nvidia-smi), None where it cannot be read"""
+    try:
+        out = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=name,power.limit", "--format=csv,noheader,nounits"],
+                             capture_output=True, text=True, timeout=30).stdout.strip().split(",")
+        return {"gpu": out[0].strip(), "power_limit_w": float(out[1])}
+    except Exception:
+        return {"gpu": None, "power_limit_w": None}
 
 
 def main():
@@ -44,6 +58,7 @@ def main():
         per_stage[name] = {"status": {int(v): int(c) for v, c in zip(vals, cnts)},
                            "iters_min_median_max": [int(it[s][ran].min()), float(np.median(it[s][ran])), int(it[s][ran].max())]
                            if ran.any() else None}
+    kt = batch.kernel_times()
     res = {
         "config": "%d x %d frames, %d ee, %s" % (args.batch, args.frames, args.n_ee, "walk" if args.sparse else "dense switches"),
         "stage3_band_above": band,
@@ -53,7 +68,10 @@ def main():
         "stage_status": st.tolist(), "stage_iters": it.tolist(), "per_stage": per_stage,
         "stage3_converged": float((st[4] == 0).mean()),
         "success": out["success"].tolist(), "launches": int(batch.launch_count()),
-        "kernels": {k: list(v) for k, v in batch.kernel_times().items()},
+        "kernels": {k: list(v) for k, v in kt.items()},
+        "eval_ms_per_launch": kt["eval"][0] / max(kt["eval"][1], 1),
+        "linesearch_ms_per_launch": kt["linesearch"][0] / max(kt["linesearch"][1], 1),
+        **gpu_card(),
     }
     if args.stage_times:
         batch.reset()

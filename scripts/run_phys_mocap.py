@@ -17,6 +17,7 @@ import glob
 import os
 import shutil
 import sys
+import time
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
@@ -46,11 +47,13 @@ def main(argv=None):
         sys.exit("No video directories in the data path!")
     dev = "cuda:%d" % a.device
     problems, meta = [], []
+    secs = {"kinematic": 0.0, "physics": 0.0, "apply": 0.0}   # wall time per stage of the pipeline, all videos
     for v in vids:
         vd = os.path.join(a.data, v)
         n = len(glob.glob(os.path.join(vd, "openpose_result", "*.json")))
         kin = os.path.join(vd, "kinematic_results")
         print("Running kinematic optimization for %s (%d frames)..." % (v, n))
+        t0 = time.time()
         chd.kinopt.optimize_2d_3d(os.path.join(vd, v + ".mp4"), a.skel_path, kin, 0, n, a.kinematic_gt_floor, device=dev)
         char_bvh = os.path.join(kin, a.character + "_out.bvh")
         if a.character == "combined":
@@ -65,9 +68,13 @@ def main(argv=None):
                                       1.0 / a.fps, False, device=dev)
         problems.append(io_formats.read_phys_inputs(pin, n))      # through the files, like the reference's binary
         meta.append((v, vd, n, char_bvh))
+        secs["kinematic"] += time.time() - t0
     print("Running physics-based optimization (%d sequences, one batch)..." % len(problems))
+    t0 = time.time()
     with chd.phys.PhysBatch(problems, device=a.device) as batch:
         out = batch.solve()
+    secs["physics"] = time.time() - t0
+    t0 = time.time()
     for i, (v, vd, n, char_bvh) in enumerate(meta):
         pout = os.path.join(vd, "phys_optim_out_" + a.character)
         os.makedirs(pout, exist_ok=True)
@@ -79,6 +86,9 @@ def main(argv=None):
                 anim = chd.results.remove_heel_from_anim(anim)                      # towr_utils.py:972-974
             chd.results.save_bvh(os.path.join(pout, "%s_%s_%s.bvh" % (v, a.character, tag)), anim, anim.names)
         print("%s: dynamics %d durations %d" % (v, out["success"][i, 0], out["success"][i, 1]))
+    secs["apply"] = time.time() - t0
+    print("wall time: kinematic %.1f s (with the phys-optim inputs), physics %.1f s, apply %.1f s (with the .bvh files)" % (
+        secs["kinematic"], secs["physics"], secs["apply"]))
 
 
 if __name__ == "__main__":
