@@ -169,21 +169,21 @@ def write_solution(path: str, dt: float, sample: np.ndarray, n_ee: int) -> None:
     """`sample` is (N, 6+7*n_ee): base_lin(3) base_ang_deg(3) ee_pos(3*n_ee) ee_force(3*n_ee)
     contact(n_ee) -- the layout SaveSolution walks (phys_optim.cpp:63-143).  Label line / value line
     pairs; values separated by single spaces, no trailing space."""
+    from .phys import sample_columns        # here, not at the top: phys imports this module
+    base, pos, frc, flag = sample_columns(n_ee, n_ee)
     N = sample.shape[0]
     with open(path, "w") as f:
         f.write("dt\n%s\n" % _g10(dt))
         f.write("num_frames\n%d\n" % N)
         f.write("num_feet\n%d\n" % n_ee)
-        f.write("base_lin\n" + " ".join(_g10(x) for x in sample[:, 0:3].reshape(-1)) + "\n")
-        f.write("base_ang\n" + " ".join(_g10(x) for x in sample[:, 3:6].reshape(-1)) + "\n")
+        f.write("base_lin\n" + " ".join(_g10(x) for x in sample[:, base[:3]].reshape(-1)) + "\n")
+        f.write("base_ang\n" + " ".join(_g10(x) for x in sample[:, base[3:]].reshape(-1)) + "\n")
         for i in range(n_ee):
-            f.write("foot%d_pos\n" % i + " ".join(_g10(x) for x in sample[:, 6 + 3 * i:9 + 3 * i].reshape(-1)) + "\n")
+            f.write("foot%d_pos\n" % i + " ".join(_g10(x) for x in sample[:, pos[3 * i:3 * i + 3]].reshape(-1)) + "\n")
         for i in range(n_ee):
-            o = 6 + 3 * n_ee + 3 * i
-            f.write("foot%d_force\n" % i + " ".join(_g10(x) for x in sample[:, o:o + 3].reshape(-1)) + "\n")
+            f.write("foot%d_force\n" % i + " ".join(_g10(x) for x in sample[:, frc[3 * i:3 * i + 3]].reshape(-1)) + "\n")
         for i in range(n_ee):
-            o = 6 + 6 * n_ee + i
-            f.write("foot%d_contact\n" % i + " ".join("%d" % int(round(x)) for x in sample[:, o]) + "\n")
+            f.write("foot%d_contact\n" % i + " ".join("%d" % int(round(x)) for x in sample[:, flag[i]]) + "\n")
 
 
 def write_success_log(path: str, dynamics_succeed: bool, durations_succeed: bool) -> None:

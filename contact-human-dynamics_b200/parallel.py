@@ -10,6 +10,8 @@ from typing import List, Sequence, Tuple
 
 import numpy as np
 
+from . import phys
+
 
 def shard_by_work(work: Sequence[float], world: int) -> List[List[int]]:
     """Deals sequence indices to ranks: sorted by estimated work (number of variables ~ iterations x size),
@@ -87,14 +89,13 @@ class ShardedSolver:
         self.slots = pad_to(self.shards)
         self.mine = self.shards[rank]
         self.n_ee_max = max(p.n_ee for p in self.problems)
-        self.stride = 6 + 7 * self.n_ee_max
+        self.stride = phys.sample_stride(self.n_ee_max)
         self.fo = max(frames_out(p) for p in self.problems)
         self.width = self.fo * self.stride + N_EXTRA
         self.solve_fn = solve_fn
         self.batch = None
         import torch
         if solve_fn is None:
-            from . import phys
             self.batch = phys.PhysBatch([self.problems[i] for i in self.mine], weights=weights, device=device,
                                         stage3_band_above=stage3_band_above) if self.mine else None
             tensor_device = tensor_device or torch.device("cuda", device)
@@ -130,7 +131,7 @@ class ShardedSolver:
             sstat, siter, success = np.zeros((6, B), np.int32), np.zeros((6, B), np.int32), np.zeros((B, 2), np.int32)
             b._chk(b.L.chd_phys_solve(b.h, None, None, success.ctypes.data, sstat.ctypes.data, siter.ctypes.data))
             # final iterate sampled on the device straight into the send buffer (no host round trip)
-            fo_l, st_l = b.dims["frames_out_max"], 6 + 7 * b.n_ee_max
+            fo_l, st_l = b.dims["frames_out_max"], phys.sample_stride(b.n_ee_max)
             if fo_l == self.fo and st_l == self.stride:
                 view = self.send[:n, :self.fo * self.stride]
                 if view.is_contiguous():

@@ -25,6 +25,19 @@ STAGES = {"1.1": 0, "1.2": 1, "2.1": 2, "2.2": 3, "3": 4, "4": 5}
 SET_NAMES = {0: "acc", 1: "terrain", 2: "rom", 3: "dyn", 4: "force", 5: "heel", 6: "height", 7: "tottime", 8: "durpos"}
 
 
+def sample_stride(n_ee_max: int) -> int:
+    """Columns of a SaveSolution sample row (phys_optim.cpp:63-143) of a batch with up to n_ee_max end-effectors:
+    base_lin (3), base_ang in degrees (3), foot positions (3 n_ee_max), foot forces (3 n_ee_max), contact flags (n_ee_max)."""
+    return 6 + 7 * n_ee_max
+
+
+def sample_columns(n_ee: int, n_ee_max: int):
+    """(base, pos, frc, flag): column indices of the base (6), foot positions (3 n_ee), foot forces (3 n_ee) and contact
+    flags (n_ee) of the first n_ee end-effectors in a sample row padded for n_ee_max (`sample_stride`)."""
+    return (np.arange(6), np.arange(6, 6 + 3 * n_ee), np.arange(6 + 3 * n_ee_max, 6 + 3 * n_ee_max + 3 * n_ee),
+            np.arange(6 + 6 * n_ee_max, 6 + 6 * n_ee_max + n_ee))
+
+
 class _Problem(C.Structure):
     _fields_ = [("n_frames", C.c_int32), ("n_ee", C.c_int32), ("dt", C.c_double),
                 ("hip_left", C.POINTER(C.c_double)), ("hip_right", C.POINTER(C.c_double)),
@@ -296,8 +309,7 @@ class PhysBatch:
     def solve(self) -> dict:
         """Full staged schedule.  Returns the three SaveSolution snapshots, frame counts, success flags."""
         B, d = self.B, self.dims
-        stride = 6 + 7 * self.n_ee_max
-        samples = np.zeros((3, B, d["frames_out_max"], stride))
+        samples = np.zeros((3, B, d["frames_out_max"], sample_stride(self.n_ee_max)))
         frames = np.zeros(B, np.int32)
         success = np.zeros((B, 2), np.int32)
         sstat = np.zeros((6, B), np.int32)
@@ -307,7 +319,7 @@ class PhysBatch:
 
     def sample(self):
         B, d = self.B, self.dims
-        out = np.zeros((B, d["frames_out_max"], 6 + 7 * self.n_ee_max))
+        out = np.zeros((B, d["frames_out_max"], sample_stride(self.n_ee_max)))
         frames = np.zeros(B, np.int32)
         self._chk(self.L.chd_phys_sample(self.h, _ptr(out), _ptr(frames)))
         return out, frames
@@ -346,9 +358,7 @@ def write_outputs(out: dict, i: int, problem: PhysProblem, out_dir: str, n_ee_ma
     n_ee = problem.n_ee
     ne_max = n_ee_max if n_ee_max is not None else (out["samples"].shape[-1] - 6) // 7
     nf = int(out["frames"][i])
-    # strip the padding columns of a mixed n_ee batch
-    cols = list(range(6)) + [6 + 3 * e + d for e in range(n_ee) for d in range(3)] + \
-        [6 + 3 * ne_max + 3 * e + d for e in range(n_ee) for d in range(3)] + [6 + 6 * ne_max + e for e in range(n_ee)]
+    cols = np.concatenate(sample_columns(n_ee, ne_max))     # strips the padding columns of a mixed n_ee batch
     for snap, name in enumerate(SOLUTION_FILES):
         write_solution(os.path.join(out_dir, name), problem.dt, out["samples"][snap, i, :nf][:, cols], n_ee)
     write_success_log(os.path.join(out_dir, "success_log.txt"), out["success"][i, 0], out["success"][i, 1])

@@ -11,7 +11,8 @@ ps = [chd.synth.make_problem(s, n_frames=F, n_ee=n_ee, dense=dense) for s in see
 b = chd.phys.PhysBatch(ps)
 out = b.solve()
 st = b.stage_stats()
-ids = {"1.1": 0, "1.2": 1, "2.1": 2, "2.2": 3, "3": 4, "4": 5}
+ids = chd.phys.STAGES
+base, pos, frc, _ = chd.phys.sample_columns(n_ee, n_ee)
 for i, p in enumerate(ps):
     ref = OracleProblem(p).solve()
     print("seed", seeds[i], "gpu iters", out["stage_iters"][:, i].tolist(), "status", out["stage_status"][:, i].tolist())
@@ -19,4 +20,4 @@ for i, p in enumerate(ps):
     print("   gpu f", ["%.6f" % st[ids[k], i, 0] for k in ref["stage_ids"]], "viol", ["%.1e" % st[ids[k], i, 2] for k in ref["stage_ids"]])
     nf = out["frames"][i]
     d = np.abs(out["samples"][2, i, :nf] - ref["durations"])
-    print("   max |diff| pos %.2e force %.2e" % (d[:, :6 + 3 * n_ee].max(), d[:, 6 + 3 * n_ee:6 + 6 * n_ee].max()))
+    print("   max |diff| pos %.2e force %.2e" % (d[:, np.r_[base, pos]].max(), d[:, frc].max()))

@@ -57,8 +57,7 @@ def main(argv=None):
             ne_max = max(p.n_ee for p in problems)
             for i, (p, od) in enumerate(zip(problems, out_dirs)):
                 nf, n_ee = int(out["frames"][i]), p.n_ee
-                cols = list(range(6)) + [6 + 3 * e + d for e in range(n_ee) for d in range(3)] + \
-                    [6 + 3 * ne_max + 3 * e + d for e in range(n_ee) for d in range(3)] + [6 + 6 * ne_max + e for e in range(n_ee)]
+                cols = np.concatenate(chd.phys.sample_columns(n_ee, ne_max))
                 chd.io_formats.write_solution(os.path.join(od, "sol_out_durations.txt"), p.dt, out["samples"][i, :nf][:, cols], n_ee)
                 chd.io_formats.write_success_log(os.path.join(od, "success_log.txt"), out["success"][i, 0], out["success"][i, 1])
         return

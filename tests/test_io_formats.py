@@ -40,8 +40,9 @@ def test_input_files_round_trip(chd, tmp_path):
 def test_solution_file_layout(chd, tmp_path):
     rng = np.random.default_rng(0)
     n_ee, N = 4, 17
-    s = rng.normal(size=(N, 6 + 7 * n_ee))
-    s[:, 6 + 6 * n_ee:] = rng.integers(0, 2, size=(N, n_ee))
+    base, _, frc, flag = chd.phys.sample_columns(n_ee, n_ee)
+    s = rng.normal(size=(N, chd.phys.sample_stride(n_ee)))
+    s[:, flag] = rng.integers(0, 2, size=(N, n_ee))
     path = str(tmp_path / "sol_out_dynamics.txt")
     chd.io_formats.write_solution(path, 1.0 / 30, s, n_ee)
     lines = open(path).read().split("\n")
@@ -52,8 +53,8 @@ def test_solution_file_layout(chd, tmp_path):
     assert not lines[7].endswith(" ") and len(lines[7].split()) == 3 * N
     r = chd.io_formats.read_solution(path)
     assert r["num_frames"] == N and r["num_feet"] == n_ee
-    np.testing.assert_allclose(r["base_lin"], s[:, 0:3], rtol=1e-9)       # 10 significant digits
-    np.testing.assert_allclose(r["foot_force"][2], s[:, 6 + 3 * n_ee + 6:6 + 3 * n_ee + 9], rtol=1e-9)
-    np.testing.assert_array_equal(r["foot_contact"][3], s[:, 6 + 6 * n_ee + 3].astype(np.int64))
+    np.testing.assert_allclose(r["base_lin"], s[:, base[:3]], rtol=1e-9)       # 10 significant digits
+    np.testing.assert_allclose(r["foot_force"][2], s[:, frc[6:9]], rtol=1e-9)
+    np.testing.assert_array_equal(r["foot_contact"][3], s[:, flag[3]].astype(np.int64))
     chd.io_formats.write_success_log(str(tmp_path / "success_log.txt"), True, False)
     assert open(str(tmp_path / "success_log.txt")).read() == "dynamics 1\ndurations 0\n"

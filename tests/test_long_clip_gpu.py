@@ -10,7 +10,8 @@ import sys
 import numpy as np
 import pytest
 
-from tests.util import GPU_STAGE_IDS, master_to_oracle_perm
+from tests.util import (assert_ipopt_termination, assert_loosely_close, assert_samples_close, assert_solves_agree,
+                        master_to_oracle_perm)
 
 pytestmark = pytest.mark.gpu
 
@@ -23,15 +24,6 @@ RTOL = 1e-10
 
 def _long(chd):
     return chd.synth.make_problem(0, n_frames=FRAMES, n_ee=N_EE)
-
-
-def _close(got, exp, n_ee):
-    """max |diff| of positions / angles, forces; asserts 1e-5 (m, deg) and 1e-3 N, contact flags bit-exact."""
-    npos, nfrc = 6 + 3 * n_ee, 6 + 6 * n_ee
-    dp, df = np.abs(got[:, :npos] - exp[:, :npos]).max(), np.abs(got[:, npos:nfrc] - exp[:, npos:nfrc]).max()
-    assert dp <= 1e-5 and df <= 1e-3, (dp, df)
-    np.testing.assert_array_equal(got[:, nfrc:], exp[:, nfrc:])
-    return dp, df
 
 
 @pytest.fixture(scope="module")
@@ -94,71 +86,11 @@ def test_long_clip_eval_parity(chd, stage):
         assert np.abs((J - Jo).data).max(initial=0.0) <= RTOL * np.abs(Jo.data).max()
 
 
-def _feet(s, n_ee, n_ee_max):
-    """sample rows laid out for n_ee_max end-effectors -> the columns of the first n_ee (base, positions, forces, flags)"""
-    cols = list(range(6)) + [6 + 3 * e + d for e in range(n_ee) for d in range(3)] + \
-        [6 + 3 * n_ee_max + 3 * e + d for e in range(n_ee) for d in range(3)] + [6 + 6 * n_ee_max + e for e in range(n_ee)]
-    return s[:, cols]
-
-
 def test_shared_and_global_forms_agree(solved):
     """The benchmark seeds solved by the shared-memory form (alone) and by the global-memory form (long clip appended):
     the same algorithm with the same arithmetic, up to the order of the gradient's atomic additions."""
-    _, ref, _, got = solved
-    st, it = got["stage_status"][:, :16], got["stage_iters"][:, :16]
-    np.testing.assert_array_equal(st[:4], ref["stage_status"][:4])
-    np.testing.assert_array_equal(it[:4], ref["stage_iters"][:4])
-    fixed = [[_close(_feet(got["samples"][snap, i, :120], 2, N_EE), ref["samples"][snap, i, :120], 2) for i in range(16)]
-             for snap in (0, 1)]
-    print("stages 1.1-2.2: max |diff| positions %.2e, forces %.2e" % (np.max([f[0] for s in fixed for f in s]),
-                                                                     np.max([f[1] for s in fixed for f in s])))
-    np.testing.assert_array_equal(st[4], ref["stage_status"][4])
-    np.testing.assert_array_equal(st[5], ref["stage_status"][5])
-    same = np.nonzero(it[4] == ref["stage_iters"][4])[0]
-    print("stage 3: iteration counts equal for %d / 16 sequences" % len(same))
-    assert len(same) >= 0.9 * 16
-    d3 = [_close(_feet(got["samples"][2, i, :120], 2, N_EE), ref["samples"][2, i, :120], 2) for i in same]
-    print("stage 3: max |diff| positions %.2e, forces %.2e" % (max(d[0] for d in d3), max(d[1] for d in d3)))
-
-
-def _kkt_residuals_ok(chd, b, i, p, stage):
-    """IPOPT's termination test at the final point of a fixed-duration stage, residuals recomputed with the oracle's
-    callbacks (as test_stage3_band_gpu.py's, without the duration columns): scaled stationarity, feasibility and
-    complementarity <= tol = 1e-3, unscaled constraint violation <= constr_viol_tol = 1e-4."""
-    from oracle.phys import OracleProblem
-    x, du, lay = b.get_x(), b.duals(), b.layout()
-    o = OracleProblem(p)
-    o.set_stage(stage)
-    n = o.n
-    o.set_x(x[i, :n])
-    sl = chd.phys.master_row_slices(b, i, lay)
-    im, io = master_to_oracle_perm(sl, o)
-    assert len(io) == o.m
-    c, J, g = o.cons(), o.jac().tocsr(), o.grad()
-    cl, cu = o.con_bounds()
-    sc, sf = du["row_scale"][i], du["obj_scale"][i]
-    y, zL, zU, s = du["y"][i], du["zL"][i], du["zU"][i], du["s"][i]
-    assert max(np.maximum(cl - c, c - cu).max(), 0.0) <= 1e-4
-    lam = np.zeros(o.m)
-    lam[io] = (sc * y)[im]
-    r = sf * g + J.T @ lam
-    free = lay["var_kkt"][i, :n] >= 0
-    lo, hi = lay["row_lo"][i, im], lay["row_hi"][i, im]
-    ineq = lo != hi
-    nbnd = int((lo[ineq] > -1e19).sum() + (hi[ineq] < 1e19).sum())
-    s_d = max(100.0, (np.abs(y[im]).sum() + (zL[im][ineq] + zU[im][ineq]).sum()) / (len(im) + nbnd)) / 100.0
-    assert np.abs(r[free]).max() / s_d <= 1e-3
-    cm = np.zeros(len(y))
-    cm[im] = c[io]
-    ri = im[ineq]
-    assert np.abs(sc[ri] * cm[ri] - s[ri]).max() <= 1e-3
-    lo_s, hi_s = lay["row_lo"][i, ri] * sc[ri], lay["row_hi"][i, ri] * sc[ri]
-    relax = lambda v: 1e-8 * np.maximum(1.0, np.abs(v))
-    hasl, hasu = lay["row_lo"][i, ri] > -1e19, lay["row_hi"][i, ri] < 1e19
-    comp = np.concatenate([((s[ri] - (lo_s - relax(lo_s))) * zL[ri])[hasl], (((hi_s + relax(hi_s)) - s[ri]) * zU[ri])[hasu]])
-    s_c = max(100.0, (zL[ri][hasl].sum() + zU[ri][hasu].sum()) / max(len(comp), 1)) / 100.0
-    assert (comp >= 0).all() and comp.max() / s_c <= 1e-3
-    assert np.abs(-y[ri] - zL[ri] + zU[ri]).max() / s_d <= 1e-3
+    _, ref, mixed, got = solved
+    assert_solves_agree(ref, got, 2, n_ee_max=mixed.n_ee_max)
 
 
 def test_long_clip_matches_oracle(chd, solved):
@@ -173,24 +105,22 @@ def test_long_clip_matches_oracle(chd, solved):
     st, it = out["stage_status"][:, i], out["stage_iters"][:, i]
     print("GPU status %s iters %s" % (st.tolist(), it.tolist()))
     print("oracle %s %s %s (%.0f s)" % (ids, g["status"].tolist(), g["iters"].tolist(), float(g["seconds"])))
-    assert st[GPU_STAGE_IDS["3"]] == -3
-    assert [int(st[GPU_STAGE_IDS[k]]) for k in ids] == [int(v) for v in g["status"]]
+    assert st[chd.phys.STAGES["3"]] == -3
+    assert [int(st[chd.phys.STAGES[k]]) for k in ids] == [int(v) for v in g["status"]]
     for k in range(4):
-        assert int(it[GPU_STAGE_IDS[ids[k]]]) == int(g["iters"][k]), (ids[k], it.tolist(), g["iters"].tolist())
+        assert int(it[chd.phys.STAGES[ids[k]]]) == int(g["iters"][k]), (ids[k], it.tolist(), g["iters"].tolist())
     nf = out["frames"][i]
     assert nf == FRAMES
     for snap, key in enumerate(["no_dynamics", "dynamics"]):
-        dp, df = _close(out["samples"][snap, i, :nf], g[key], N_EE)
+        dp, df = assert_samples_close(out["samples"][snap, i, :nf], g[key], N_EE)
         print("%s: max |diff| positions %.2e, forces %.2e" % (key, dp, df))
-    # stage 4 replaces stage 3: the tolerances of test_stage3_band_gpu.py::test_banded_above_limit_matches_oracle
-    got, exp = out["samples"][2, i, :nf], g["durations"]
-    print("stage 4: iterations GPU %d oracle %d, max |diff| COM %.2e" % (it[GPU_STAGE_IDS["4"]], g["iters"][4],
-                                                                      np.abs(got[:, :3] - exp[:, :3]).max()))
-    assert np.abs(got[:, :3] - exp[:, :3]).max() < 0.02
-    assert (got[:, 30:] != exp[:, 30:]).mean() < 0.02
+    # stage 4 replaces stage 3: the loose check of a stage that takes its own path on either side
+    print("stage 4: iterations GPU %d oracle %d" % (it[chd.phys.STAGES["4"]], g["iters"][4]))
+    dcom = assert_loosely_close(out["samples"][2, i, :nf], g["durations"], N_EE)
+    print("stage 4: max |diff| COM %.2e" % dcom)
     assert out["success"][i].tolist() == [int(v) for v in g["success"]]
-    if st[GPU_STAGE_IDS["4"]] == 0:
-        _kkt_residuals_ok(chd, b, i, p, "4")
+    if st[chd.phys.STAGES["4"]] == 0:
+        assert_ipopt_termination(chd, b, i, p, "4")
 
 
 def test_long_clip_through_phys_optim_files(chd, tmp_path):

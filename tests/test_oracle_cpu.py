@@ -122,4 +122,4 @@ def test_oracle_ipm_converges_and_satisfies_constraints(chd):
     lo, hi = o.con_bounds()
     viol = np.maximum(lo - c, 0) + np.maximum(c - hi, 0)
     assert viol.max() <= 1e-4                                # IPOPT constr_viol_tol
-    assert res["durations"].shape == (60, 6 + 7 * 2)
+    assert res["durations"].shape == (60, chd.phys.sample_stride(2))

@@ -55,15 +55,15 @@ def test_shard_by_work_balanced(chd):
 
 def _oracle_solve_fn(problems):
     """stand-in for the CUDA solve of a shard in the CPU test: the oracle solves the same NLPs (test infrastructure)"""
+    import chd
     from oracle.phys import OracleProblem
-    ids = {"1.1": 0, "1.2": 1, "2.1": 2, "2.2": 3, "3": 4, "4": 5}
     finals, frames, succ = [], [], []
     sstat, siter = np.full((6, len(problems)), -9, np.int32), np.zeros((6, len(problems)), np.int32)
     for i, p in enumerate(problems):
         r = OracleProblem(p).solve()
         finals.append(r["durations"]), frames.append(len(r["durations"])), succ.append(r["success"])
         for k, s in zip(r["stage_ids"], r["stages"]):
-            sstat[ids[k], i], siter[ids[k], i] = s["status"], s["iters"]
+            sstat[chd.phys.STAGES[k], i], siter[chd.phys.STAGES[k], i] = s["status"], s["iters"]
     fo = max(frames)
     blk = np.zeros((len(problems), fo, finals[0].shape[1]))
     for i, f in enumerate(finals):

@@ -144,8 +144,8 @@ def test_prepare_input_files_round_trip(chd, clip, tmp_path):
 def test_load_results_parses_solution_files(chd, tmp_path):
     rng = np.random.default_rng(0)
     N, n_ee = 12, 4
-    s = rng.normal(size=(N, 6 + 7 * n_ee))
-    s[:, 6 + 6 * n_ee:] = rng.integers(0, 2, (N, n_ee))
+    s = rng.normal(size=(N, chd.phys.sample_stride(n_ee)))
+    s[:, chd.phys.sample_columns(n_ee, n_ee)[3]] = rng.integers(0, 2, (N, n_ee))
     for name in ("sol_out_no_dynamics.txt", "sol_out_dynamics.txt", "sol_out_durations.txt"):
         chd.io_formats.write_solution(str(tmp_path / name), 1 / 30.0, s, n_ee)
     chd.io_formats.write_success_log(str(tmp_path / "success_log.txt"), True, False)

@@ -20,13 +20,14 @@ def test_solution_file_round_trip_through_load_results(chd, tmp_path_factory, se
     chd.io_formats.write_solution(path, 1.0 / 30.0, sample, n_ee)
     r = chd.results.load_towr_results(path)
     assert r.num_feet == n_ee and r.base_pos.shape == (N, 3)
-    np.testing.assert_allclose(r.base_pos, -sample[:, [0, 2, 1]], rtol=1e-9, atol=1e-12)
+    base, pos, frc, flag = chd.phys.sample_columns(n_ee, n_ee)
+    np.testing.assert_allclose(r.base_pos, -sample[:, base[[0, 2, 1]]], rtol=1e-9, atol=1e-12)
     for e in range(n_ee):
-        np.testing.assert_allclose(r.feet_pos[:, e], -sample[:, 6 + 3 * e:9 + 3 * e][:, [0, 2, 1]], rtol=1e-9, atol=1e-12)
-        np.testing.assert_allclose(r.feet_force[:, e], -sample[:, 6 + 3 * n_ee + 3 * e:9 + 3 * n_ee + 3 * e][:, [0, 2, 1]], rtol=1e-9, atol=1e-9)
-    np.testing.assert_array_equal(r.feet_contact, sample[:, 6 + 6 * n_ee:].astype(int))
+        np.testing.assert_allclose(r.feet_pos[:, e], -sample[:, pos[3 * e:3 * e + 3]][:, [0, 2, 1]], rtol=1e-9, atol=1e-12)
+        np.testing.assert_allclose(r.feet_force[:, e], -sample[:, frc[3 * e:3 * e + 3]][:, [0, 2, 1]], rtol=1e-9, atol=1e-9)
+    np.testing.assert_array_equal(r.feet_contact, sample[:, flag].astype(int))
     C = chd.prepare.C_BVH_TO_TOWR
-    R = chd.results.rot_zyx(np.radians(np.array([[float("%.10g" % v) for v in row] for row in sample[:, 3:6]])))
+    R = chd.results.rot_zyx(np.radians(np.array([[float("%.10g" % v) for v in row] for row in sample[:, base[3:]]])))
     np.testing.assert_allclose(r.base_R, C @ R @ C.T, atol=1e-12)
     np.testing.assert_allclose(chd.results.rot_zyx(r.base_rot), r.base_R, atol=1e-9)      # base_rot are the Euler angles of base_R
 
