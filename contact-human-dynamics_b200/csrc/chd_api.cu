@@ -4,6 +4,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <numeric>
 #include <vector>
 
 #include "../../include/chd.h"
@@ -31,6 +32,7 @@ __global__ void chd_k_linesearch(ChdDev D);
 __global__ void chd_k_sample(ChdDev D, double* out, int* frames_out);
 __global__ void chd_k_snapshot(ChdDev D, int* frames_out);
 __global__ void chd_k_sched_reset(ChdDev D);
+__global__ void chd_k_admit(ChdDev D, ChdAdmit A);   // chd_queue.cu
 
 #define CHD_CUDA(x)                                                                          \
   do {                                                                                       \
@@ -41,7 +43,7 @@ __global__ void chd_k_sched_reset(ChdDev D);
     }                                                                                        \
   } while (0)
 
-enum { KT_EVAL = 0, KT_KKT = 1, KT_LS = 2, KT_INIT = 3, KT_SAMPLE = 4, KT_N = 8 };
+enum { KT_EVAL = 0, KT_KKT = 1, KT_LS = 2, KT_INIT = 3, KT_SAMPLE = 4, KT_ADMIT = 5, KT_N = 8 };
 
 // Form of the evaluation and line-search kernels for a batch: with the iterate (and the gradient) in shared memory
 // when twice the longest sequence's iterate fits the opt-in limit, otherwise with both in global memory (D.x / D.grad /
@@ -58,6 +60,23 @@ static ChdIterForm chd_iter_form(int n_max, int smem_optin) {
             (size_t)n_max * sizeof(double) + red};
   return {chd_k_eval<true>, chd_k_linesearch<true>, red, red};
 }
+
+// Queue of clips solved through the slots of a batch (chd_phys_queue_create): the layout rows of every clip packed
+// into one record per clip, the admission kernel's segment table and the state of the running solve.
+struct ChdQueue {
+  int n = 0;                          // clips
+  size_t rec_bytes = 0;               // bytes of one record (every row starts 16-byte aligned)
+  char* store = nullptr;              // n records, page-locked (host-only handles: pageable)
+  char* d_stage = nullptr;            // device staging area, one record per slot
+  int *h_slot = nullptr, *d_slot = nullptr;   // slots being refilled (page-locked / device)
+  ChdAdmit adm = {};
+  int admit_blocks = 1;               // CTAs per admitted slot
+  std::vector<int> clip;              // clip held by every slot, -1: none (harvested)
+  int next = 0;                       // first clip not admitted yet
+  // outputs of the running chd_phys_queue_solve, indexed by clip
+  double *samples = nullptr, *stage_stats = nullptr;
+  int32_t *frames = nullptr, *success = nullptr, *stage_status = nullptr, *stage_iters = nullptr;
+};
 
 struct chd_phys_batch {
   ChdHostBatch hb;
@@ -85,6 +104,7 @@ struct chd_phys_batch {
   // pristine copies of the tables stage 3 rewrites (chd_phys_reset)
   double *poly_T0 = nullptr, *poly_tend0 = nullptr, *phase_tend0 = nullptr;
   int* ent_col0 = nullptr;
+  ChdQueue* queue = nullptr;   // a queue handle: the batch's sequences are slots that clips pass through
 };
 
 namespace {
@@ -162,11 +182,15 @@ int set_schedule(chd_phys_batch* b, const int* sched, int nsched, int override_s
   return 0;
 }
 
-// runs the uploaded schedule to completion: every sequence walks through its stages at its own pace
+int queue_refill(chd_phys_batch* b, int it, int* last_it);
+
+// runs the uploaded schedule to completion: every sequence walks through its stages at its own pace (a queue refills
+// the slots whose clip has finished at the check points, and the loop runs until the last admitted clip finishes)
 int run_schedule(chd_phys_batch* b) {
   const int B = b->hb.B;
   const int check_every = 8;
-  for (int it = 0; it <= b->sched_max_iter; ++it) {
+  int last_it = b->sched_max_iter;
+  for (int it = 0; it <= last_it; ++it) {
     {
       Timer t(b, KT_INIT);
       chd_k_stage_begin<<<B, CHD_THREADS, 0, b->stream>>>(b->D);
@@ -221,6 +245,10 @@ int run_schedule(chd_phys_batch* b) {
     if ((it % check_every) == check_every - 1) {
       CHD_CUDA(cudaMemcpyAsync(b->h_ipm, b->D.ipm, B * sizeof(ChdIpm), cudaMemcpyDeviceToHost, b->stream));
       CHD_CUDA(cudaStreamSynchronize(b->stream));
+      if (b->queue) {
+        const int rc = queue_refill(b, it, &last_it);
+        if (rc) return rc;
+      }
       bool any = false;
       for (int i = 0; i < B; ++i) any |= (b->h_ipm[i].phase != CHD_PH_FINISHED);
       if (!any) break;
@@ -230,6 +258,161 @@ int run_schedule(chd_phys_batch* b) {
   CHD_CUDA(cudaStreamSynchronize(b->stream));
   CHD_CUDA(cudaStreamSynchronize(b->copy_stream));
   CHD_CUDA(cudaGetLastError());
+  return 0;
+}
+
+size_t align16(size_t v) { return (v + 15) & ~(size_t)15; }
+
+// Every host layout table with one row per sequence, with the device arrays a clip's row goes to when it is admitted
+// to a slot: the read-only tables; the iterate; the tables stage 3 rewrites with their pristine and trial copies.
+template <class F>
+void queue_tables(chd_phys_batch* b, F&& f) {
+  ChdHostBatch& hb = b->hb;
+  ChdDev& D = b->D;
+  f(hb.seq, D.seq), f(hb.sets, D.sets), f(hb.node_var, D.node_var), f(hb.itab, D.itab), f(hb.ent_ptr, D.ent_ptr);
+  f(hb.ent_col, D.ent_col, b->ent_col0), f(hb.ent_row, D.ent_row), f(hb.col_ptr, D.col_ptr), f(hb.col_ent, D.col_ent);
+  f(hb.var_kkt, D.var_kkt), f(hb.row_kkt, D.row_kkt), f(hb.row_set, D.row_set), f(hb.poly_ph, D.poly_ph);
+  f(hb.node_const, D.node_const), f(hb.par, D.par), f(hb.t_dyn, D.t_dyn), f(hb.t_rom, D.t_rom), f(hb.t_data, D.t_data);
+  f(hb.row_lo, D.row_lo), f(hb.row_hi, D.row_hi), f(hb.dur0, D.dur0), f(hb.x0, D.x, b->d_x0);
+  f(hb.poly_T, D.poly_T, b->poly_T0, D.poly_Tt), f(hb.poly_tend, D.poly_tend, b->poly_tend0, D.poly_tendt);
+  f(hb.phase_tend, D.phase_tend, b->phase_tend0);
+}
+
+// Packs the layout of all hb.B clips into one record per clip and keeps the first `slots` rows of every table as the
+// batch's own layout (the strides stay those of all clips).
+int queue_pack(chd_phys_batch* b, int slots) {
+  ChdQueue& q = *(b->queue = new ChdQueue());
+  const size_t n = b->hb.B;
+  q.n = (int)n;
+  queue_tables(b, [&](auto& v, const void*, const void* = nullptr, const void* = nullptr) {
+    q.rec_bytes = align16(q.rec_bytes) + v.size() / n * sizeof(v[0]);
+  });
+  q.rec_bytes = align16(q.rec_bytes);
+  if (b->host_only) q.store = (char*)std::malloc(n * q.rec_bytes);
+  else CHD_CUDA(cudaMallocHost((void**)&q.store, n * q.rec_bytes));
+  if (!q.store) return -3;
+  std::memset(q.store, 0, n * q.rec_bytes);
+  size_t off = 0;
+  queue_tables(b, [&](auto& v, const void*, const void* = nullptr, const void* = nullptr) {
+    const size_t row = v.size() / n * sizeof(v[0]);
+    off = align16(off);
+    for (size_t i = 0; i < n; ++i) std::memcpy(q.store + i * q.rec_bytes + off, (const char*)v.data() + i * row, row);
+    v.resize(v.size() / n * slots);
+    off += row;
+  });
+  b->hb.B = slots;
+  return 0;
+}
+
+// Segment table of the admission kernel over the batch's device arrays, staging area, slot list.
+int queue_device(chd_phys_batch* b, int sms) {
+  ChdQueue& q = *b->queue;
+  const ChdHostBatch& hb = b->hb;
+  const ChdDev& D = b->D;
+  const size_t S = hb.B;
+  ChdAdmit& A = q.adm;
+  A.rec_bytes = q.rec_bytes;
+  size_t off = 0, slot_bytes = 0;
+  bool ok = true;
+  auto seg = [&](const void* dst, size_t row, long long src) {
+    if (A.nseg == CHD_ADMIT_SEGS) ok = false;
+    else A.seg[A.nseg++] = {(char*)dst, row, row, src}, slot_bytes += row;
+  };
+  queue_tables(b, [&](auto& v, const void* d0, const void* d1 = nullptr, const void* d2 = nullptr) {
+    const size_t row = v.size() / S * sizeof(v[0]);
+    off = align16(off);
+    for (const void* d : {d0, d1, d2})
+      if (d) seg(d, row, (long long)off);
+    off += row;
+  });
+  // zero fills: what dev_alloc zeroes at batch creation
+  const size_t nb = hb.n_max * sizeof(double), mb = hb.m_max * sizeof(double), kb = (size_t)(hb.Na_max + hb.nb_max) * sizeof(double);
+  for (const void* p : {(const void*)D.xt, (const void*)D.jty, (const void*)D.dx, (const void*)D.grad}) seg(p, nb, -1);
+  seg(D.unobs, hb.n_max, -1);
+  for (const double* p : {D.g, D.gt, D.sc, D.dL, D.dU, D.s, D.y, D.zL, D.zU, D.ds, D.dy, D.dzL, D.dzU}) seg(p, mb, -1);
+  seg(D.rflag, hb.m_max * sizeof(int), -1);
+  seg(D.Jv, hb.slots_max * sizeof(double), -1);
+  seg(D.cost, 2 * sizeof(double), -1);
+  seg(D.Kwork, D.kstride * sizeof(double), -1);
+  seg(D.Kbase, D.kstride * sizeof(double), -1);
+  for (const double* p : {D.sol, D.rhs0, D.rhs1}) seg(p, kb, -1);
+  if (D.scratch) seg(D.scratch, D.scratch_stride * sizeof(double), -1);
+  seg(b->d_frames, sizeof(int), -1);
+  const size_t snap = (size_t)hb.fo_max * (6 + 7 * (size_t)hb.n_ee_max) * sizeof(double);
+  for (int s = 0; s < 3; ++s) {
+    // the three SaveSolution snapshots are 3 x B x fo_max x stride: one row per slot in each
+    if (A.nseg == CHD_ADMIT_SEGS) ok = false;
+    else A.seg[A.nseg++] = {(char*)D.snapshots + s * S * snap, snap, snap, -1}, slot_bytes += snap;
+  }
+  if (!ok) {
+    fprintf(stderr, "libchd: more than %d admission segments\n", CHD_ADMIT_SEGS);
+    return -3;
+  }
+  // enough CTAs per slot that a single admitted slot spreads over the GPU, about 64 KB each
+  q.admit_blocks = (int)std::min<size_t>(4 * (size_t)sms, std::max<size_t>(1, slot_bytes / 65536));
+  CHD_CUDA(cudaMallocAsync((void**)&q.d_stage, S * q.rec_bytes, b->stream));
+  b->allocs.push_back(q.d_stage);
+  CHD_CUDA(cudaMallocAsync((void**)&q.d_slot, S * sizeof(int), b->stream));
+  b->allocs.push_back(q.d_slot);
+  CHD_CUDA(cudaMallocHost((void**)&q.h_slot, S * sizeof(int)));
+  q.clip.assign(S, -1);
+  return 0;
+}
+
+// admits the next k clips of the queue into `slots` (in that order): one upload of their records, one launch
+int queue_admit(chd_phys_batch* b, const int* slots, int k) {
+  ChdQueue& q = *b->queue;
+  for (int j = 0; j < k; ++j) q.h_slot[j] = slots[j], q.clip[slots[j]] = q.next + j;
+  Timer t(b, KT_ADMIT);
+  CHD_CUDA(cudaMemcpyAsync(q.d_stage, q.store + (size_t)q.next * q.rec_bytes, k * q.rec_bytes, cudaMemcpyHostToDevice, b->stream));
+  CHD_CUDA(cudaMemcpyAsync(q.d_slot, q.h_slot, k * sizeof(int), cudaMemcpyHostToDevice, b->stream));
+  b->h2d_bytes += (int64_t)(k * (q.rec_bytes + sizeof(int)));
+  q.adm.rec = q.d_stage, q.adm.slot = q.d_slot;
+  chd_k_admit<<<dim3(q.admit_blocks, k), 256, 0, b->stream>>>(b->D, q.adm);
+  q.next += k;
+  return 0;
+}
+
+// outputs of the clip in `slot` (its schedule is over, or the loop's bound was reached) into the clip's place
+int queue_harvest(chd_phys_batch* b, int slot) {
+  ChdQueue& q = *b->queue;
+  const int c = q.clip[slot];
+  if (c < 0) return 0;
+  const ChdHostBatch& hb = b->hb;
+  const size_t S = hb.B, n = q.n, row = (size_t)hb.fo_max * (6 + 7 * (size_t)hb.n_ee_max);
+  if (q.samples)
+    for (size_t s = 0; s < 3; ++s)
+      CHD_CUDA(cudaMemcpyAsync(q.samples + (s * n + c) * row, b->D.snapshots + (s * S + slot) * row, row * sizeof(double),
+                               cudaMemcpyDeviceToHost, b->stream));
+  if (q.frames) CHD_CUDA(cudaMemcpyAsync(q.frames + c, b->d_frames + slot, sizeof(int), cudaMemcpyDeviceToHost, b->stream));
+  const ChdIpm& I = b->h_ipm[slot];
+  if (q.success) q.success[2 * c] = I.st_status[CHD_STAGE_22] == 0, q.success[2 * c + 1] = I.st_status[CHD_STAGE_3] == 0 || I.st_status[CHD_STAGE_4] == 0;
+  for (size_t s = 0; s < 6; ++s) {
+    if (q.stage_status) q.stage_status[s * n + c] = I.st_status[s];
+    if (q.stage_iters) q.stage_iters[s * n + c] = I.st_iters[s];
+    if (q.stage_stats)
+      for (int k = 0; k < 4; ++k) q.stage_stats[(s * n + c) * 4 + k] = I.st_stat[s][k];
+  }
+  q.clip[slot] = -1;
+  return 0;
+}
+
+// At a check point of run_schedule (h_ipm just copied): while clips are pending, the slots whose clip has finished are
+// harvested and refilled with the next clips, in slot order.
+int queue_refill(chd_phys_batch* b, int it, int* last_it) {
+  ChdQueue& q = *b->queue;
+  std::vector<int> freed;
+  for (int i = 0; i < b->hb.B && (int)freed.size() < q.n - q.next; ++i)
+    if (b->h_ipm[i].phase == CHD_PH_FINISHED) freed.push_back(i);
+  if (freed.empty()) return 0;
+  // this iteration's side-stream kernels (chd_k_kcopy, chd_k_curv, chd_k_hess_dur) may still read the slots' state
+  CHD_CUDA(cudaStreamWaitEvent(b->stream, b->ev_copy, 0));
+  int rc;
+  for (int s : freed)
+    if ((rc = queue_harvest(b, s))) return rc;
+  if ((rc = queue_admit(b, freed.data(), (int)freed.size()))) return rc;
+  for (int s : freed) b->h_ipm[s].phase = CHD_PH_BEGIN;   // as the admission kernel left it
+  *last_it = std::max(*last_it, it + 1 + b->sched_max_iter);
   return 0;
 }
 
@@ -269,18 +452,18 @@ int chd_measure_fp64_peak(double* dfma_gflops, double* dmma_gflops) {
   return 0;
 }
 
-static int batch_create_impl(const chd_phys_problem* problems, int32_t batch, const chd_phys_weights* weights, int32_t device,
-                             const chd_phys_options& opt, chd_phys_batch* b);
+static int batch_create_impl(const chd_phys_problem* problems, int32_t batch, int32_t slots, const chd_phys_weights* weights,
+                             int32_t device, const chd_phys_options& opt, chd_phys_batch* b);
 
-int chd_phys_batch_create(const chd_phys_problem* problems, int32_t batch, const chd_phys_weights* weights, int32_t device,
-                          const chd_phys_options* opt, chd_phys_batch** out) {
-  if (!problems || batch <= 0 || !out) return -1;
+// a batch (slots = 0) or a queue of `batch` clips through `slots` slots
+static int create(const chd_phys_problem* problems, int32_t batch, int32_t slots, const chd_phys_weights* weights,
+                  int32_t device, const chd_phys_options* opt, chd_phys_batch** out) {
   chd_phys_options o = {-1};
   if (opt) o = *opt;
   if (o.stage3_band_above < -1 || o.stage3_band_above > CHD_MAX_DUR) return -1;
   chd_phys_batch* b = new chd_phys_batch();
   std::memset(&b->D, 0, sizeof(b->D));
-  const int rc = batch_create_impl(problems, batch, weights, device, o, b);
+  const int rc = batch_create_impl(problems, batch, slots, weights, device, o, b);
   if (rc) {
     chd_phys_batch_destroy(b);   // single cleanup path: streams, events, pooled allocations, host buffers
     return rc;
@@ -289,8 +472,20 @@ int chd_phys_batch_create(const chd_phys_problem* problems, int32_t batch, const
   return 0;
 }
 
-static int batch_create_impl(const chd_phys_problem* problems, int32_t batch, const chd_phys_weights* weights, int32_t device,
-                             const chd_phys_options& opt, chd_phys_batch* b) {
+int chd_phys_batch_create(const chd_phys_problem* problems, int32_t batch, const chd_phys_weights* weights, int32_t device,
+                          const chd_phys_options* opt, chd_phys_batch** out) {
+  if (!problems || batch <= 0 || !out) return -1;
+  return create(problems, batch, 0, weights, device, opt, out);
+}
+
+int chd_phys_queue_create(const chd_phys_problem* problems, int32_t n, int32_t slots, const chd_phys_weights* weights,
+                          int32_t device, const chd_phys_options* opt, chd_phys_batch** out) {
+  if (!problems || n <= 0 || slots <= 0 || !out) return -1;
+  return create(problems, n, std::min(slots, n), weights, device, opt, out);
+}
+
+static int batch_create_impl(const chd_phys_problem* problems, int32_t batch, int32_t slots, const chd_phys_weights* weights,
+                             int32_t device, const chd_phys_options& opt, chd_phys_batch* b) {
   const bool host_only = device == -2;  // layout tables only, no CUDA call (CPU-side tests of the host logic)
   if (device >= 0) CHD_CUDA(cudaSetDevice(device));
   chd_phys_weights w = {0.4, 1.7, 0.3, 0.1, 0.1};  // phys_optim.cpp:27-31
@@ -301,6 +496,8 @@ static int batch_create_impl(const chd_phys_problem* problems, int32_t batch, co
   ChdDev& D = b->D;
   std::memset(&D, 0, sizeof(D));
   b->host_only = host_only;
+  // a queue: the layout of all clips goes into the record store, the batch keeps `slots` rows of it
+  if (slots && (rc = queue_pack(b, slots))) return rc;
   if (host_only) return 0;
   D.B = hb.B, D.S = hb.S, D.Pmax = hb.Pmax, D.n_max = hb.n_max, D.m_max = hb.m_max, D.slots_max = hb.slots_max;
   D.sets_max = hb.sets_max, D.tab_max = hb.tab_max, D.F_max = hb.F_max, D.Kd_max = hb.Kd_max, D.Kr_max = hb.Kr_max;
@@ -384,6 +581,7 @@ static int batch_create_impl(const chd_phys_problem* problems, int32_t batch, co
   CHD_CUDA(cudaMallocAsync((void**)&b->d_stages, 6 * sizeof(ChdStageDev), b->stream));
   b->allocs.push_back(b->d_stages);
   if ((rc = dev_alloc(b, 3 * B * hb.fo_max * stride, &D.snapshots))) return rc;
+  if (b->queue && (rc = queue_device(b, sms))) return rc;
   CHD_CUDA(cudaStreamSynchronize(b->stream));
   return 0;
 }
@@ -395,6 +593,11 @@ void chd_phys_batch_destroy(chd_phys_batch* b) {
     cudaStreamSynchronize(b->stream);
   }
   std::free(b->h_ipm);
+  if (b->queue) {
+    if (b->host_only) std::free(b->queue->store);
+    else cudaFreeHost(b->queue->store), cudaFreeHost(b->queue->h_slot);
+    delete b->queue;
+  }
   if (b->ev0) cudaEventDestroy(b->ev0);
   if (b->ev1) cudaEventDestroy(b->ev1);
   if (b->ev_kkt) cudaEventDestroy(b->ev_kkt);
@@ -427,7 +630,7 @@ int chd_phys_get_sizes_fixed(const chd_phys_batch* b, int32_t* s) {
   return 0;
 }
 int chd_phys_get_x(const chd_phys_batch* b, double* x) {
-  if (!b || !x) return -1;
+  if (!b || !x || b->queue) return -1;
   if (b->host_only) {
     std::memcpy(x, b->hb.x0.data(), b->hb.x0.size() * sizeof(double));
     return 0;
@@ -437,7 +640,7 @@ int chd_phys_get_x(const chd_phys_batch* b, double* x) {
   return 0;
 }
 int chd_phys_set_x(chd_phys_batch* b, const double* x) {
-  if (!b || !x || b->host_only) return -1;
+  if (!b || !x || b->host_only || b->queue) return -1;
   CHD_CUDA(cudaMemcpy(b->D.x, x, (size_t)b->hb.B * b->hb.n_max * sizeof(double), cudaMemcpyHostToDevice));
   chd_k_tables<<<b->hb.B, 64, 0, b->stream>>>(b->D);   // spline tables follow the durations held in x
   b->launches++;
@@ -446,7 +649,7 @@ int chd_phys_set_x(chd_phys_batch* b, const double* x) {
 }
 
 int chd_phys_eval(chd_phys_batch* b, int32_t stage, double* cost, double* grad, double* g, double* jac_vals) {
-  if (!b || stage < 0 || stage > 5 || b->host_only) return -1;
+  if (!b || stage < 0 || stage > 5 || b->host_only || b->queue) return -1;
   const ChdHostBatch& hb = b->hb;
   int sched[1] = {stage};
   int rc = set_schedule(b, sched, 1, -1, 0);
@@ -505,7 +708,7 @@ int chd_phys_get_ent_col(const chd_phys_batch* b, int32_t* ent_col) {
 }
 
 int chd_phys_get_duals(const chd_phys_batch* b, double* y, double* zL, double* zU, double* s, double* row_scale, double* obj_scale) {
-  if (!b || b->host_only) return -1;
+  if (!b || b->host_only || b->queue) return -1;
   const size_t B = b->hb.B, mm = B * b->hb.m_max;
   CHD_CUDA(cudaStreamSynchronize(b->stream));
   if (y) CHD_CUDA(cudaMemcpy(y, b->D.y, mm * sizeof(double), cudaMemcpyDeviceToHost));
@@ -531,7 +734,7 @@ int chd_phys_stage_stats(const chd_phys_batch* b, double* stats) {
 }
 
 int chd_phys_solve_stage(chd_phys_batch* b, int32_t stage, int32_t max_iter, int32_t* status, int32_t* iters, double* stats) {
-  if (!b || stage < 0 || stage > 5 || b->host_only) return -1;
+  if (!b || stage < 0 || stage > 5 || b->host_only || b->queue) return -1;
   const int B = b->hb.B;
   int sched[1] = {stage};
   int rc = set_schedule(b, sched, 1, stage, max_iter);
@@ -551,7 +754,7 @@ int chd_phys_solve_stage(chd_phys_batch* b, int32_t stage, int32_t max_iter, int
 }
 
 int chd_phys_sample_device(chd_phys_batch* b, double* out_device, void* stream) {
-  if (!b || !out_device || b->host_only) return -1;
+  if (!b || !out_device || b->host_only || b->queue) return -1;
   cudaStream_t st = stream ? (cudaStream_t)stream : b->stream;
   if (st == b->stream) {
     Timer t(b, KT_SAMPLE);
@@ -572,7 +775,7 @@ int chd_phys_sample_device(chd_phys_batch* b, double* out_device, void* stream) 
 }
 
 int chd_phys_sample(chd_phys_batch* b, double* out, int32_t* frames_out) {
-  if (!b || !out || b->host_only) return -1;
+  if (!b || !out || b->host_only || b->queue) return -1;
   const ChdHostBatch& hb = b->hb;
   const size_t stride = 6 + 7 * (size_t)hb.n_ee_max, cnt = (size_t)hb.B * hb.fo_max * stride;
   CHD_CUDA(cudaMemsetAsync(b->d_samples, 0, cnt * sizeof(double), b->stream));
@@ -590,7 +793,7 @@ int chd_phys_sample(chd_phys_batch* b, double* out, int32_t* frames_out) {
 // (more phase durations than CHD_MAX_DUR with the switch times in the border, or a banded layout too wide).
 int chd_phys_solve(chd_phys_batch* b, double* samples, int32_t* frames_out, int32_t* success, int32_t* stage_status,
                    int32_t* stage_iters) {
-  if (!b || b->host_only) return -1;
+  if (!b || b->host_only || b->queue) return -1;
   const ChdHostBatch& hb = b->hb;
   const int B = hb.B;
   const size_t stride = 6 + 7 * (size_t)hb.n_ee_max, snap = (size_t)B * hb.fo_max * stride;
@@ -614,10 +817,34 @@ int chd_phys_solve(chd_phys_batch* b, double* samples, int32_t* frames_out, int3
   return 0;
 }
 
+// Queue of n clips through the batch's slots: every clip is admitted in queue order into the first free slot, and a
+// slot is refilled at the check point after its clip finished.  Outputs as chd_phys_solve's, indexed by clip.
+int chd_phys_queue_solve(chd_phys_batch* b, double* samples, int32_t* frames_out, int32_t* success, int32_t* stage_status,
+                         int32_t* stage_iters, double* stage_stats) {
+  if (!b || b->host_only || !b->queue) return -1;
+  ChdQueue& q = *b->queue;
+  const int S = b->hb.B;
+  int sched[6] = {CHD_STAGE_11, CHD_STAGE_12, CHD_STAGE_21, CHD_STAGE_22, CHD_STAGE_3, CHD_STAGE_4};
+  int rc = set_schedule(b, sched, 6, -1, 0);
+  if (rc) return rc;
+  q.samples = samples, q.frames = frames_out, q.success = success, q.stage_status = stage_status;
+  q.stage_iters = stage_iters, q.stage_stats = stage_stats;
+  q.next = 0;
+  q.clip.assign(S, -1);
+  std::vector<int> slots(S);
+  std::iota(slots.begin(), slots.end(), 0);
+  if ((rc = queue_admit(b, slots.data(), S))) return rc;
+  if ((rc = run_schedule(b))) return rc;
+  for (int i = 0; i < S; ++i)
+    if ((rc = queue_harvest(b, i))) return rc;
+  CHD_CUDA(cudaStreamSynchronize(b->stream));
+  return 0;
+}
+
 int64_t chd_phys_launch_count(const chd_phys_batch* b) { return b ? b->launches : 0; }
 int64_t chd_phys_h2d_bytes(const chd_phys_batch* b) { return b ? b->h2d_bytes : 0; }
 int chd_phys_reset(chd_phys_batch* b) {
-  if (!b || b->host_only) return -1;
+  if (!b || b->host_only || b->queue) return -1;
   CHD_CUDA(cudaMemcpyAsync(b->D.x, b->d_x0, (size_t)b->hb.B * b->hb.n_max * sizeof(double), cudaMemcpyDeviceToDevice, b->stream));
   // the input durations are back: host-built spline tables and Jacobian columns
   const ChdHostBatch& hb = b->hb;

@@ -94,6 +94,23 @@ struct ChdDev {
   double* snapshots;                          // 3 x B x fo_max x (6 + 7 n_ee_max)
 };
 
+// Admission of queued clips into freed slots (chd_k_admit, chd_queue.cu).  A segment is one per-sequence row of a
+// device array: the admitted slot's row is copied from the clip's staged record, or zeroed (src < 0).
+#define CHD_ADMIT_SEGS 64
+struct ChdAdmitSeg {
+  char* dst;             // row of slot 0
+  size_t slot_bytes;     // distance between the rows of two slots
+  size_t bytes;          // bytes of one row
+  long long src;         // offset of the row in a clip record; -1: zero fill
+};
+struct ChdAdmit {
+  const char* rec;       // staged records, rec_bytes apart: record j goes to slot slot[j]
+  size_t rec_bytes;
+  const int* slot;
+  int nseg;
+  ChdAdmitSeg seg[CHD_ADMIT_SEGS];
+};
+
 // IPM constants (Opts of oracle/ipm_oracle.cpp; IPOPT defaults unless noted)
 #define CHD_TOL 1e-3            /* phys_optim.cpp:578 */
 #define CHD_CONSTR_VIOL_TOL 1e-4
@@ -154,6 +171,12 @@ __device__ __forceinline__ double chd_row_res(int f, double d, const double& dL,
 __device__ __forceinline__ void chd_row_barrier(int f, double mu, ChdGaps gap, double& acc) {
   if (f & CHD_ROW_HASL) acc -= mu * log(gap.L);
   if (f & CHD_ROW_HASU) acc -= mu * log(gap.U);
+}
+
+// puts one sequence at the start of the schedule D.sched (chd_k_sched_reset, chd_k_admit)
+__device__ __forceinline__ void chd_sched_begin(const ChdDev& D, ChdIpm& I) {
+  I.pos = 0, I.stage = D.sched[0], I.phase = CHD_PH_BEGIN, I.snap = -1, I.step_ready = 0, I.kw_req = 0, I.status = 1;
+  for (int q = 0; q < 6; ++q) I.st_status[q] = -9, I.st_iters[q] = 0;
 }
 
 // a stage ended for this sequence: record its outcome, request the snapshot, move on in the schedule

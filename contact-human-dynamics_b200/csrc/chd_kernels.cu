@@ -453,7 +453,5 @@ __global__ void chd_k_clear_dyn(ChdDev D) {
 __global__ void chd_k_sched_reset(ChdDev D) {
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b >= D.B) return;
-  ChdIpm& I = D.ipm[b];
-  I.pos = 0, I.stage = D.sched[0], I.phase = CHD_PH_BEGIN, I.snap = -1, I.step_ready = 0, I.kw_req = 0, I.status = 1;
-  for (int q = 0; q < 6; ++q) I.st_status[q] = -9, I.st_iters[q] = 0;
+  chd_sched_begin(D, D.ipm[b]);
 }

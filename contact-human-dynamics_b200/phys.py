@@ -91,6 +91,9 @@ SIGNATURES = {
     "chd_phys_reset": (_int, [_vp]),
     "chd_phys_kernel_times": (_int, [_vp, _vp, _vp, _int]),
     "chd_phys_set_timing": (_int, [_vp, _int]),
+    "chd_phys_queue_create": (_int, [C.POINTER(_Problem), _i32, _i32, C.POINTER(_Weights), _i32, C.POINTER(_Options),
+                                     C.POINTER(_vp)]),
+    "chd_phys_queue_solve": (_int, [_vp] * 7),
     "chd_contact_create": (_int, [_vp, _vp, _vp, C.c_float, _i32, C.POINTER(_vp)]),
     "chd_contact_destroy": (None, [_vp]),
     "chd_contact_forward": (_int, [_vp, _vp, _i32, _i32, _vp, _vp, _vp, _vp]),
@@ -346,6 +349,85 @@ class PhysBatch:
     def _chk(self, rc):
         if rc != 0:
             raise RuntimeError("libchd call failed with code %d" % rc)
+
+
+class PhysQueue:
+    """Any number of clips solved through `slots` device slots: a slot takes the next clip as soon as its clip has
+    finished, so device memory scales with `slots` and the slowest clip's tail is paid once per queue rather than once
+    per batch.  The clips enter in descending `chd.parallel.work_estimate` order (the longest first, so that the queue's
+    final tail is short); `solve()` returns `PhysBatch.solve()`'s dict plus `stage_stats` (6, N, 4), in input order.
+    Each clip's results are those of a `PhysBatch` of the same clips (`stage3_band_above`: see `PhysBatch`)."""
+
+    def __init__(self, problems: Sequence[PhysProblem], slots: int, weights=(0.4, 1.7, 0.3, 0.1, 0.1), device: int = -1,
+                 stage3_band_above: Optional[int] = None):
+        from .parallel import work_estimate
+        self.L = load_lib()
+        self.problems = list(problems)
+        N = len(self.problems)
+        # queue position k holds problems[order[k]]; stable, so equal estimates keep their input order
+        self.order = np.argsort(-np.asarray(work_estimate(self.problems), dtype=np.float64), kind="stable")
+        arr, self._keep = make_problem_array([self.problems[i] for i in self.order])
+        w = _Weights(*[float(x) for x in weights])
+        opt = None if stage3_band_above is None else C.byref(_Options(int(stage3_band_above)))
+        h = C.c_void_p()
+        rc = self.L.chd_phys_queue_create(arr, N, int(slots), C.byref(w), device, opt, C.byref(h))
+        if rc != 0:
+            raise RuntimeError("chd_phys_queue_create failed with code %d" % rc)
+        self.h = h
+        d = _Dims()
+        self.L.chd_phys_get_dims(self.h, C.byref(d))
+        self.dims = {k: getattr(d, k) for k, _ in _Dims._fields_}
+        self.N, self.slots = N, self.dims["batch"]
+        self.n_ee_max = max(p.n_ee for p in self.problems)
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def close(self):
+        if getattr(self, "h", None):
+            self.L.chd_phys_batch_destroy(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def solve(self) -> dict:
+        """Full staged schedule of every clip; the same keys and shapes as `PhysBatch.solve()` for N sequences, plus
+        stage_stats (6, N, 4) (`PhysBatch.stage_stats`)."""
+        N, d = self.N, self.dims
+        out = dict(samples=np.zeros((3, N, d["frames_out_max"], sample_stride(self.n_ee_max))),
+                   frames=np.zeros(N, np.int32), success=np.zeros((N, 2), np.int32),
+                   stage_status=np.zeros((6, N), np.int32), stage_iters=np.zeros((6, N), np.int32),
+                   stage_stats=np.zeros((6, N, 4)))
+        rc = self.L.chd_phys_queue_solve(self.h, *[_ptr(out[k]) for k in ("samples", "frames", "success", "stage_status",
+                                                                          "stage_iters", "stage_stats")])
+        if rc != 0:
+            raise RuntimeError("libchd call failed with code %d" % rc)
+        inv = np.argsort(self.order)          # queue position of every input clip
+        axis = dict(samples=1, frames=0, success=0, stage_status=1, stage_iters=1, stage_stats=1)
+        return {k: np.take(v, inv, axis=axis[k]) for k, v in out.items()}
+
+    def launch_count(self) -> int:
+        return int(self.L.chd_phys_launch_count(self.h))
+
+    def h2d_bytes(self) -> int:
+        """Bytes uploaded so far: the slots' tables at creation and the records of every admitted clip."""
+        return int(self.L.chd_phys_h2d_bytes(self.h))
+
+    def set_timing(self, on: bool):
+        self.L.chd_phys_set_timing(self.h, int(on))
+
+    def kernel_times(self, reset=False):
+        ms, cnt = np.zeros(8), np.zeros(8, np.int64)
+        self.L.chd_phys_kernel_times(self.h, _ptr(ms), _ptr(cnt), int(reset))
+        names = ["eval", "kkt", "linesearch", "init", "sample", "admit"]
+        return {k: (float(ms[i]), int(cnt[i])) for i, k in enumerate(names)}
 
 
 SOLUTION_FILES = ("sol_out_no_dynamics.txt", "sol_out_dynamics.txt", "sol_out_durations.txt")

@@ -143,6 +143,23 @@ int chd_phys_sample(chd_phys_batch* b, double* out, int32_t* frames_out);
  * [device] buffer (e.g. an NCCL send buffer) on the given stream (cudaStream_t passed as void*). */
 int chd_phys_sample_device(chd_phys_batch* b, double* out_device, void* stream);
 
+/* Physics solve queue: n clips solved through `slots` sequences of one batch (slots is clamped to n).  The layout is
+ * built once over all n clips, so every clip fits every slot and chd_phys_get_dims reports the strides of a batch of
+ * the n clips with batch = slots: outputs are sized n x frames_out_max x stride.  Device memory scales with slots.
+ * Returns -1 for n <= 0, slots <= 0, problems or out NULL or an option out of range, -5 as chd_phys_batch_create.
+ * On a queue handle the calls that address slots (get_x, set_x, eval, solve_stage, solve, sample, sample_device,
+ * reset, get_duals) return -1; the layout queries describe the first `slots` clips; the instrumentation calls work,
+ * chd_phys_h2d_bytes includes the uploads of every admission and chd_phys_kernel_times' entry 5 times them. */
+int chd_phys_queue_create(const chd_phys_problem* problems, int32_t n, int32_t slots, const chd_phys_weights* weights,
+                          int32_t device, const chd_phys_options* opt, chd_phys_batch** out);
+/* The staged schedule of chd_phys_solve for every clip of the queue.  The first `slots` clips start in slots 0, 1, ...;
+ * whenever a slot's clip has finished (checked every 8 iterations) the next clip in queue order takes it, a refilled
+ * slot being the same to the solver as that row of a new batch.  Outputs [host] as chd_phys_solve's plus
+ * stage_stats (chd_phys_stage_stats' 6 x n x 4 block), indexed by clip (n, not slots); any may be NULL.  A clip's
+ * results are those of a chd_phys_batch_create batch of the same n clips.  Calling it again starts the queue over. */
+int chd_phys_queue_solve(chd_phys_batch* b, double* samples, int32_t* frames_out, int32_t* success, int32_t* stage_status,
+                         int32_t* stage_iters, double* stage_stats);
+
 /* Number of kernels launched by this batch so far. */
 int64_t chd_phys_launch_count(const chd_phys_batch* b);
 /* Bytes copied host -> device by chd_phys_batch_create (problem data + layout tables). */
@@ -151,7 +168,8 @@ int64_t chd_phys_h2d_bytes(const chd_phys_batch* b);
 int chd_phys_reset(chd_phys_batch* b);
 
 /* Per-kernel accumulated CUDA-event time (ms) and launch counts since the last reset:
- * names: 0 eval, 1 kkt (assemble+factor+solve), 2 linesearch, 3 init, 4 sample.  [host] arrays of 8. */
+ * names: 0 eval, 1 kkt (assemble+factor+solve), 2 linesearch, 3 init, 4 sample, 5 admission of a queue (upload +
+ * chd_k_admit).  [host] arrays of 8. */
 int chd_phys_kernel_times(chd_phys_batch* b, double* ms8, int64_t* launches8, int reset);
 int chd_phys_set_timing(chd_phys_batch* b, int enable);
 

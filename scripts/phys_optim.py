@@ -4,7 +4,8 @@
 output files, solved on the GPU.  `scripts/run_phys_mocap.py:159-174` can point its `--towr-phys-optim-path` here.
 
 Extension: `--in_dir` / `--out_dir` / `--nframes` accept comma separated lists so that many clips are solved as one
-batch (that is where the GPU pays off); `--n_ee 2` selects the toes-only parameterisation.
+batch (that is where the GPU pays off); `--n_ee 2` selects the toes-only parameterisation; `--slots S` solves the list
+through a queue of S device slots (`chd.phys.PhysQueue`: memory for S clips, each slot refilled as its clip finishes).
 """
 import argparse
 import os
@@ -29,7 +30,11 @@ def main(argv=None):
     ap.add_argument("--n_ee", type=int, default=4)
     ap.add_argument("--stage3_long", action="store_true",
                     help="run stage 3 on sequences with more than 96 phase durations too (switch times as band unknowns)")
+    ap.add_argument("--slots", type=int, default=0,
+                    help="solve the clips through a queue of this many device slots instead of one batch")
     args = ap.parse_args(argv)
+    if args.slots and int(os.environ.get("WORLD_SIZE", 1)) > 1:
+        ap.error("--slots solves on one GPU: it cannot be combined with WORLD_SIZE > 1")
     import chd
     in_dirs = args.in_dir.split(",")
     out_dirs = args.out_dir.split(",")
@@ -61,7 +66,10 @@ def main(argv=None):
                 chd.io_formats.write_solution(os.path.join(od, "sol_out_durations.txt"), p.dt, out["samples"][i, :nf][:, cols], n_ee)
                 chd.io_formats.write_success_log(os.path.join(od, "success_log.txt"), out["success"][i, 0], out["success"][i, 1])
         return
-    batch = chd.phys.PhysBatch(problems, weights=weights, stage3_band_above=band)
+    if args.slots:
+        batch = chd.phys.PhysQueue(problems, args.slots, weights=weights, stage3_band_above=band)
+    else:
+        batch = chd.phys.PhysBatch(problems, weights=weights, stage3_band_above=band)
     out = batch.solve()
     for i, (p, od) in enumerate(zip(problems, out_dirs)):
         chd.phys.write_outputs(out, i, p, od, batch.n_ee_max)
