@@ -73,6 +73,11 @@ struct ChdQueue {
   int admit_blocks = 1;               // CTAs per admitted slot
   std::vector<int> clip;              // clip held by every slot, -1: none (harvested)
   int next = 0;                       // first clip not admitted yet
+  // claim source (chd_phys_queue_set_claim), NULL: the queue's own order
+  chd_phys_claim_fn* claim = nullptr;
+  void* claim_ctx = nullptr;
+  bool exhausted = false;             // the source returned fewer positions than asked during this solve
+  std::vector<char> given;            // positions the source handed out during this solve
   // outputs of the running chd_phys_queue_solve, indexed by clip
   double *samples = nullptr, *stage_stats = nullptr;
   int32_t *frames = nullptr, *success = nullptr, *stage_status = nullptr, *stage_iters = nullptr;
@@ -359,17 +364,37 @@ int queue_device(chd_phys_batch* b, int sms) {
   return 0;
 }
 
-// admits the next k clips of the queue into `slots` (in that order): one upload of their records, one launch
-int queue_admit(chd_phys_batch* b, const int* slots, int k) {
+// admits the k clips at queue positions first, first + 1, ... into `slots` (in that order): one upload of their
+// records, one launch
+int queue_admit(chd_phys_batch* b, const int* slots, int k, int first) {
   ChdQueue& q = *b->queue;
-  for (int j = 0; j < k; ++j) q.h_slot[j] = slots[j], q.clip[slots[j]] = q.next + j;
+  for (int j = 0; j < k; ++j) q.h_slot[j] = slots[j], q.clip[slots[j]] = first + j;
   Timer t(b, KT_ADMIT);
-  CHD_CUDA(cudaMemcpyAsync(q.d_stage, q.store + (size_t)q.next * q.rec_bytes, k * q.rec_bytes, cudaMemcpyHostToDevice, b->stream));
+  CHD_CUDA(cudaMemcpyAsync(q.d_stage, q.store + (size_t)first * q.rec_bytes, k * q.rec_bytes, cudaMemcpyHostToDevice, b->stream));
   CHD_CUDA(cudaMemcpyAsync(q.d_slot, q.h_slot, k * sizeof(int), cudaMemcpyHostToDevice, b->stream));
   b->h2d_bytes += (int64_t)(k * (q.rec_bytes + sizeof(int)));
   q.adm.rec = q.d_stage, q.adm.slot = q.d_slot;
   chd_k_admit<<<dim3(q.admit_blocks, k), 256, 0, b->stream>>>(b->D, q.adm);
-  q.next += k;
+  return 0;
+}
+
+// asks the claim source for `want` positions: the k it hands out start at *first.  -1 if it fails, or hands out more
+// than asked, a range outside [0, n) or a position it already handed out in this solve; the work in flight is drained
+// first, so that nothing reaches the outputs after chd_phys_queue_solve has returned.
+int queue_claim(chd_phys_batch* b, int want, int* first, int* k) {
+  ChdQueue& q = *b->queue;
+  int32_t f = 0;
+  const int32_t got = q.claim(q.claim_ctx, want, &f);
+  bool ok = got >= 0 && got <= want && (got == 0 || (f >= 0 && f <= q.n - got));
+  for (int i = 0; ok && i < got; ++i) ok = !q.given[f + i];
+  if (!ok) {
+    cudaStreamSynchronize(b->stream);
+    cudaStreamSynchronize(b->copy_stream);
+    return -1;
+  }
+  for (int i = 0; i < got; ++i) q.given[f + i] = 1;
+  q.exhausted = got < want;
+  *first = f, *k = got;
   return 0;
 }
 
@@ -398,20 +423,26 @@ int queue_harvest(chd_phys_batch* b, int slot) {
 }
 
 // At a check point of run_schedule (h_ipm just copied): while clips are pending, the slots whose clip has finished are
-// harvested and refilled with the next clips, in slot order.
+// harvested and refilled with the next clips, in slot order.  With a claim source the next clips are the ones it hands
+// out, and once it has run dry the finished slots are left to the final harvest.
 int queue_refill(chd_phys_batch* b, int it, int* last_it) {
   ChdQueue& q = *b->queue;
+  if (q.exhausted) return 0;
+  const int pending = q.claim ? b->hb.B : q.n - q.next;
   std::vector<int> freed;
-  for (int i = 0; i < b->hb.B && (int)freed.size() < q.n - q.next; ++i)
+  for (int i = 0; i < b->hb.B && (int)freed.size() < pending; ++i)
     if (b->h_ipm[i].phase == CHD_PH_FINISHED) freed.push_back(i);
   if (freed.empty()) return 0;
+  int rc, first = q.next, k = (int)freed.size();
+  if (q.claim && (rc = queue_claim(b, k, &first, &k))) return rc;
   // this iteration's side-stream kernels (chd_k_kcopy, chd_k_curv, chd_k_hess_dur) may still read the slots' state
   CHD_CUDA(cudaStreamWaitEvent(b->stream, b->ev_copy, 0));
-  int rc;
   for (int s : freed)
     if ((rc = queue_harvest(b, s))) return rc;
-  if ((rc = queue_admit(b, freed.data(), (int)freed.size()))) return rc;
-  for (int s : freed) b->h_ipm[s].phase = CHD_PH_BEGIN;   // as the admission kernel left it
+  if (k == 0) return 0;
+  if ((rc = queue_admit(b, freed.data(), k, first))) return rc;
+  if (!q.claim) q.next += k;
+  for (int j = 0; j < k; ++j) b->h_ipm[freed[j]].phase = CHD_PH_BEGIN;   // as the admission kernel left it
   *last_it = std::max(*last_it, it + 1 + b->sched_max_iter);
   return 0;
 }
@@ -818,26 +849,47 @@ int chd_phys_solve(chd_phys_batch* b, double* samples, int32_t* frames_out, int3
 }
 
 // Queue of n clips through the batch's slots: every clip is admitted in queue order into the first free slot, and a
-// slot is refilled at the check point after its clip finished.  Outputs as chd_phys_solve's, indexed by clip.
+// slot is refilled at the check point after its clip finished.  Outputs as chd_phys_solve's, indexed by clip.  With a
+// claim source only the clips it hands out are admitted and written.
 int chd_phys_queue_solve(chd_phys_batch* b, double* samples, int32_t* frames_out, int32_t* success, int32_t* stage_status,
                          int32_t* stage_iters, double* stage_stats) {
   if (!b || b->host_only || !b->queue) return -1;
   ChdQueue& q = *b->queue;
   const int S = b->hb.B;
+  int rc, first = 0, k = S;
+  q.exhausted = false;
+  if (q.claim) {
+    q.given.assign(q.n, 0);
+    if ((rc = queue_claim(b, S, &first, &k))) return rc;
+    if (k == 0) return 0;   // nothing for this handle: no output is touched
+  }
   int sched[6] = {CHD_STAGE_11, CHD_STAGE_12, CHD_STAGE_21, CHD_STAGE_22, CHD_STAGE_3, CHD_STAGE_4};
-  int rc = set_schedule(b, sched, 6, -1, 0);
-  if (rc) return rc;
+  if ((rc = set_schedule(b, sched, 6, -1, 0))) return rc;
   q.samples = samples, q.frames = frames_out, q.success = success, q.stage_status = stage_status;
   q.stage_iters = stage_iters, q.stage_stats = stage_stats;
-  q.next = 0;
   q.clip.assign(S, -1);
   std::vector<int> slots(S);
   std::iota(slots.begin(), slots.end(), 0);
-  if ((rc = queue_admit(b, slots.data(), S))) return rc;
+  if ((rc = queue_admit(b, slots.data(), k, first))) return rc;
+  q.next = k;
+  if (k < S) {
+    // slots the claim source left empty: finished from the start, so every kernel passes over them
+    std::vector<ChdIpm> idle(S - k);
+    std::memset(idle.data(), 0, idle.size() * sizeof(ChdIpm));
+    for (ChdIpm& I : idle) I.phase = CHD_PH_FINISHED, I.snap = -1;
+    CHD_CUDA(cudaMemcpyAsync(b->D.ipm + k, idle.data(), idle.size() * sizeof(ChdIpm), cudaMemcpyHostToDevice, b->stream));
+    b->h2d_bytes += (int64_t)(idle.size() * sizeof(ChdIpm));
+  }
   if ((rc = run_schedule(b))) return rc;
   for (int i = 0; i < S; ++i)
     if ((rc = queue_harvest(b, i))) return rc;
   CHD_CUDA(cudaStreamSynchronize(b->stream));
+  return 0;
+}
+
+int chd_phys_queue_set_claim(chd_phys_batch* b, chd_phys_claim_fn* claim, void* ctx) {
+  if (!b || !b->queue) return -1;
+  b->queue->claim = claim, b->queue->claim_ctx = claim ? ctx : nullptr;
   return 0;
 }
 

@@ -6,6 +6,7 @@ Everything here is backend agnostic (`nccl` on the GPU box, `gloo` in the CPU te
 """
 from __future__ import annotations
 
+import itertools
 from typing import List, Sequence, Tuple
 
 import numpy as np
@@ -74,17 +75,118 @@ def frames_out(p) -> int:
     return int((T + 1e-5) / p.dt) + 1
 
 
+class StoreClaim:
+    """Claim source of a `PhysQueue` (its `claim`) shared by processes through a c10d store (`torch.distributed.Store`:
+    the process group's store under torchrun, or a `FileStore`).  A claim of `want` positions is one atomic
+    `store.add(key, want)`, which returns the new total t, and hands out [t - want, t) ∩ [0, n): every position of
+    [0, n) goes to exactly one claim of one process.  `restart()` moves to a fresh counter (the key's next generation) so
+    that a repeated solve starts over; every process must restart as often as the others."""
+
+    def __init__(self, store, key: str, n: int):
+        self.store, self.key, self.n, self.generation = store, key, int(n), 0
+
+    def restart(self):
+        self.generation += 1
+
+    def __call__(self, want: int) -> Tuple[int, int]:
+        t = int(self.store.add("%s/%d" % (self.key, self.generation), int(want)))
+        lo, hi = min(t - int(want), self.n), min(t, self.n)
+        return lo, hi - lo
+
+
+# Row of a rank's block in the merge of queue results (merge_solved): clip index, the three SaveSolution snapshots
+# (3 x fo x stride), then frames, success[2], stage_status[6], stage_iters[6], stage_stats[6 x 4].
+Q_EXTRA = 1 + 2 + 6 + 6 + 24
+
+
+def merge_solved(local: dict, world: int, group=None, tensor_device=None) -> dict:
+    """Merges the `PhysQueue.solve()` results of `world` ranks that each solved some of the same N clips (`solved`;
+    every rank's arrays have the same shapes) into every clip's result, by clip index.  The ranks' solved counts are
+    all-gathered, every rank's block of solved rows is padded to the largest count, and one `all_gather_into_tensor`
+    moves the blocks, each row carrying its clip index, the three snapshots and the status trailer.  Rows are copied,
+    never summed, so every bit of a result (a -0.0 too) arrives as its rank computed it.  Returns `PhysQueue.solve()`'s
+    keys over all N clips in input order, plus `solved_by` (N, the rank that solved each clip, -1: none) and
+    `d2h_bytes` (the gathered block).  `tensor_device`: where the collective's tensors live (cuda for nccl, the
+    default cpu for gloo)."""
+    import torch
+    import torch.distributed as dist
+    dev = tensor_device or torch.device("cpu")
+    _, N, fo, stride = local["samples"].shape
+    snap = 3 * fo * stride
+    width = 1 + snap + Q_EXTRA
+    mine = np.nonzero(local["solved"])[0]
+    n = len(mine)
+    collective = world > 1 and dist.is_initialized()
+    counts = torch.tensor([n], dtype=torch.int64, device=dev)
+    if collective:
+        counts = torch.empty(world, dtype=torch.int64, device=dev)
+        dist.all_gather_into_tensor(counts, torch.tensor([n], dtype=torch.int64, device=dev), group=group)
+    counts = counts.cpu().numpy()
+    cmax = int(counts.max())
+    blk = np.zeros((cmax, width))
+    blk[:n, 0] = mine
+    blk[:n, 1:1 + snap] = local["samples"][:, mine].transpose(1, 0, 2, 3).reshape(n, snap)
+    tr = blk[:n, 1 + snap:]
+    tr[:, 0] = local["frames"][mine]
+    tr[:, 1:3] = local["success"][mine]
+    tr[:, 3:9] = local["stage_status"][:, mine].T
+    tr[:, 9:15] = local["stage_iters"][:, mine].T
+    tr[:, 15:39] = local["stage_stats"][:, mine].transpose(1, 0, 2).reshape(n, 24)
+    g = blk
+    if collective and cmax > 0:
+        send = torch.from_numpy(blk).to(dev)
+        recv = torch.empty((world * cmax, width), dtype=torch.float64, device=dev)
+        dist.all_gather_into_tensor(recv, send, group=group)
+        g = recv.cpu().numpy()
+    rows = np.concatenate([g[r * cmax:r * cmax + int(counts[r])] for r in range(len(counts))])
+    rank_of = np.repeat(np.arange(len(counts)), counts)
+    idx = rows[:, 0].astype(np.int64)
+    if len(np.unique(idx)) != len(idx) or (len(idx) and (idx.min() < 0 or idx.max() >= N)):
+        raise RuntimeError("merge of queue results: a clip was solved by more than one rank, or a clip index is out of range")
+    tr = rows[:, 1 + snap:]
+    out = dict(samples=np.zeros((3, N, fo, stride)), frames=np.zeros(N, np.int32), success=np.zeros((N, 2), np.int32),
+               stage_status=np.zeros((6, N), np.int32), stage_iters=np.zeros((6, N), np.int32),
+               stage_stats=np.zeros((6, N, 4)), solved=np.zeros(N, bool), solved_by=np.full(N, -1, np.int32))
+    out["samples"][:, idx] = rows[:, 1:1 + snap].reshape(len(idx), 3, fo, stride).transpose(1, 0, 2, 3)
+    out["frames"][idx] = tr[:, 0]
+    out["success"][idx] = tr[:, 1:3]
+    out["stage_status"][:, idx] = tr[:, 3:9].T
+    out["stage_iters"][:, idx] = tr[:, 9:15].T
+    out["stage_stats"][:, idx] = tr[:, 15:39].reshape(len(idx), 6, 4).transpose(1, 0, 2)
+    out["solved"][idx] = True
+    out["solved_by"][idx] = rank_of
+    out["d2h_bytes"] = int(g.nbytes)
+    return out
+
+
+_QUEUE_KEYS = itertools.count()   # one counter key per queue-mode ShardedSolver, created in the same order on every rank
+
+
 class ShardedSolver:
     """One process per GPU (torchrun).  Every rank holds the same problem list, solves its shard on its device and
     takes part in a single all_gather of the fixed-size result block (final SaveSolution snapshot + status trailer).
 
     `solve_fn(problems) -> dict(final=(n, fo, stride) array, frames, success, stage_status (6,n), stage_iters (6,n))`
     replaces the CUDA solve in the CPU (gloo) tests; the default drives `PhysBatch` on `device` (`stage3_band_above`:
-    see `PhysBatch`)."""
+    see `PhysBatch`).
+
+    `slots`: instead of a static shard, every rank runs a `PhysQueue` of `slots` device slots over all N clips (so
+    every clip fits every slot on every rank and its result does not depend on the rank that solved it), and all
+    ranks claim their next clips from one counter (`StoreClaim`) in `store`, by default the process group's store.  A
+    rank that finishes early simply claims more.  `solve()` then merges the ranks' results by clip index
+    (`merge_solved`) and returns `PhysQueue.solve()`'s keys over all N clips, including all three snapshots, plus
+    `solved_by`.  Every rank keeps the page-locked record store of all N clips (about 106 MB per 256 clips of 120
+    frames, 2 feet), and every rank must call `solve()` as often as the others.  With `slots`, `solve_fn(problems)`
+    stands in for `PhysQueue.solve()` over all N problems and returns its dict, `solved` marking the clips this rank
+    solved."""
 
     def __init__(self, problems, weights=(0.4, 1.7, 0.3, 0.1, 0.1), device: int = 0, rank: int = 0, world: int = 1,
-                 group=None, solve_fn=None, tensor_device=None, stage3_band_above=None):
+                 group=None, solve_fn=None, tensor_device=None, stage3_band_above=None, slots=None, store=None):
         self.problems, self.rank, self.world, self.group = list(problems), rank, world, group
+        self.queue_slots, self.queue = slots, None
+        if slots is not None:
+            self._init_queue(weights, device, solve_fn, tensor_device, stage3_band_above, slots, store)
+            return
         self.shards = shard_by_work(work_estimate(self.problems), world)
         self.slots = pad_to(self.shards)
         self.mine = self.shards[rank]
@@ -104,10 +206,41 @@ class ShardedSolver:
         self.recv = torch.zeros((world * self.slots, self.width), dtype=torch.float64, device=self.tdev) if world > 1 else None
         self.last_ms = {}
 
+    def _init_queue(self, weights, device, solve_fn, tensor_device, stage3_band_above, slots, store):
+        import torch
+        self.solve_fn, self.batch, self.last_ms = solve_fn, None, {}
+        self.n_ee_max = max(p.n_ee for p in self.problems)
+        if solve_fn is None:
+            if store is None:
+                from torch.distributed import distributed_c10d
+                store = distributed_c10d._get_default_store()
+            self.claim = StoreClaim(store, "chd/phys_queue/%d" % next(_QUEUE_KEYS), len(self.problems))
+            self.queue = phys.PhysQueue(self.problems, slots, weights=weights, device=device,
+                                        stage3_band_above=stage3_band_above, claim=self.claim)
+            tensor_device = tensor_device or torch.device("cuda", device)
+        self.tdev = tensor_device or torch.device("cpu")
+
     def close(self):
         if self.batch is not None:
             self.batch.close()
             self.batch = None
+        if self.queue is not None:
+            self.queue.close()
+            self.queue = None
+
+    def _solve_queue(self) -> dict:
+        import time
+        t0 = time.perf_counter()
+        if self.solve_fn is not None:
+            local = self.solve_fn(self.problems)
+        else:
+            self.claim.restart()
+            local = self.queue.solve()
+        t1 = time.perf_counter()
+        out = merge_solved(local, self.world, self.group, self.tdev)
+        t2 = time.perf_counter()
+        self.last_ms = {"solve_ms": 1e3 * (t1 - t0), "gather_ms": 1e3 * (t2 - t1)}
+        return out
 
     def _solve_local(self, resident: bool):
         """fills self.send; returns the local status arrays"""
@@ -156,7 +289,10 @@ class ShardedSolver:
 
     def solve(self, resident: bool = False) -> dict:
         """Solves the shard (resident=True: device-side reset of an already uploaded batch) and gathers.  Every rank
-        returns the full result in the original sequence order."""
+        returns the full result in the original sequence order.  With `slots`: the queue solve and the merge of every
+        clip's results (resident does not apply: a queue always starts over)."""
+        if self.queue_slots is not None:
+            return self._solve_queue()
         import time
         import torch
         import torch.distributed as dist
@@ -184,9 +320,11 @@ class ShardedSolver:
 
 
 def solve_sharded(problems, weights=(0.4, 1.7, 0.3, 0.1, 0.1), device: int = 0, rank: int = 0, world: int = 1, group=None,
-                  solve_fn=None, tensor_device=None, stage3_band_above=None) -> dict:
-    """shard -> solve -> one gather -> unshard for a list of `PhysProblem`s (see ShardedSolver)."""
-    s = ShardedSolver(problems, weights, device, rank, world, group, solve_fn, tensor_device, stage3_band_above)
+                  solve_fn=None, tensor_device=None, stage3_band_above=None, slots=None, store=None) -> dict:
+    """shard -> solve -> one gather -> unshard for a list of `PhysProblem`s (see ShardedSolver; `slots`: a queue on
+    every rank, claimed from one shared counter, merged by clip index)."""
+    s = ShardedSolver(problems, weights, device, rank, world, group, solve_fn, tensor_device, stage3_band_above, slots,
+                      store)
     try:
         return s.solve()
     finally:

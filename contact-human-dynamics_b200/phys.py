@@ -65,6 +65,9 @@ class _Dims(C.Structure):
 
 _vp, _i32, _i64, _int, _f64 = C.c_void_p, C.c_int32, C.c_int64, C.c_int, C.c_double
 
+# chd_phys_claim_fn: (ctx, want, *first) -> k; passed to chd_phys_queue_set_claim as c_void_p (C.cast)
+CLAIM_FN = C.CFUNCTYPE(C.c_int32, C.c_void_p, C.c_int32, C.POINTER(C.c_int32))
+
 # Every function of include/chd.h, name -> (restype, argtypes); load_lib applies it.  Arrays, handles and streams are
 # passed as c_void_p.
 SIGNATURES = {
@@ -94,6 +97,7 @@ SIGNATURES = {
     "chd_phys_queue_create": (_int, [C.POINTER(_Problem), _i32, _i32, C.POINTER(_Weights), _i32, C.POINTER(_Options),
                                      C.POINTER(_vp)]),
     "chd_phys_queue_solve": (_int, [_vp] * 7),
+    "chd_phys_queue_set_claim": (_int, [_vp] * 3),
     "chd_contact_create": (_int, [_vp, _vp, _vp, C.c_float, _i32, C.POINTER(_vp)]),
     "chd_contact_destroy": (None, [_vp]),
     "chd_contact_forward": (_int, [_vp, _vp, _i32, _i32, _vp, _vp, _vp, _vp]),
@@ -355,11 +359,20 @@ class PhysQueue:
     """Any number of clips solved through `slots` device slots: a slot takes the next clip as soon as its clip has
     finished, so device memory scales with `slots` and the slowest clip's tail is paid once per queue rather than once
     per batch.  The clips enter in descending `chd.parallel.work_estimate` order (the longest first, so that the queue's
-    final tail is short); `solve()` returns `PhysBatch.solve()`'s dict plus `stage_stats` (6, N, 4), in input order.
-    Each clip's results are those of a `PhysBatch` of the same clips (`stage3_band_above`: see `PhysBatch`)."""
+    final tail is short); `solve()` returns `PhysBatch.solve()`'s dict plus `stage_stats` (6, N, 4) and `solved` (N),
+    in input order.  Each clip's results are those of a `PhysBatch` of the same clips (`stage3_band_above`: see
+    `PhysBatch`).
+
+    `claim`: a callable `want -> (first, k)` that decides which queue positions this queue solves
+    (`chd_phys_queue_set_claim`): it is asked for `slots` positions when a solve starts and for as many as there are
+    finished slots at every refill check point, and hands out the k consecutive positions first .. first + k - 1
+    (0 <= k <= want; fewer than asked: nothing is left).  Queue positions are the `work_estimate` order (`order`), which
+    is the same in every process that holds the same problem list, so processes that share one source
+    (`chd.parallel.StoreClaim`) split the clips between them.  Only the clips handed out are solved: `solved` marks
+    them, the other clips' rows stay zero."""
 
     def __init__(self, problems: Sequence[PhysProblem], slots: int, weights=(0.4, 1.7, 0.3, 0.1, 0.1), device: int = -1,
-                 stage3_band_above: Optional[int] = None):
+                 stage3_band_above: Optional[int] = None, claim=None):
         from .parallel import work_estimate
         self.L = load_lib()
         self.problems = list(problems)
@@ -379,6 +392,27 @@ class PhysQueue:
         self.dims = {k: getattr(d, k) for k, _ in _Dims._fields_}
         self.N, self.slots = N, self.dims["batch"]
         self.n_ee_max = max(p.n_ee for p in self.problems)
+        self.claim, self._claimed, self._claim_error = claim, [], None
+        self._claim_cb = None                  # the ctypes callback: alive as long as the handle holds it
+        if claim is not None:
+            self._claim_cb = CLAIM_FN(self._on_claim)
+            rc = self.L.chd_phys_queue_set_claim(self.h, C.cast(self._claim_cb, C.c_void_p), None)
+            if rc != 0:
+                self.close()
+                raise RuntimeError("chd_phys_queue_set_claim failed with code %d" % rc)
+
+    def _on_claim(self, ctx, want, first):
+        """chd_phys_claim_fn over `claim`: records the positions handed out; an exception in `claim` becomes -1 and is
+        raised again by solve()."""
+        try:
+            f, k = (int(v) for v in self.claim(int(want)))
+        except BaseException as e:            # must not cross the C frames
+            self._claim_error = e
+            return -1
+        first[0] = f
+        if k > 0:
+            self._claimed.append((f, k))
+        return k
 
     def __enter__(self):
         return self
@@ -398,19 +432,29 @@ class PhysQueue:
             pass
 
     def solve(self) -> dict:
-        """Full staged schedule of every clip; the same keys and shapes as `PhysBatch.solve()` for N sequences, plus
-        stage_stats (6, N, 4) (`PhysBatch.stage_stats`)."""
+        """Full staged schedule of every clip (with `claim`: of the clips it hands out); the same keys and shapes as
+        `PhysBatch.solve()` for N sequences, plus stage_stats (6, N, 4) (`PhysBatch.stage_stats`) and solved (N bools)."""
         N, d = self.N, self.dims
         out = dict(samples=np.zeros((3, N, d["frames_out_max"], sample_stride(self.n_ee_max))),
                    frames=np.zeros(N, np.int32), success=np.zeros((N, 2), np.int32),
                    stage_status=np.zeros((6, N), np.int32), stage_iters=np.zeros((6, N), np.int32),
                    stage_stats=np.zeros((6, N, 4)))
+        self._claimed, self._claim_error = [], None
         rc = self.L.chd_phys_queue_solve(self.h, *[_ptr(out[k]) for k in ("samples", "frames", "success", "stage_status",
                                                                           "stage_iters", "stage_stats")])
+        if self._claim_error is not None:
+            e, self._claim_error = self._claim_error, None
+            raise RuntimeError("the claim source of the queue failed") from e
         if rc != 0:
             raise RuntimeError("libchd call failed with code %d" % rc)
+        solved = np.ones(N, bool)
+        if self.claim is not None:
+            solved[:] = False
+            for f, k in self._claimed:
+                solved[f:f + k] = True
+        out["solved"] = solved
         inv = np.argsort(self.order)          # queue position of every input clip
-        axis = dict(samples=1, frames=0, success=0, stage_status=1, stage_iters=1, stage_stats=1)
+        axis = dict(samples=1, frames=0, success=0, stage_status=1, stage_iters=1, stage_stats=1, solved=0)
         return {k: np.take(v, inv, axis=axis[k]) for k, v in out.items()}
 
     def launch_count(self) -> int:

@@ -156,9 +156,23 @@ int chd_phys_queue_create(const chd_phys_problem* problems, int32_t n, int32_t s
  * whenever a slot's clip has finished (checked every 8 iterations) the next clip in queue order takes it, a refilled
  * slot being the same to the solver as that row of a new batch.  Outputs [host] as chd_phys_solve's plus
  * stage_stats (chd_phys_stage_stats' 6 x n x 4 block), indexed by clip (n, not slots); any may be NULL.  A clip's
- * results are those of a chd_phys_batch_create batch of the same n clips.  Calling it again starts the queue over. */
+ * results are those of a chd_phys_batch_create batch of the same n clips.  Calling it again starts the queue over.
+ * With a claim source set (chd_phys_queue_set_claim) the clips come from it instead: only the clips it hands out are
+ * solved and written, the rows of the others are left as they were.  Returns -1 if the source fails or misbehaves. */
 int chd_phys_queue_solve(chd_phys_batch* b, double* samples, int32_t* frames_out, int32_t* success, int32_t* stage_status,
                          int32_t* stage_iters, double* stage_stats);
+
+/* Hands out queue positions: writes the first of k consecutive positions to *first and returns k (0 <= k <= want);
+ * 0 = nothing left, negative = error.  Called on the host thread inside chd_phys_queue_solve. */
+typedef int32_t(chd_phys_claim_fn)(void* ctx, int32_t want, int32_t* first);
+/* Lets a claim source decide which clips of the queue this handle solves, e.g. a counter shared by several processes
+ * that each hold a queue of the same n clips.  chd_phys_queue_solve then asks it for `slots` positions at the start
+ * and, at every refill check point, for as many positions as there are finished slots; the k positions it returns
+ * enter the first k of those slots as one upload.  Once it returns fewer than asked it is not asked again: finished
+ * slots are still harvested but no longer refilled.  The solve returns -1, and the handle stays usable, if the source
+ * returns a negative value, a range outside [0, n), or a position it already handed out in this solve (checked on the
+ * host before any upload).  claim = NULL restores the queue's own order.  Returns -1 for NULL or a batch handle. */
+int chd_phys_queue_set_claim(chd_phys_batch* b, chd_phys_claim_fn* claim, void* ctx);
 
 /* Number of kernels launched by this batch so far. */
 int64_t chd_phys_launch_count(const chd_phys_batch* b);

@@ -5,6 +5,9 @@ Two configurations:
   short: 256 clips of 120 frames, 2 feet (chd.synth.make_problem seeds 0..255, bench.py's inputs): the queue at 64 and
          128 slots against four consecutive 64-clip batches;
   long:  64 clips of 600 frames, 4 feet, densely switching: the queue at 16 slots against four 16-clip batches.
+A third, `--config claim`, times the short configuration's 64-slot queue in its own order against the same queue fed by a
+`chd.parallel.StoreClaim` over a FileStore (one process: the cost of the claim callback and the store round trips that
+the multi-GPU queue of `ShardedSolver(slots=...)` adds).
 Every arm is warmed up, then the arms alternate in one process; each timed repetition is creation + solve (what a user
 of either pays).  A second pass with kernel timing on gives `chd_k_kkt` ms per launch and the admission time.  Per clip
 the outputs of every arm are compared with the batches' (statuses, iteration counts, trajectories).  Prints the card's
@@ -66,9 +69,11 @@ def solve_batches(chd, ps, per, timing=False):
     return out, {"kkt_ms": kkt_ms, "kkt_launches": kkt_n}
 
 
-def solve_queue(chd, ps, slots, timing=False, meter=None):
+def solve_queue(chd, ps, slots, timing=False, meter=None, claim=None):
     u0 = meter.used() if meter else 0
-    q = chd.phys.PhysQueue(ps, slots)
+    if claim is not None:
+        claim.restart()                                 # a fresh counter: the queue starts over
+    q = chd.phys.PhysQueue(ps, slots, claim=claim)
     dev_bytes = (meter.used() - u0) if meter else None
     h0 = q.h2d_bytes()
     q.set_timing(timing)
@@ -126,9 +131,57 @@ def run(chd, name, ps, per, slot_list, reps, meter):
     return res
 
 
+class CountingClaim:
+    """A claim source that counts its calls (store round trips) on the way to another, and the host time they take."""
+
+    def __init__(self, inner):
+        self.inner, self.calls, self.seconds = inner, 0, 0.0
+
+    def restart(self):
+        self.calls, self.seconds = 0, 0.0
+        self.inner.restart()
+
+    def __call__(self, want):
+        t0 = time.perf_counter()
+        r = self.inner(want)
+        self.calls += 1
+        self.seconds += time.perf_counter() - t0
+        return r
+
+
+def run_claim(chd, ps, slots, reps):
+    """The queue in its own order against the same queue claiming from a FileStore counter, alternated."""
+    import tempfile
+    import torch.distributed as dist
+    frames = int(sum(p.n_frames for p in ps))
+    with tempfile.TemporaryDirectory() as tmp:
+        claim = CountingClaim(chd.parallel.StoreClaim(dist.FileStore(os.path.join(tmp, "claims"), 1), "bench", len(ps)))
+        arms = [("queue%d" % slots, lambda: solve_queue(chd, ps, slots)),
+                ("queue%d_store_claim" % slots, lambda: solve_queue(chd, ps, slots, claim=claim))]
+        for _, f in arms:                              # warm-up
+            f()
+        times = {a: [] for a, _ in arms}
+        outs = {}
+        for r in range(reps):
+            for a, f in arms:
+                t0 = time.perf_counter()
+                outs[a] = f()[0]
+                times[a].append(time.perf_counter() - t0)
+        res = {"config": "%d x 120 frames, 2 feet: own order vs StoreClaim over a FileStore" % len(ps), "clips": len(ps),
+               "frames": frames, "arms": {}}
+        for a, _ in arms:
+            med = float(np.median(times[a]))
+            res["arms"][a] = {"wall_s": [round(t, 4) for t in times[a]], "frames_per_s": round(frames / med, 1),
+                              "vs_own_order": compare(outs[arms[0][0]], outs[a])}
+        res["arms"][arms[1][0]]["claim_calls"] = claim.calls
+        res["arms"][arms[1][0]]["claim_ms"] = round(1e3 * claim.seconds, 3)       # in the callback, last solve
+        res["arms"][arms[1][0]]["all_solved"] = bool(outs[arms[1][0]]["solved"].all())
+    return res
+
+
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--config", choices=["short", "long", "both"], default="both")
+    ap.add_argument("--config", choices=["short", "long", "both", "claim"], default="both")
     ap.add_argument("--reps", type=int, default=3, help="timed repetitions of every arm (short configuration)")
     ap.add_argument("--reps-long", type=int, default=1)
     ap.add_argument("--out", default=None, help="also write the JSON lines to this file")
@@ -141,6 +194,10 @@ def main():
     if args.config in ("short", "both"):
         ps = [chd.synth.make_problem(s, 120, 2) for s in range(256)]
         lines.append(run(chd, "256 x 120 frames, 2 feet", ps, 64, [64, 128], args.reps, meter))
+        print(json.dumps(dict(lines[-1], card=info)), flush=True)
+    if args.config == "claim":
+        ps = [chd.synth.make_problem(s, 120, 2) for s in range(256)]
+        lines.append(run_claim(chd, ps, 64, args.reps))
         print(json.dumps(dict(lines[-1], card=info)), flush=True)
     if args.config in ("long", "both"):
         ps = [chd.synth.make_problem(s, 600, 4, dense=True) for s in range(64)]

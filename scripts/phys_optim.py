@@ -6,6 +6,8 @@ output files, solved on the GPU.  `scripts/run_phys_mocap.py:159-174` can point 
 Extension: `--in_dir` / `--out_dir` / `--nframes` accept comma separated lists so that many clips are solved as one
 batch (that is where the GPU pays off); `--n_ee 2` selects the toes-only parameterisation; `--slots S` solves the list
 through a queue of S device slots (`chd.phys.PhysQueue`: memory for S clips, each slot refilled as its clip finishes).
+Under torchrun, `--slots S` runs such a queue on every rank's GPU, the ranks claiming their next clips from one shared
+counter (`chd.parallel.ShardedSolver(slots=S)`), and rank 0 writes the four files of every clip.
 """
 import argparse
 import os
@@ -15,6 +17,15 @@ import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+
+
+def write_results(out, problems, out_dirs, n_ee_max):
+    """The four output files of every clip (`chd.phys.write_outputs`) and its status line, from a `solve()` result with
+    all three snapshots: the one-GPU run and rank 0 of a `--slots` run under torchrun write through here."""
+    import chd
+    for i, (p, od) in enumerate(zip(problems, out_dirs)):
+        chd.phys.write_outputs(out, i, p, od, n_ee_max)
+        print("[%d] stages status %s iterations %s -> %s" % (i, out["stage_status"][:, i].tolist(), out["stage_iters"][:, i].tolist(), od))
 
 
 def main(argv=None):
@@ -33,8 +44,6 @@ def main(argv=None):
     ap.add_argument("--slots", type=int, default=0,
                     help="solve the clips through a queue of this many device slots instead of one batch")
     args = ap.parse_args(argv)
-    if args.slots and int(os.environ.get("WORLD_SIZE", 1)) > 1:
-        ap.error("--slots solves on one GPU: it cannot be combined with WORLD_SIZE > 1")
     import chd
     in_dirs = args.in_dir.split(",")
     out_dirs = args.out_dir.split(",")
@@ -48,6 +57,19 @@ def main(argv=None):
     weights = (args.w_com_lin, args.w_com_ang, args.w_ee, args.w_smooth, args.w_dur)
     band = 96 if args.stage3_long else None
     world, rank, local = int(os.environ.get("WORLD_SIZE", 1)), int(os.environ.get("RANK", 0)), int(os.environ.get("LOCAL_RANK", 0))
+    if world > 1 and args.slots:
+        # torchrun with a queue on every GPU: each rank claims its next clips from one counter in the process group's
+        # store, and the results of every clip, all three snapshots included, are merged by clip index on every rank
+        import torch
+        import torch.distributed as dist
+        torch.cuda.set_device(local)
+        dist.init_process_group("nccl", device_id=torch.device("cuda", local))
+        out = chd.parallel.solve_sharded(problems, weights=weights, device=local, rank=rank, world=world,
+                                         stage3_band_above=band, slots=args.slots)
+        dist.destroy_process_group()
+        if rank == 0:
+            write_results(out, problems, out_dirs, max(p.n_ee for p in problems))
+        return
     if world > 1:
         # torchrun: one process per GPU, sequences sharded by predicted work, one gather of the final trajectories;
         # only the durations snapshot travels, so the sharded mode writes sol_out_durations.txt + success_log.txt
@@ -71,9 +93,7 @@ def main(argv=None):
     else:
         batch = chd.phys.PhysBatch(problems, weights=weights, stage3_band_above=band)
     out = batch.solve()
-    for i, (p, od) in enumerate(zip(problems, out_dirs)):
-        chd.phys.write_outputs(out, i, p, od, batch.n_ee_max)
-        print("[%d] stages status %s iterations %s -> %s" % (i, out["stage_status"][:, i].tolist(), out["stage_iters"][:, i].tolist(), od))
+    write_results(out, problems, out_dirs, batch.n_ee_max)
 
 
 if __name__ == "__main__":
