@@ -1,6 +1,7 @@
 // C ABI of the phys-optim path (see include/chd.h).  Host driver: device memory, stage loops, launches.
 #include <cuda_runtime.h>
 
+#include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -33,6 +34,7 @@ __global__ void chd_k_sample(ChdDev D, double* out, int* frames_out);
 __global__ void chd_k_snapshot(ChdDev D, int* frames_out);
 __global__ void chd_k_sched_reset(ChdDev D);
 __global__ void chd_k_admit(ChdDev D, ChdAdmit A);   // chd_queue.cu
+__global__ void chd_k_cost_terms(ChdDev D, int finished_only, double* out);
 
 #define CHD_CUDA(x)                                                                          \
   do {                                                                                       \
@@ -79,7 +81,7 @@ struct ChdQueue {
   bool exhausted = false;             // the source returned fewer positions than asked during this solve
   std::vector<char> given;            // positions the source handed out during this solve
   // outputs of the running chd_phys_queue_solve, indexed by clip
-  double *samples = nullptr, *stage_stats = nullptr;
+  double *samples = nullptr, *stage_stats = nullptr, *terms = nullptr;
   int32_t *frames = nullptr, *success = nullptr, *stage_status = nullptr, *stage_iters = nullptr;
 };
 
@@ -103,7 +105,10 @@ struct chd_phys_batch {
   ChdIpm* h_ipm = nullptr;  // host copy of the per-sequence solver state
   double* d_x0 = nullptr;
   int64_t h2d_bytes = 0;
+  std::vector<ChdStageDev> stages;   // B x 6 rows of the stage table (a queue: of the slots; its records hold every clip's)
   ChdStageDev* d_stages = nullptr;
+  double* terms_out = nullptr;        // chd_phys_set_cost_terms_out: [host] where a solve writes the final cost terms
+  double* d_terms = nullptr;          // B x CHD_PHYS_N_TERMS (chd_k_cost_terms)
   int sched_max_iter = 0;
   bool sched_has_dur = false;   // the running schedule contains stage 3 (its cost Hessian is rebuilt every iteration)
   // pristine copies of the tables stage 3 rewrites (chd_phys_reset)
@@ -172,22 +177,28 @@ void launch_eval(chd_phys_batch* b) {
 
 // uploads the stage table (optionally with an iteration-cap override for one stage) and the schedule
 int set_schedule(chd_phys_batch* b, const int* sched, int nsched, int override_stage, int override_max_iter) {
-  ChdStageDev tab[6];
-  for (int s = 0; s < 6; ++s) tab[s] = stage_dev(b->hb.stage[s], s);
-  if (override_stage >= 0 && override_max_iter > 0) tab[override_stage].max_iter = override_max_iter;
-  CHD_CUDA(cudaMemcpyAsync(b->d_stages, tab, sizeof(tab), cudaMemcpyHostToDevice, b->stream));
-  b->D.stages = b->d_stages;
+  std::vector<ChdStageDev> tab = b->stages;
+  if (override_stage >= 0 && override_max_iter > 0)
+    for (size_t i = 0; i < tab.size(); i += 6) tab[i + override_stage].max_iter = override_max_iter;
+  CHD_CUDA(cudaMemcpyAsync(b->d_stages, tab.data(), tab.size() * sizeof(ChdStageDev), cudaMemcpyHostToDevice, b->stream));
+  const ChdStageDev* t = tab.data();   // the caps of every sequence are the same
   b->D.nsched = nsched;
   for (int i = 0; i < nsched; ++i) b->D.sched[i] = sched[i];
   b->sched_max_iter = 0;
   b->sched_has_dur = false;
-  for (int i = 0; i < nsched; ++i) b->sched_max_iter += tab[sched[i]].max_iter + 2, b->sched_has_dur |= sched[i] == CHD_STAGE_3;
+  for (int i = 0; i < nsched; ++i) b->sched_max_iter += t[sched[i]].max_iter + 2, b->sched_has_dur |= sched[i] == CHD_STAGE_3;
   chd_k_sched_reset<<<(b->hb.B + 127) / 128, 128, 0, b->stream>>>(b->D);
   b->launches++;
   return 0;
 }
 
 int queue_refill(chd_phys_batch* b, int it, int* last_it);
+
+// the cost terms of every sequence (finished_only: of those whose schedule is over) into d_terms
+void launch_cost_terms(chd_phys_batch* b, int finished_only) {
+  chd_k_cost_terms<<<b->hb.B, CHD_TERMS_THREADS, 0, b->stream>>>(b->D, finished_only, b->d_terms);
+  b->launches++;
+}
 
 // runs the uploaded schedule to completion: every sequence walks through its stages at its own pace (a queue refills
 // the slots whose clip has finished at the check points, and the loop runs until the last admitted clip finishes)
@@ -280,7 +291,7 @@ void queue_tables(chd_phys_batch* b, F&& f) {
   f(hb.node_const, D.node_const), f(hb.par, D.par), f(hb.t_dyn, D.t_dyn), f(hb.t_rom, D.t_rom), f(hb.t_data, D.t_data);
   f(hb.row_lo, D.row_lo), f(hb.row_hi, D.row_hi), f(hb.dur0, D.dur0), f(hb.x0, D.x, b->d_x0);
   f(hb.poly_T, D.poly_T, b->poly_T0, D.poly_Tt), f(hb.poly_tend, D.poly_tend, b->poly_tend0, D.poly_tendt);
-  f(hb.phase_tend, D.phase_tend, b->phase_tend0);
+  f(hb.phase_tend, D.phase_tend, b->phase_tend0), f(b->stages, D.stages);
 }
 
 // Packs the layout of all hb.B clips into one record per clip and keeps the first `slots` rows of every table as the
@@ -410,6 +421,9 @@ int queue_harvest(chd_phys_batch* b, int slot) {
       CHD_CUDA(cudaMemcpyAsync(q.samples + (s * n + c) * row, b->D.snapshots + (s * S + slot) * row, row * sizeof(double),
                                cudaMemcpyDeviceToHost, b->stream));
   if (q.frames) CHD_CUDA(cudaMemcpyAsync(q.frames + c, b->d_frames + slot, sizeof(int), cudaMemcpyDeviceToHost, b->stream));
+  if (q.terms)
+    CHD_CUDA(cudaMemcpyAsync(q.terms + (size_t)c * CHD_PHYS_N_TERMS, b->d_terms + (size_t)slot * CHD_PHYS_N_TERMS,
+                             CHD_PHYS_N_TERMS * sizeof(double), cudaMemcpyDeviceToHost, b->stream));
   const ChdIpm& I = b->h_ipm[slot];
   if (q.success) q.success[2 * c] = I.st_status[CHD_STAGE_22] == 0, q.success[2 * c + 1] = I.st_status[CHD_STAGE_3] == 0 || I.st_status[CHD_STAGE_4] == 0;
   for (size_t s = 0; s < 6; ++s) {
@@ -437,6 +451,7 @@ int queue_refill(chd_phys_batch* b, int it, int* last_it) {
   if (q.claim && (rc = queue_claim(b, k, &first, &k))) return rc;
   // this iteration's side-stream kernels (chd_k_kcopy, chd_k_curv, chd_k_hess_dur) may still read the slots' state
   CHD_CUDA(cudaStreamWaitEvent(b->stream, b->ev_copy, 0));
+  if (q.terms) launch_cost_terms(b, 1);   // before admission overwrites the finished slots
   for (int s : freed)
     if ((rc = queue_harvest(b, s))) return rc;
   if (k == 0) return 0;
@@ -489,9 +504,21 @@ static int batch_create_impl(const chd_phys_problem* problems, int32_t batch, in
 // a batch (slots = 0) or a queue of `batch` clips through `slots` slots
 static int create(const chd_phys_problem* problems, int32_t batch, int32_t slots, const chd_phys_weights* weights,
                   int32_t device, const chd_phys_options* opt, chd_phys_batch** out) {
-  chd_phys_options o = {-1};
+  chd_phys_options o = {-1, nullptr};
   if (opt) o = *opt;
   if (o.stage3_band_above < -1 || o.stage3_band_above > CHD_MAX_DUR) return -1;
+  // a weight must be finite and not negative
+  auto bad = [](const chd_phys_weights& w) {
+    for (double v : {w.w_com_lin, w.w_com_ang, w.w_ee, w.w_smooth, w.w_dur})
+      if (!std::isfinite(v) || v < 0.0) return true;
+    return false;
+  };
+  if (o.clip_weights) {
+    for (int i = 0; i < batch; ++i)
+      if (bad(o.clip_weights[i])) return -1;
+  } else if (weights && bad(*weights)) {
+    return -1;
+  }
   chd_phys_batch* b = new chd_phys_batch();
   std::memset(&b->D, 0, sizeof(b->D));
   const int rc = batch_create_impl(problems, batch, slots, weights, device, o, b);
@@ -521,9 +548,14 @@ static int batch_create_impl(const chd_phys_problem* problems, int32_t batch, in
   if (device >= 0) CHD_CUDA(cudaSetDevice(device));
   chd_phys_weights w = {0.4, 1.7, 0.3, 0.1, 0.1};  // phys_optim.cpp:27-31
   if (weights) w = *weights;
-  int rc = chd_build_layout(problems, batch, w, b->hb, opt.stage3_band_above);
+  // one weight tuple per problem: the clip's own (chd_phys_options.clip_weights) or the batch's
+  std::vector<chd_phys_weights> wv(batch, w);
+  if (opt.clip_weights) wv.assign(opt.clip_weights, opt.clip_weights + batch);
+  int rc = chd_build_layout(problems, batch, wv.data(), b->hb, opt.stage3_band_above);
   if (rc) return rc;
   ChdHostBatch& hb = b->hb;
+  b->stages.resize(hb.stage.size());
+  for (size_t i = 0; i < hb.stage.size(); ++i) b->stages[i] = stage_dev(hb.stage[i], (int)(i % 6));
   ChdDev& D = b->D;
   std::memset(&D, 0, sizeof(D));
   b->host_only = host_only;
@@ -609,8 +641,10 @@ static int batch_create_impl(const chd_phys_problem* problems, int32_t batch, in
   b->allocs.push_back(b->d_frames);
   b->h_ipm = (ChdIpm*)std::malloc(B * sizeof(ChdIpm));   // pageable: pinned allocation / release is slow per batch
   if (!b->h_ipm) return -3;
-  CHD_CUDA(cudaMallocAsync((void**)&b->d_stages, 6 * sizeof(ChdStageDev), b->stream));
+  CHD_CUDA(cudaMallocAsync((void**)&b->d_stages, b->stages.size() * sizeof(ChdStageDev), b->stream));
   b->allocs.push_back(b->d_stages);
+  D.stages = b->d_stages;
+  if ((rc = dev_alloc(b, B * CHD_PHYS_N_TERMS, &b->d_terms))) return rc;
   if ((rc = dev_alloc(b, 3 * B * hb.fo_max * stride, &D.snapshots))) return rc;
   if (b->queue && (rc = queue_device(b, sms))) return rc;
   CHD_CUDA(cudaStreamSynchronize(b->stream));
@@ -844,6 +878,10 @@ int chd_phys_solve(chd_phys_batch* b, double* samples, int32_t* frames_out, int3
   }
   if (samples) CHD_CUDA(cudaMemcpyAsync(samples, b->D.snapshots, 3 * snap * sizeof(double), cudaMemcpyDeviceToHost, b->stream));
   if (frames_out) CHD_CUDA(cudaMemcpyAsync(frames_out, b->d_frames, B * sizeof(int), cudaMemcpyDeviceToHost, b->stream));
+  if (b->terms_out) {   // x is every sequence's final iterate, the one of the durations snapshot
+    launch_cost_terms(b, 0);
+    CHD_CUDA(cudaMemcpyAsync(b->terms_out, b->d_terms, (size_t)B * CHD_PHYS_N_TERMS * sizeof(double), cudaMemcpyDeviceToHost, b->stream));
+  }
   CHD_CUDA(cudaStreamSynchronize(b->stream));
   return 0;
 }
@@ -866,7 +904,7 @@ int chd_phys_queue_solve(chd_phys_batch* b, double* samples, int32_t* frames_out
   int sched[6] = {CHD_STAGE_11, CHD_STAGE_12, CHD_STAGE_21, CHD_STAGE_22, CHD_STAGE_3, CHD_STAGE_4};
   if ((rc = set_schedule(b, sched, 6, -1, 0))) return rc;
   q.samples = samples, q.frames = frames_out, q.success = success, q.stage_status = stage_status;
-  q.stage_iters = stage_iters, q.stage_stats = stage_stats;
+  q.stage_iters = stage_iters, q.stage_stats = stage_stats, q.terms = b->terms_out;
   q.clip.assign(S, -1);
   std::vector<int> slots(S);
   std::iota(slots.begin(), slots.end(), 0);
@@ -881,6 +919,7 @@ int chd_phys_queue_solve(chd_phys_batch* b, double* samples, int32_t* frames_out
     b->h2d_bytes += (int64_t)(idle.size() * sizeof(ChdIpm));
   }
   if ((rc = run_schedule(b))) return rc;
+  if (q.terms) launch_cost_terms(b, 0);
   for (int i = 0; i < S; ++i)
     if ((rc = queue_harvest(b, i))) return rc;
   CHD_CUDA(cudaStreamSynchronize(b->stream));
@@ -890,6 +929,31 @@ int chd_phys_queue_solve(chd_phys_batch* b, double* samples, int32_t* frames_out
 int chd_phys_queue_set_claim(chd_phys_batch* b, chd_phys_claim_fn* claim, void* ctx) {
   if (!b || !b->queue) return -1;
   b->queue->claim = claim, b->queue->claim_ctx = claim ? ctx : nullptr;
+  return 0;
+}
+
+int chd_phys_get_stage_weights(const chd_phys_batch* b, double* w) {
+  if (!b || !w) return -1;
+  for (const ChdStageDev& s : b->stages) {
+    for (int q = 0; q < 3; ++q) w[q] = s.w_data[q], w[3 + q] = s.w_vel[q], w[6 + q] = s.w_acc[q];
+    w[9] = s.w_dur;
+    w += 10;
+  }
+  return 0;
+}
+
+int chd_phys_cost_terms(chd_phys_batch* b, double* terms) {
+  if (!b || !terms || b->host_only || b->queue) return -1;
+  launch_cost_terms(b, 0);
+  CHD_CUDA(cudaMemcpyAsync(terms, b->d_terms, (size_t)b->hb.B * CHD_PHYS_N_TERMS * sizeof(double), cudaMemcpyDeviceToHost, b->stream));
+  CHD_CUDA(cudaStreamSynchronize(b->stream));
+  CHD_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int chd_phys_set_cost_terms_out(chd_phys_batch* b, double* terms) {
+  if (!b || b->host_only) return -1;
+  b->terms_out = terms;
   return 0;
 }
 

@@ -10,6 +10,7 @@
 #define CHD_NL_FLOOR 1e-4
 #define CHD_UNOBS_EPS 1e-14 /* "sees": diagonal of the scaled cost Hessian above this (a sample sitting exactly on a node gives weights of 1e-17) */
 #define CHD_DW_UNOBS 1e-4   /* fixed Levenberg-Marquardt weight of foot-motion node values no cost sample sees (zero diagonal of the cost Hessian) */
+#define CHD_TERMS_THREADS 256
 #define CHD_CURV_MIN 1e-8   /* multiplier threshold below which y^+ Jd^T Jd is not added (same in oracle/ipm_oracle.cpp) */
 
 // row flags
@@ -89,7 +90,7 @@ struct ChdDev {
   double *rhs0, *rhs1;                        // right-hand side of the KKT system as rhs0 + mu * rhs1 (chd_k_asm), [B][Na_max + nb_max]
   size_t scratch_stride;                      // doubles per sequence in `scratch`
   ChdIpm* ipm;                                // B
-  const ChdStageDev* stages;                  // 6 stage configurations (device)
+  const ChdStageDev* stages;                  // B x 6 stage configurations, [b * 6 + stage id] (chd_stage)
   int sched[8], nsched;                       // stage ids of the running schedule
   double* snapshots;                          // 3 x B x fo_max x (6 + 7 n_ee_max)
 };
@@ -172,6 +173,9 @@ __device__ __forceinline__ void chd_row_barrier(int f, double mu, ChdGaps gap, d
   if (f & CHD_ROW_HASL) acc -= mu * log(gap.L);
   if (f & CHD_ROW_HASU) acc -= mu * log(gap.U);
 }
+
+// configuration of `stage` for sequence b: every sequence has its own six rows (its cost weights)
+__device__ __forceinline__ const ChdStageDev& chd_stage(const ChdDev& D, int b, int stage) { return D.stages[(size_t)b * 6 + stage]; }
 
 // puts one sequence at the start of the schedule D.sched (chd_k_sched_reset, chd_k_admit)
 __device__ __forceinline__ void chd_sched_begin(const ChdDev& D, ChdIpm& I) {

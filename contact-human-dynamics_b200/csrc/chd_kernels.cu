@@ -9,6 +9,7 @@
 //   chd_k_linesearch  : filter backtracking line search (trial point in shared memory, or in global memory when the
 //                       iterate is too long for it), update
 //   chd_k_sample      : SaveSolution sampling (phys_optim.cpp:63-143)
+//   chd_k_cost_terms  : the unweighted cost terms at the current x
 #include <cuda_runtime.h>
 
 #include "chd_block.cuh"
@@ -18,7 +19,7 @@
 __global__ void chd_k_stage_begin(ChdDev D) {
   const int b = blockIdx.x;
   if (D.ipm[b].phase != CHD_PH_BEGIN) return;
-  const ChdStageDev sg = D.stages[D.ipm[b].stage];
+  const ChdStageDev sg = chd_stage(D, b, D.ipm[b].stage);
   const int max_iter = sg.max_iter;
   const ChdSeq* h = D.seq + b;
   if (sg.opt_dur && h->n_dur == 0) {
@@ -88,7 +89,7 @@ __global__ void __launch_bounds__(CHD_THREADS) chd_k_eval(ChdDev D) {
   extern __shared__ double sm[];
   const int b = blockIdx.x;
   if (D.ipm[b].phase != CHD_PH_BEGIN && D.ipm[b].phase != CHD_PH_RUN) return;
-  const ChdStageDev sg = D.stages[D.ipm[b].stage];
+  const ChdStageDev sg = chd_stage(D, b, D.ipm[b].stage);
   const ChdSeq* h = D.seq + b;
   const double* xs;
   double *gs, *red;
@@ -205,7 +206,7 @@ __global__ void __launch_bounds__(CHD_THREADS) chd_k_linesearch(ChdDev D) {
   const int b = blockIdx.x;
   ChdIpm& I = D.ipm[b];
   if (I.phase != CHD_PH_RUN || !I.step_ready) return;
-  const ChdStageDev sg = D.stages[I.stage];
+  const ChdStageDev& sg = chd_stage(D, b, I.stage);
   const ChdSeq* h = D.seq + b;
   const int n = h->n, m = h->m, tid = threadIdx.x, nt = blockDim.x;
   const size_t ro = (size_t)b * D.m_max, vo = (size_t)b * D.n_max;
@@ -362,6 +363,49 @@ __global__ void __launch_bounds__(CHD_THREADS) chd_k_linesearch(ChdDev D) {
 }
 template __global__ void chd_k_linesearch<false>(ChdDev D);
 template __global__ void chd_k_linesearch<true>(ChdDev D);
+
+// ------------------------------------------------------------------ cost terms --------------------
+// The CHD_PHYS_N_TERMS unweighted cost terms of a sequence at the current x (chd_phys_cost_terms): data fit of the base
+// position, the base orientation and the feet; velocity smoothing (same order); acceleration smoothing (same order);
+// duration change.  The cost items of chd_eval_all with weight 1, all of them whatever the stage, on the spline tables
+// of the current durations.  Per-thread accumulators and a fixed-order tree reduction, no atomics: a sequence's terms
+// are bitwise the same run to run and in any batch with the same strides.  finished_only: only the sequences whose
+// schedule is over (the slots a queue harvests at a check point).  out: B x CHD_PHYS_N_TERMS.
+__global__ void __launch_bounds__(CHD_TERMS_THREADS) chd_k_cost_terms(ChdDev D, int finished_only, double* out) {
+  __shared__ double red[CHD_PHYS_N_TERMS][CHD_TERMS_THREADS];
+  const int b = blockIdx.x, tid = threadIdx.x;
+  if (finished_only && D.ipm[b].phase != CHD_PH_FINISHED) return;
+  ChdCtx c;
+  chd_make_ctx(D, b, D.x + (size_t)b * D.n_max, c);
+  const ChdSeq* h = c.h;
+  double acc[CHD_PHYS_N_TERMS];
+#pragma unroll
+  for (int q = 0; q < CHD_PHYS_N_TERMS; ++q) acc[q] = 0.0;
+  const int nsp = 2 + h->n_ee, F = h->F, ns = h->n_smooth;
+  for (int it = tid; it < nsp * F; it += blockDim.x) {
+    const int s = it / F, i = it % F, cls = s < 2 ? s : 2;
+    const double d = chd_item_data<false>(c, s, i, 1.0, nullptr);
+    const double v = i < ns ? chd_item_smooth<false>(c, s, i, 0, 1.0, nullptr) : 0.0;
+    const double a = i < ns ? chd_item_smooth<false>(c, s, i, 1, 1.0, nullptr) : 0.0;
+#pragma unroll
+    for (int q = 0; q < 3; ++q)
+      if (q == cls) acc[q] += d, acc[3 + q] += v, acc[6 + q] += a;
+  }
+  if (h->n_dur)
+    for (int ee = 0; ee < h->n_ee; ++ee)
+      for (int k = tid; k < h->n_phases[ee] - 1; k += blockDim.x) acc[9] += chd_item_durcost<false>(c, ee, k, 1.0, nullptr);
+#pragma unroll
+  for (int q = 0; q < CHD_PHYS_N_TERMS; ++q) red[q][tid] = acc[q];
+  __syncthreads();
+  for (int off = blockDim.x / 2; off > 0; off >>= 1) {
+    if (tid < off) {
+#pragma unroll
+      for (int q = 0; q < CHD_PHYS_N_TERMS; ++q) red[q][tid] += red[q][tid + off];
+    }
+    __syncthreads();
+  }
+  if (tid < CHD_PHYS_N_TERMS) out[(size_t)b * CHD_PHYS_N_TERMS + tid] = red[tid][0];
+}
 
 // ------------------------------------------------------------------ sampling ----------------------
 // SaveSolution (phys_optim.cpp:63-143): t accumulates dt while t <= T + 1e-5.

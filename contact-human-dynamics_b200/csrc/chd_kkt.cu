@@ -132,7 +132,7 @@ __global__ void __launch_bounds__(CHD_THREADS) chd_k_hess_dur(ChdDev D) {
   const int b = blockIdx.y;
   const ChdIpm& I = D.ipm[b];
   if (I.phase != CHD_PH_RUN || !I.kw_req) return;
-  const ChdStageDev sg = D.stages[I.stage];
+  const ChdStageDev sg = chd_stage(D, b, I.stage);
   if (!sg.opt_dur) return;
   chd_hess_build(D, b, sg, D.Kwork + (size_t)b * D.kstride, blockIdx.x, gridDim.x);
 }
@@ -147,7 +147,7 @@ __global__ void __launch_bounds__(128) chd_k_hess_fin(ChdDev D, int mode) {
     if (I.phase != CHD_PH_BEGIN) return;
     base = D.Kbase + (size_t)b * D.kstride;
   } else {
-    if (I.phase != CHD_PH_RUN || !I.kw_req || !D.stages[I.stage].opt_dur) return;
+    if (I.phase != CHD_PH_RUN || !I.kw_req || !chd_stage(D, b, I.stage).opt_dur) return;
     base = D.Kwork + (size_t)b * D.kstride;
   }
   const ChdSeq* h = D.seq + b;
@@ -279,7 +279,7 @@ __global__ void __launch_bounds__(256, 2) chd_k_hess_base(ChdDev D) {
   __shared__ double s_ws[8][192];
   const int b = blockIdx.y;
   if (D.ipm[b].phase != CHD_PH_BEGIN) return;
-  const ChdStageDev sg = D.stages[D.ipm[b].stage];
+  const ChdStageDev sg = chd_stage(D, b, D.ipm[b].stage);
   ChdKT K;
   chd_kt_init(D, D.seq + b, D.Kwork + (size_t)b * D.kstride, K);
   K.ovf = &D.ipm[b].band_ovf;
@@ -298,7 +298,7 @@ __global__ void __launch_bounds__(256, 2) chd_k_hess_base(ChdDev D) {
 __device__ __forceinline__ void chd_assemble(const ChdDev& D, int b, const ChdKT& K, double delta_w, double sf, int t0, int tstep,
                                              double* g0, double* g1) {
   const ChdSeq* h = D.seq + b;
-  const int n = D.stages[D.ipm[b].stage].opt_dur ? h->n : h->n - h->n_dur;   // the durations are unknowns in stage 3 only
+  const int n = chd_stage(D, b, D.ipm[b].stage).opt_dur ? h->n : h->n - h->n_dur;   // the durations are unknowns in stage 3 only
   const int m = h->m, Na = K.Na;
   const size_t ro = (size_t)b * D.m_max, vo = (size_t)b * D.n_max;
   const int* rf = D.rflag + ro;
@@ -411,7 +411,7 @@ __device__ __forceinline__ void chd_kkt_ctx_init(const ChdDev& D, ChdIpm& I, Chd
   extern __shared__ double sm[];
   const int b = blockIdx.x;
   c.b = b, c.I = &I;
-  c.sg = D.stages[I.stage];
+  c.sg = chd_stage(D, b, I.stage);
   const ChdSeq* h = c.h = D.seq + b;
   c.n = h->n, c.m = h->m, c.tid = threadIdx.x, c.nt = blockDim.x;
   c.lane = c.tid & 31, c.warp = c.tid >> 5, c.nwarp = c.nt >> 5;
@@ -1118,7 +1118,7 @@ __global__ void __launch_bounds__(256) chd_k_kcopy(ChdDev D) {
   const int b = blockIdx.y;
   if (!D.ipm[b].kw_req) return;
   if (blockIdx.x == 0) chd_rhs_clear(D, b);
-  if (D.stages[D.ipm[b].stage].opt_dur && D.ipm[b].phase == CHD_PH_RUN) {
+  if (chd_stage(D, b, D.ipm[b].stage).opt_dur && D.ipm[b].phase == CHD_PH_RUN) {
     // stage 3: the cost Hessian moves with the durations; chd_k_hess_dur rebuilds it into a cleared Kwork after the line search
     chd_hess_clear(D, b, D.Kwork + (size_t)b * D.kstride, blockIdx.x, gridDim.x);
     return;
@@ -1147,7 +1147,7 @@ __global__ void __launch_bounds__(256) chd_k_curv(ChdDev D) {
   chd_kt_init(D, D.seq + b, D.Kwork + (size_t)b * D.kstride, K);
   K.ovf = &D.ipm[b].band_ovf;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  chd_curv_rows(D, b, K, D.stages[I.stage], blockIdx.x * 8 + warp, gridDim.x * 8, lane, s_ws + warp * 192);
+  chd_curv_rows(D, b, K, chd_stage(D, b, I.stage), blockIdx.x * 8 + warp, gridDim.x * 8, lane, s_ws + warp * 192);
 }
 
 // Jacobian-dependent matrix entries and right-hand side of every running sequence, on a Kwork that holds the cost
@@ -1164,7 +1164,7 @@ __global__ void __launch_bounds__(256) chd_k_asm(ChdDev D) {
   K.ovf = &D.ipm[b].band_ovf;
   // the band chd_k_kkt factors in a fixed-duration stage: a Jacobian coupling outside it (stage 4 on the durations a
   // failed stage 3 left behind) fails the stage instead of being left out of the factorisation
-  if (!D.stages[I.stage].opt_dur) K.q = D.Qfix - 1;
+  if (!chd_stage(D, b, I.stage).opt_dur) K.q = D.Qfix - 1;
   const size_t go = (size_t)b * (D.Na_max + D.nb_max);
   chd_assemble(D, b, K, I.delta_w, I.sf, blockIdx.x * blockDim.x + threadIdx.x, gridDim.x * blockDim.x, D.rhs0 + go, D.rhs1 + go);
 }

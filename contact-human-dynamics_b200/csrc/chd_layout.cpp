@@ -624,7 +624,7 @@ int build_sequence(const chd_phys_problem& p, SeqBuild& sb, int band_above) {
 
 }  // namespace
 
-int chd_build_layout(const chd_phys_problem* problems, int batch, const chd_phys_weights& wt, ChdHostBatch& hb,
+int chd_build_layout(const chd_phys_problem* problems, int batch, const chd_phys_weights* w, ChdHostBatch& hb,
                      int stage3_band_above) {
   std::vector<SeqBuild> sbs(batch);
   {
@@ -767,28 +767,34 @@ int chd_build_layout(const chd_phys_problem* problems, int batch, const chd_phys
     std::copy(sb.row_kkt.begin(), sb.row_kkt.end(), hb.row_kkt.begin() + (size_t)i * hb.m_max);
     std::copy(sb.sets.begin(), sb.sets.end(), hb.sets.begin() + (size_t)i * hb.sets_max);
   }
-  // staged schedule (phys_optim.cpp:554-749, SURVEY Appendix B)
+  // staged schedule (phys_optim.cpp:554-749, SURVEY Appendix B): six stage rows per sequence, which differ only in the
+  // user weights (stages 2.1, 2.2, 3 and 4); stages 1.1 and 1.2 keep their fixed weights
   const unsigned ACC = CHD_MASK(CHD_SET_ACC), LEG = CHD_MASK(CHD_SET_TERRAIN) | CHD_MASK(CHD_SET_ROM),
                  HEEL = CHD_MASK(CHD_SET_HEEL), DYN = CHD_MASK(CHD_SET_DYN) | CHD_MASK(CHD_SET_FORCE),
                  HGT = CHD_MASK(CHD_SET_HEIGHT);
-  ChdStageCfg s1 = {ACC, {1.0, 1.0, 1.0}, {0.1, 0.1, 0.1}, {0, 0, 0}, 7000, 0.0};
-  ChdStageCfg s2 = {ACC | LEG | DYN | HEEL, {wt.w_com_lin, wt.w_com_ang, wt.w_ee}, {0.001, 0.001, wt.w_smooth},
-                    {0.0001, 0.0001, 0.0001}, 7000, 0.0};
-  hb.stage[CHD_STAGE_11] = s1;
-  hb.stage[CHD_STAGE_12] = s1;
-  hb.stage[CHD_STAGE_12].set_mask = ACC | LEG | HEEL;
-  hb.stage[CHD_STAGE_21] = s2;
-  hb.stage[CHD_STAGE_22] = s2;
-  hb.stage[CHD_STAGE_22].set_mask |= HGT;
-  hb.stage[CHD_STAGE_22].max_iter = 2500;
-  // stage 3 (phys_optim.cpp:663-711): every set of 2.2 + TotalTime (+ the duration bounds as rows), no acceleration
-  // smoothing (:693, vel_smooth_cost.cpp:72-79), DurationCost (:696-703)
-  hb.stage[CHD_STAGE_3] = hb.stage[CHD_STAGE_22];
-  hb.stage[CHD_STAGE_3].set_mask |= CHD_MASK(CHD_SET_TOTTIME) | CHD_MASK(CHD_SET_DURPOS);
-  for (int q = 0; q < 3; ++q) hb.stage[CHD_STAGE_3].w_acc[q] = 0.0;
-  hb.stage[CHD_STAGE_3].w_dur = wt.w_dur;
-  hb.stage[CHD_STAGE_3].max_iter = 2000;
-  hb.stage[CHD_STAGE_4] = hb.stage[CHD_STAGE_22];
-  hb.stage[CHD_STAGE_4].max_iter = 7000;
+  hb.stage.resize((size_t)B * 6);
+  for (int i = 0; i < B; ++i) {
+    const chd_phys_weights& wt = w[i];
+    ChdStageCfg* st = hb.stage.data() + (size_t)i * 6;
+    ChdStageCfg s1 = {ACC, {1.0, 1.0, 1.0}, {0.1, 0.1, 0.1}, {0, 0, 0}, 7000, 0.0};
+    ChdStageCfg s2 = {ACC | LEG | DYN | HEEL, {wt.w_com_lin, wt.w_com_ang, wt.w_ee}, {0.001, 0.001, wt.w_smooth},
+                      {0.0001, 0.0001, 0.0001}, 7000, 0.0};
+    st[CHD_STAGE_11] = s1;
+    st[CHD_STAGE_12] = s1;
+    st[CHD_STAGE_12].set_mask = ACC | LEG | HEEL;
+    st[CHD_STAGE_21] = s2;
+    st[CHD_STAGE_22] = s2;
+    st[CHD_STAGE_22].set_mask |= HGT;
+    st[CHD_STAGE_22].max_iter = 2500;
+    // stage 3 (phys_optim.cpp:663-711): every set of 2.2 + TotalTime (+ the duration bounds as rows), no acceleration
+    // smoothing (:693, vel_smooth_cost.cpp:72-79), DurationCost (:696-703)
+    st[CHD_STAGE_3] = st[CHD_STAGE_22];
+    st[CHD_STAGE_3].set_mask |= CHD_MASK(CHD_SET_TOTTIME) | CHD_MASK(CHD_SET_DURPOS);
+    for (int q = 0; q < 3; ++q) st[CHD_STAGE_3].w_acc[q] = 0.0;
+    st[CHD_STAGE_3].w_dur = wt.w_dur;
+    st[CHD_STAGE_3].max_iter = 2000;
+    st[CHD_STAGE_4] = st[CHD_STAGE_22];
+    st[CHD_STAGE_4].max_iter = 7000;
+  }
   return 0;
 }

@@ -29,11 +29,16 @@ struct ChdHostBatch {
   std::vector<int> poly_ph;          // B x S x Pmax: phase | poly-in-phase << 12 | polys-in-phase << 20 (phase based splines)
   std::vector<int> ent_row, col_ptr, col_ent;   // row of every Jacobian slot; slots grouped by column (gathers instead of atomics)
   std::vector<ChdSet> sets;
-  ChdStageCfg stage[6];
+  std::vector<ChdStageCfg> stage;    // B x 6: the stages of every sequence (its weights), [b * 6 + stage id]
   int par_stride() const { return (18 + 3 * n_ee_max) * F_max; }
 };
 
-// returns 0 on success; negative on malformed input.  stage3_band_above: see chd_phys_options (-1: switch times are
-// border unknowns, stage 3 limited to CHD_MAX_DUR of them)
-int chd_build_layout(const chd_phys_problem* problems, int batch, const chd_phys_weights& w, ChdHostBatch& out,
+// returns 0 on success; negative on malformed input.  w: the weights of every problem (batch entries).
+// stage3_band_above: see chd_phys_options (-1: switch times are border unknowns, stage 3 limited to CHD_MAX_DUR of them)
+int chd_build_layout(const chd_phys_problem* problems, int batch, const chd_phys_weights* w, ChdHostBatch& out,
                      int stage3_band_above = -1);
+// the same weights for every problem
+inline int chd_build_layout(const chd_phys_problem* problems, int batch, const chd_phys_weights& w, ChdHostBatch& out,
+                            int stage3_band_above = -1) {
+  return chd_build_layout(problems, batch, std::vector<chd_phys_weights>(batch, w).data(), out, stage3_band_above);
+}

@@ -95,8 +95,10 @@ class StoreClaim:
 
 
 # Row of a rank's block in the merge of queue results (merge_solved): clip index, the three SaveSolution snapshots
-# (3 x fo x stride), then frames, success[2], stage_status[6], stage_iters[6], stage_stats[6 x 4].
+# (3 x fo x stride), then frames, success[2], stage_status[6], stage_iters[6], stage_stats[6 x 4] and, when the results
+# carry them, the cost terms[10].
 Q_EXTRA = 1 + 2 + 6 + 6 + 24
+Q_TERMS = len(phys.COST_TERMS)
 
 
 def merge_solved(local: dict, world: int, group=None, tensor_device=None) -> dict:
@@ -106,14 +108,16 @@ def merge_solved(local: dict, world: int, group=None, tensor_device=None) -> dic
     moves the blocks, each row carrying its clip index, the three snapshots and the status trailer.  Rows are copied,
     never summed, so every bit of a result (a -0.0 too) arrives as its rank computed it.  Returns `PhysQueue.solve()`'s
     keys over all N clips in input order, plus `solved_by` (N, the rank that solved each clip, -1: none) and
-    `d2h_bytes` (the gathered block).  `tensor_device`: where the collective's tensors live (cuda for nccl, the
-    default cpu for gloo)."""
+    `d2h_bytes` (the gathered block).  `cost_terms`, when every rank's results have them, travel in the row next to
+    the stage statistics.  `tensor_device`: where the collective's tensors live (cuda for nccl, the default cpu for
+    gloo)."""
     import torch
     import torch.distributed as dist
     dev = tensor_device or torch.device("cpu")
     _, N, fo, stride = local["samples"].shape
     snap = 3 * fo * stride
-    width = 1 + snap + Q_EXTRA
+    terms = "cost_terms" in local
+    width = 1 + snap + Q_EXTRA + (Q_TERMS if terms else 0)
     mine = np.nonzero(local["solved"])[0]
     n = len(mine)
     collective = world > 1 and dist.is_initialized()
@@ -132,6 +136,8 @@ def merge_solved(local: dict, world: int, group=None, tensor_device=None) -> dic
     tr[:, 3:9] = local["stage_status"][:, mine].T
     tr[:, 9:15] = local["stage_iters"][:, mine].T
     tr[:, 15:39] = local["stage_stats"][:, mine].transpose(1, 0, 2).reshape(n, 24)
+    if terms:
+        tr[:, 39:39 + Q_TERMS] = local["cost_terms"][mine]
     g = blk
     if collective and cmax > 0:
         send = torch.from_numpy(blk).to(dev)
@@ -153,6 +159,9 @@ def merge_solved(local: dict, world: int, group=None, tensor_device=None) -> dic
     out["stage_status"][:, idx] = tr[:, 3:9].T
     out["stage_iters"][:, idx] = tr[:, 9:15].T
     out["stage_stats"][:, idx] = tr[:, 15:39].reshape(len(idx), 6, 4).transpose(1, 0, 2)
+    if terms:
+        out["cost_terms"] = np.zeros((N, Q_TERMS))
+        out["cost_terms"][idx] = tr[:, 39:39 + Q_TERMS]
     out["solved"][idx] = True
     out["solved_by"][idx] = rank_of
     out["d2h_bytes"] = int(g.nbytes)
@@ -178,12 +187,16 @@ class ShardedSolver:
     `solved_by`.  Every rank keeps the page-locked record store of all N clips (about 106 MB per 256 clips of 120
     frames, 2 feet), and every rank must call `solve()` as often as the others.  With `slots`, `solve_fn(problems)`
     stands in for `PhysQueue.solve()` over all N problems and returns its dict, `solved` marking the clips this rank
-    solved."""
+    solved.
 
-    def __init__(self, problems, weights=(0.4, 1.7, 0.3, 0.1, 0.1), device: int = 0, rank: int = 0, world: int = 1,
+    `weights`: one 5-tuple for every problem or one per problem (`phys.clip_weights`).  `solve(cost_terms=True)`
+    (with `slots` only) also returns every clip's unweighted cost terms (`phys.COST_TERMS`), merged by clip index."""
+
+    def __init__(self, problems, weights=phys.DEFAULT_WEIGHTS, device: int = 0, rank: int = 0, world: int = 1,
                  group=None, solve_fn=None, tensor_device=None, stage3_band_above=None, slots=None, store=None):
         self.problems, self.rank, self.world, self.group = list(problems), rank, world, group
         self.queue_slots, self.queue = slots, None
+        per = phys.clip_weights(weights, len(self.problems))
         if slots is not None:
             self._init_queue(weights, device, solve_fn, tensor_device, stage3_band_above, slots, store)
             return
@@ -198,7 +211,8 @@ class ShardedSolver:
         self.batch = None
         import torch
         if solve_fn is None:
-            self.batch = phys.PhysBatch([self.problems[i] for i in self.mine], weights=weights, device=device,
+            self.batch = phys.PhysBatch([self.problems[i] for i in self.mine], device=device,
+                                        weights=weights if per is None else per[self.mine],
                                         stage3_band_above=stage3_band_above) if self.mine else None
             tensor_device = tensor_device or torch.device("cuda", device)
         self.tdev = tensor_device or torch.device("cpu")
@@ -228,14 +242,14 @@ class ShardedSolver:
             self.queue.close()
             self.queue = None
 
-    def _solve_queue(self) -> dict:
+    def _solve_queue(self, cost_terms: bool) -> dict:
         import time
         t0 = time.perf_counter()
         if self.solve_fn is not None:
             local = self.solve_fn(self.problems)
         else:
             self.claim.restart()
-            local = self.queue.solve()
+            local = self.queue.solve(cost_terms=cost_terms)
         t1 = time.perf_counter()
         out = merge_solved(local, self.world, self.group, self.tdev)
         t2 = time.perf_counter()
@@ -287,12 +301,15 @@ class ShardedSolver:
         self.send[:, self.fo * self.stride:] = torch.from_numpy(trailer).to(self.tdev)
         return trailer
 
-    def solve(self, resident: bool = False) -> dict:
+    def solve(self, resident: bool = False, cost_terms: bool = False) -> dict:
         """Solves the shard (resident=True: device-side reset of an already uploaded batch) and gathers.  Every rank
         returns the full result in the original sequence order.  With `slots`: the queue solve and the merge of every
-        clip's results (resident does not apply: a queue always starts over)."""
+        clip's results (resident does not apply: a queue always starts over), with `cost_terms` as
+        `PhysQueue.solve`'s."""
         if self.queue_slots is not None:
-            return self._solve_queue()
+            return self._solve_queue(cost_terms)
+        if cost_terms:
+            raise ValueError("cost_terms needs the queue form of the sharded solve (slots=S)")
         import time
         import torch
         import torch.distributed as dist
@@ -319,14 +336,15 @@ class ShardedSolver:
                     stage_iters=tr[:, 9:15].astype(np.int32).T, d2h_bytes=int(g.nbytes))
 
 
-def solve_sharded(problems, weights=(0.4, 1.7, 0.3, 0.1, 0.1), device: int = 0, rank: int = 0, world: int = 1, group=None,
-                  solve_fn=None, tensor_device=None, stage3_band_above=None, slots=None, store=None) -> dict:
+def solve_sharded(problems, weights=phys.DEFAULT_WEIGHTS, device: int = 0, rank: int = 0, world: int = 1, group=None,
+                  solve_fn=None, tensor_device=None, stage3_band_above=None, slots=None, store=None,
+                  cost_terms: bool = False) -> dict:
     """shard -> solve -> one gather -> unshard for a list of `PhysProblem`s (see ShardedSolver; `slots`: a queue on
-    every rank, claimed from one shared counter, merged by clip index)."""
+    every rank, claimed from one shared counter, merged by clip index; `weights` and `cost_terms` as there)."""
     s = ShardedSolver(problems, weights, device, rank, world, group, solve_fn, tensor_device, stage3_band_above, slots,
                       store)
     try:
-        return s.solve()
+        return s.solve(cost_terms=cost_terms)
     finally:
         s.close()
 

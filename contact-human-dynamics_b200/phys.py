@@ -23,6 +23,11 @@ _LIB = None
 
 STAGES = {"1.1": 0, "1.2": 1, "2.1": 2, "2.2": 3, "3": 4, "4": 5}
 SET_NAMES = {0: "acc", 1: "terrain", 2: "rom", 3: "dyn", 4: "force", 5: "heel", 6: "height", 7: "tottime", 8: "durpos"}
+# The unweighted cost terms of `PhysBatch.cost_terms` / `solve(cost_terms=True)`, in column order (chd_phys_cost_terms):
+# data fit, velocity smoothing and acceleration smoothing of the base position, the base orientation and the feet, then
+# the change of the phase durations.
+COST_TERMS = ("data_lin", "data_ang", "data_ee", "vel_lin", "vel_ang", "vel_ee", "acc_lin", "acc_ang", "acc_ee", "dur")
+DEFAULT_WEIGHTS = (0.4, 1.7, 0.3, 0.1, 0.1)   # w_com_lin, w_com_ang, w_ee, w_smooth, w_dur (phys_optim.cpp:27-31)
 
 
 def sample_stride(n_ee_max: int) -> int:
@@ -55,7 +60,35 @@ class _Weights(C.Structure):
 
 
 class _Options(C.Structure):
-    _fields_ = [("stage3_band_above", C.c_int32)]
+    _fields_ = [("stage3_band_above", C.c_int32), ("clip_weights", C.POINTER(_Weights))]
+
+
+def clip_weights(weights, n: int) -> Optional[np.ndarray]:
+    """`weights` as the batch classes take it: one 5-tuple (w_com_lin, w_com_ang, w_ee, w_smooth, w_dur) for every
+    problem -> None, or one 5-tuple per problem -> an (n, 5) array.  Any other shape raises ValueError; the library
+    refuses a weight that is negative or not finite."""
+    w = np.asarray(weights, dtype=np.float64)
+    if w.shape == (5,):
+        return None
+    if w.shape != (n, 5):
+        raise ValueError("weights: one 5-tuple, or one 5-tuple per problem (%d), not an array of shape %s" % (n, w.shape))
+    return w
+
+
+def _create_args(weights, n: int, stage3_band_above: Optional[int], order=None):
+    """(weights argument, options argument, buffers to keep alive) of chd_phys_batch_create / chd_phys_queue_create;
+    `order`: problem i of the call is problems[order[i]]."""
+    per = clip_weights(weights, n)
+    band = -1 if stage3_band_above is None else int(stage3_band_above)   # outside -1..96: refused by the library (-1)
+    if per is None:
+        w = _Weights(*[float(x) for x in weights])
+        opt = None if stage3_band_above is None else _Options(band, None)
+        return C.byref(w), (C.byref(opt) if opt is not None else None), (w, opt)
+    if order is not None:
+        per = per[order]
+    arr = (_Weights * n)(*[_Weights(*[float(x) for x in row]) for row in per])
+    opt = _Options(band, C.cast(arr, C.POINTER(_Weights)))
+    return None, C.byref(opt), (arr, opt)
 
 
 class _Dims(C.Structure):
@@ -85,6 +118,9 @@ SIGNATURES = {
     "chd_phys_get_ent_col": (_int, [_vp, _vp]),
     "chd_phys_get_duals": (_int, [_vp] * 7),
     "chd_phys_stage_stats": (_int, [_vp, _vp]),
+    "chd_phys_get_stage_weights": (_int, [_vp, _vp]),
+    "chd_phys_cost_terms": (_int, [_vp, _vp]),
+    "chd_phys_set_cost_terms_out": (_int, [_vp, _vp]),
     "chd_phys_solve_stage": (_int, [_vp, _i32, _i32, _vp, _vp, _vp]),
     "chd_phys_solve": (_int, [_vp] * 6),
     "chd_phys_sample": (_int, [_vp, _vp, _vp]),
@@ -184,21 +220,21 @@ def make_problem_array(problems):
 
 
 class PhysBatch:
-    """`stage3_band_above`: sequences with more phase-duration variables than this carry their switch times as banded
-    KKT unknowns, which lets stage 3 run beyond the 96 the dense border holds (0 bands every sequence; None: none)."""
+    """`weights`: one 5-tuple (w_com_lin, w_com_ang, w_ee, w_smooth, w_dur) for every sequence, or one per sequence
+    (`clip_weights`).  `stage3_band_above`: sequences with more phase-duration variables than this carry their switch
+    times as banded KKT unknowns, which lets stage 3 run beyond the 96 the dense border holds (0 bands every sequence;
+    None: none)."""
 
-    def __init__(self, problems: Sequence[PhysProblem], weights=(0.4, 1.7, 0.3, 0.1, 0.1), device: int = -1,
+    def __init__(self, problems: Sequence[PhysProblem], weights=DEFAULT_WEIGHTS, device: int = -1,
                  host_only: bool = False, stage3_band_above: Optional[int] = None):
         self.L = load_lib()
         self.problems = list(problems)
         B = len(self.problems)
         arr, self._keep = make_problem_array(self.problems)
-        w = _Weights(*[float(x) for x in weights])
+        w, opt, _ = _create_args(weights, B, stage3_band_above)
         h = C.c_void_p()
         dev = -2 if host_only else device
-        # values outside 0..96 are rejected by the library (code -1)
-        opt = None if stage3_band_above is None else C.byref(_Options(int(stage3_band_above)))
-        rc = self.L.chd_phys_batch_create(arr, B, C.byref(w), dev, opt, C.byref(h))
+        rc = self.L.chd_phys_batch_create(arr, B, w, dev, opt, C.byref(h))
         if rc != 0:
             raise RuntimeError("chd_phys_batch_create failed with code %d (no CUDA device? no CPU fallback exists)" % rc)
         self.h = h
@@ -276,6 +312,19 @@ class PhysBatch:
         self._chk(self.L.chd_phys_stage_stats(self.h, _ptr(out)))
         return out
 
+    def stage_weights(self) -> np.ndarray:
+        """(B, 6, 10): the cost weights of every sequence's six stages: w_data, w_vel, w_acc (base lin, base ang, feet
+        each) and w_dur, so that a stage's cost is `cost_terms() @ stage_weights()[:, stage]` row by row."""
+        out = np.zeros((self.B, 6, 10))
+        self._chk(self.L.chd_phys_get_stage_weights(self.h, _ptr(out)))
+        return out
+
+    def cost_terms(self) -> np.ndarray:
+        """(B, 10): the unweighted cost terms at the current x, columns `COST_TERMS` (chd_phys_cost_terms)."""
+        out = np.zeros((self.B, len(COST_TERMS)))
+        self._chk(self.L.chd_phys_cost_terms(self.h, _ptr(out)))
+        return out
+
     def slot_index(self) -> dict:
         """Column-oriented view of the Jacobian slots: ent_row (B,slots_max), col_ptr (B,n_max+1), col_ent (B,slots_max)."""
         B, d = self.B, self.dims
@@ -313,16 +362,21 @@ class PhysBatch:
         return dict(status=st, iters=it, f=stats[:, 0], E0=stats[:, 1], viol=stats[:, 2], dual=stats[:, 3],
                     compl=stats[:, 4], mu=stats[:, 5], delta_w=stats[:, 6], ls_fail=stats[:, 7])
 
-    def solve(self) -> dict:
-        """Full staged schedule.  Returns the three SaveSolution snapshots, frame counts, success flags."""
+    def solve(self, cost_terms: bool = False) -> dict:
+        """Full staged schedule.  Returns the three SaveSolution snapshots, frame counts, success flags; with
+        `cost_terms` also `cost_terms` (B, 10): the unweighted cost terms (`COST_TERMS`) of every final iterate."""
         B, d = self.B, self.dims
         samples = np.zeros((3, B, d["frames_out_max"], sample_stride(self.n_ee_max)))
         frames = np.zeros(B, np.int32)
         success = np.zeros((B, 2), np.int32)
         sstat = np.zeros((6, B), np.int32)
         siter = np.zeros((6, B), np.int32)
-        self._chk(self.L.chd_phys_solve(self.h, _ptr(samples), _ptr(frames), _ptr(success), _ptr(sstat), _ptr(siter)))
-        return dict(samples=samples, frames=frames, success=success, stage_status=sstat, stage_iters=siter)
+        out = dict(samples=samples, frames=frames, success=success, stage_status=sstat, stage_iters=siter)
+        with _terms_out(self, B, cost_terms) as terms:
+            self._chk(self.L.chd_phys_solve(self.h, _ptr(samples), _ptr(frames), _ptr(success), _ptr(sstat), _ptr(siter)))
+        if terms is not None:
+            out["cost_terms"] = terms
+        return out
 
     def sample(self):
         B, d = self.B, self.dims
@@ -355,6 +409,23 @@ class PhysBatch:
             raise RuntimeError("libchd call failed with code %d" % rc)
 
 
+class _terms_out:
+    """Points the handle's cost-terms output (chd_phys_set_cost_terms_out) at a fresh (n, 10) array for one solve, and
+    back to NULL afterwards, so that the library never holds a pointer into freed memory."""
+
+    def __init__(self, obj, n: int, on: bool):
+        self.obj, self.terms = obj, (np.zeros((n, len(COST_TERMS))) if on else None)
+
+    def __enter__(self):
+        if self.terms is not None:
+            self.obj._chk(self.obj.L.chd_phys_set_cost_terms_out(self.obj.h, _ptr(self.terms)))
+        return self.terms
+
+    def __exit__(self, *exc):
+        if self.terms is not None:
+            self.obj.L.chd_phys_set_cost_terms_out(self.obj.h, None)
+
+
 class PhysQueue:
     """Any number of clips solved through `slots` device slots: a slot takes the next clip as soon as its clip has
     finished, so device memory scales with `slots` and the slowest clip's tail is paid once per queue rather than once
@@ -369,9 +440,11 @@ class PhysQueue:
     (0 <= k <= want; fewer than asked: nothing is left).  Queue positions are the `work_estimate` order (`order`), which
     is the same in every process that holds the same problem list, so processes that share one source
     (`chd.parallel.StoreClaim`) split the clips between them.  Only the clips handed out are solved: `solved` marks
-    them, the other clips' rows stay zero."""
+    them, the other clips' rows stay zero.
 
-    def __init__(self, problems: Sequence[PhysProblem], slots: int, weights=(0.4, 1.7, 0.3, 0.1, 0.1), device: int = -1,
+    `weights`: as `PhysBatch`'s, one 5-tuple per problem in input order (each clip keeps its own through every slot)."""
+
+    def __init__(self, problems: Sequence[PhysProblem], slots: int, weights=DEFAULT_WEIGHTS, device: int = -1,
                  stage3_band_above: Optional[int] = None, claim=None):
         from .parallel import work_estimate
         self.L = load_lib()
@@ -380,10 +453,9 @@ class PhysQueue:
         # queue position k holds problems[order[k]]; stable, so equal estimates keep their input order
         self.order = np.argsort(-np.asarray(work_estimate(self.problems), dtype=np.float64), kind="stable")
         arr, self._keep = make_problem_array([self.problems[i] for i in self.order])
-        w = _Weights(*[float(x) for x in weights])
-        opt = None if stage3_band_above is None else C.byref(_Options(int(stage3_band_above)))
+        w, opt, _ = _create_args(weights, N, stage3_band_above, self.order)
         h = C.c_void_p()
-        rc = self.L.chd_phys_queue_create(arr, N, int(slots), C.byref(w), device, opt, C.byref(h))
+        rc = self.L.chd_phys_queue_create(arr, N, int(slots), w, device, opt, C.byref(h))
         if rc != 0:
             raise RuntimeError("chd_phys_queue_create failed with code %d" % rc)
         self.h = h
@@ -431,17 +503,19 @@ class PhysQueue:
         except Exception:
             pass
 
-    def solve(self) -> dict:
+    def solve(self, cost_terms: bool = False) -> dict:
         """Full staged schedule of every clip (with `claim`: of the clips it hands out); the same keys and shapes as
-        `PhysBatch.solve()` for N sequences, plus stage_stats (6, N, 4) (`PhysBatch.stage_stats`) and solved (N bools)."""
+        `PhysBatch.solve()` for N sequences (`cost_terms` included), plus stage_stats (6, N, 4)
+        (`PhysBatch.stage_stats`) and solved (N bools)."""
         N, d = self.N, self.dims
         out = dict(samples=np.zeros((3, N, d["frames_out_max"], sample_stride(self.n_ee_max))),
                    frames=np.zeros(N, np.int32), success=np.zeros((N, 2), np.int32),
                    stage_status=np.zeros((6, N), np.int32), stage_iters=np.zeros((6, N), np.int32),
                    stage_stats=np.zeros((6, N, 4)))
         self._claimed, self._claim_error = [], None
-        rc = self.L.chd_phys_queue_solve(self.h, *[_ptr(out[k]) for k in ("samples", "frames", "success", "stage_status",
-                                                                          "stage_iters", "stage_stats")])
+        with _terms_out(self, N, cost_terms) as terms:
+            rc = self.L.chd_phys_queue_solve(self.h, *[_ptr(out[k]) for k in ("samples", "frames", "success",
+                                                                              "stage_status", "stage_iters", "stage_stats")])
         if self._claim_error is not None:
             e, self._claim_error = self._claim_error, None
             raise RuntimeError("the claim source of the queue failed") from e
@@ -453,12 +527,18 @@ class PhysQueue:
             for f, k in self._claimed:
                 solved[f:f + k] = True
         out["solved"] = solved
+        if terms is not None:
+            out["cost_terms"] = terms
         inv = np.argsort(self.order)          # queue position of every input clip
-        axis = dict(samples=1, frames=0, success=0, stage_status=1, stage_iters=1, stage_stats=1, solved=0)
+        axis = dict(samples=1, frames=0, success=0, stage_status=1, stage_iters=1, stage_stats=1, solved=0, cost_terms=0)
         return {k: np.take(v, inv, axis=axis[k]) for k, v in out.items()}
 
     def launch_count(self) -> int:
         return int(self.L.chd_phys_launch_count(self.h))
+
+    def _chk(self, rc):
+        if rc != 0:
+            raise RuntimeError("libchd call failed with code %d" % rc)
 
     def h2d_bytes(self) -> int:
         """Bytes uploaded so far: the slots' tables at creation and the records of every admitted clip."""

@@ -62,14 +62,20 @@ typedef struct chd_phys_dims {
  *   stage3_band_above: a sequence with more phase-duration variables than this carries its switch times as banded
  *   KKT unknowns (time ordered with the node values) instead of dense border unknowns, which lifts the limit of 96
  *   that stage 3 otherwise has.  -1: no sequence (the default); 0 .. 96 otherwise.  A banded sequence whose band would
- *   be too wide for the KKT kernels keeps stage 3 off (status -3). */
+ *   be too wide for the KKT kernels keeps stage 3 off (status -3).
+ *   clip_weights: NULL (the default), or [host] one weight tuple per problem (`batch` entries for a batch, `n` for a
+ *   queue), which overrides the `weights` argument: each sequence runs stages 2.1, 2.2, 3 and 4 with its own weights
+ *   (stages 1.1 and 1.2 have fixed ones).  A sequence's results are those of a batch of the same problems that all use
+ *   its tuple.  Read during creation only. */
 typedef struct chd_phys_options {
   int32_t stage3_band_above;
+  const chd_phys_weights* clip_weights;
 } chd_phys_options;
 /* Builds the NLP layouts of `batch` sequences on the host and uploads them to the current CUDA device.
- * device < 0 keeps the current device.  weights and opt may be NULL: the defaults.  Returns -1 for a bad argument or an
- * option out of range, -5 when the batch's KKT band + border does not fit the factorisation kernels.  The length of a
- * sequence is not limited otherwise: iterates too long for shared memory are evaluated from global memory. */
+ * device < 0 keeps the current device.  weights and opt may be NULL: the defaults.  Returns -1 for a bad argument, an
+ * option out of range or a weight that is negative or not finite (checked before any device work), -5 when the batch's
+ * KKT band + border does not fit the factorisation kernels.  The length of a sequence is not limited otherwise:
+ * iterates too long for shared memory are evaluated from global memory. */
 int chd_phys_batch_create(const chd_phys_problem* problems, int32_t batch, const chd_phys_weights* weights,
                           int32_t device, const chd_phys_options* opt, chd_phys_batch** out);
 void chd_phys_batch_destroy(chd_phys_batch* b);
@@ -114,6 +120,27 @@ int chd_phys_get_ent_col(const chd_phys_batch* b, int32_t* ent_col);
  * (what IpoptCalculatedQuantities reports as the scaled multipliers; unscaled y = y * row_scale / obj_scale). */
 int chd_phys_get_duals(const chd_phys_batch* b, double* y, double* zL, double* zU, double* s, double* row_scale,
                        double* obj_scale);
+/* Cost weights of every sequence's six stages as the solver uses them: [host] batch x 6 x 10 doubles, per stage
+ * w_data (base lin, base ang, feet), w_vel (same order), w_acc (same order), w_dur.  A queue handle: of its first
+ * `slots` clips, like the other layout queries.  Works on host-only layouts. */
+int chd_phys_get_stage_weights(const chd_phys_batch* b, double* w);
+
+/* The unweighted cost terms at the current x: terms [host] batch x CHD_PHYS_N_TERMS doubles, per sequence
+ *   0-2 data fit (data_cost.cpp) of the base position, the base orientation, the feet (summed over end-effectors),
+ *   3-5 velocity smoothing (vel_smooth_cost.cpp, position differences) in the same order,
+ *   6-8 acceleration smoothing (velocity differences) in the same order,
+ *   9   duration change (duration_cost.cpp; 0 for a sequence without free phase durations),
+ * each with weight 1, all ten whatever the stage (after stage 3, on the spline tables of the moved durations).  So
+ * the cost chd_phys_eval reports for a stage is the sum of these terms times that stage's weights
+ * (chd_phys_get_stage_weights).  A sequence's terms are bitwise the same from call to call.  -1 on a queue handle. */
+enum { CHD_PHYS_N_TERMS = 10 };
+int chd_phys_cost_terms(chd_phys_batch* b, double* terms);
+/* Opt-in: every later chd_phys_solve / chd_phys_queue_solve also writes each clip's cost terms (chd_phys_cost_terms) at
+ * its final iterate, the one of the durations snapshot, to terms [host] batch (a queue: n) x CHD_PHYS_N_TERMS, indexed
+ * like the other outputs (a queue takes them from a finished slot before its next clip is admitted).  NULL, the
+ * default, turns it off; a solve then issues no extra launch or copy.  The buffer must stay valid while solves run. */
+int chd_phys_set_cost_terms_out(chd_phys_batch* b, double* terms);
+
 /* Residuals of every stage of the last chd_phys_solve / chd_phys_solve_stage: stats [host] 6 x batch x 4 =
  * objective, scaled NLP error E0 (IPOPT's overall error, tol 1e-3), unscaled max constraint violation
  * (constr_viol_tol 1e-4), unscaled dual infeasibility. */

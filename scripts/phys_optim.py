@@ -7,7 +7,8 @@ Extension: `--in_dir` / `--out_dir` / `--nframes` accept comma separated lists s
 batch (that is where the GPU pays off); `--n_ee 2` selects the toes-only parameterisation; `--slots S` solves the list
 through a queue of S device slots (`chd.phys.PhysQueue`: memory for S clips, each slot refilled as its clip finishes).
 Under torchrun, `--slots S` runs such a queue on every rank's GPU, the ranks claiming their next clips from one shared
-counter (`chd.parallel.ShardedSolver(slots=S)`), and rank 0 writes the four files of every clip.
+counter (`chd.parallel.ShardedSolver(slots=S)`), and rank 0 writes the four files of every clip.  Every `--w_*` flag takes
+one value for all clips or a comma separated list aligned with `--in_dir`, one value per clip.
 """
 import argparse
 import os
@@ -28,16 +29,31 @@ def write_results(out, problems, out_dirs, n_ee_max):
         print("[%d] stages status %s iterations %s -> %s" % (i, out["stage_status"][:, i].tolist(), out["stage_iters"][:, i].tolist(), od))
 
 
+WEIGHT_FLAGS = ("w_com_lin", "w_com_ang", "w_ee", "w_smooth", "w_dur")
+WEIGHT_DEFAULTS = ("0.4", "1.7", "0.3", "0.1", "0.1")   # phys_optim.cpp:27-31
+
+
+def parse_weights(args, n):
+    """The `--w_*` flags as the solvers take them: one 5-tuple when every flag holds a single value, else one 5-tuple
+    per clip, a single value standing for every clip.  A list whose length is not n raises ValueError."""
+    cols = []
+    for k in WEIGHT_FLAGS:
+        v = [float(x) for x in str(getattr(args, k)).split(",")]
+        if len(v) not in (1, n):
+            raise ValueError("--%s: %d values for %d clips" % (k, len(v), n))
+        cols.append(v)
+    if all(len(v) == 1 for v in cols):
+        return tuple(v[0] for v in cols)
+    return [tuple(v[i] if len(v) > 1 else v[0] for v in cols) for i in range(n)]
+
+
 def main(argv=None):
     ap = argparse.ArgumentParser(allow_abbrev=False)
     ap.add_argument("--out_dir", default="sol_out")
     ap.add_argument("--in_dir", default="./")
     ap.add_argument("--nframes", default="100")
-    ap.add_argument("--w_com_lin", type=float, default=0.4)
-    ap.add_argument("--w_com_ang", type=float, default=1.7)
-    ap.add_argument("--w_ee", type=float, default=0.3)
-    ap.add_argument("--w_smooth", type=float, default=0.1)
-    ap.add_argument("--w_dur", type=float, default=0.1)
+    for k, v in zip(WEIGHT_FLAGS, WEIGHT_DEFAULTS):
+        ap.add_argument("--" + k, default=v, help="one value, or one per clip (comma separated)")
     ap.add_argument("--n_ee", type=int, default=4)
     ap.add_argument("--stage3_long", action="store_true",
                     help="run stage 3 on sequences with more than 96 phase durations too (switch times as band unknowns)")
@@ -52,9 +68,12 @@ def main(argv=None):
         nframes = nframes * len(in_dirs)
     assert len(in_dirs) == len(out_dirs) == len(nframes)
     print("Out Dir: %s\nInput Directory: %s\nnum frames: %s" % (args.out_dir, args.in_dir, args.nframes))
-    print("Optim weights (%g, %g, %g, %g)\nDuration cost weight %g" % (args.w_com_lin, args.w_com_ang, args.w_ee, args.w_smooth, args.w_dur))
+    weights = parse_weights(args, len(in_dirs))
+    if isinstance(weights, tuple):
+        print("Optim weights (%g, %g, %g, %g)\nDuration cost weight %g" % weights)
+    else:
+        print("Optim weights (%s, %s, %s, %s)\nDuration cost weight %s" % tuple(getattr(args, k) for k in WEIGHT_FLAGS))
     problems = [chd.io_formats.read_phys_inputs(d, f, n_ee=args.n_ee) for d, f in zip(in_dirs, nframes)]
-    weights = (args.w_com_lin, args.w_com_ang, args.w_ee, args.w_smooth, args.w_dur)
     band = 96 if args.stage3_long else None
     world, rank, local = int(os.environ.get("WORLD_SIZE", 1)), int(os.environ.get("RANK", 0)), int(os.environ.get("LOCAL_RANK", 0))
     if world > 1 and args.slots:
