@@ -80,7 +80,12 @@ struct ChdQueue {
   void* claim_ctx = nullptr;
   bool exhausted = false;             // the source returned fewer positions than asked during this solve
   std::vector<char> given;            // positions the source handed out during this solve
-  // outputs of the running chd_phys_queue_solve, indexed by clip
+};
+
+// Outputs of the running chd_phys_solve / chd_phys_queue_solve (NULL: not asked for), indexed by sequence (a queue: by
+// clip) with n sequences (clips) per stage row.
+struct ChdSolveOut {
+  size_t n = 0;
   double *samples = nullptr, *stage_stats = nullptr, *terms = nullptr;
   int32_t *frames = nullptr, *success = nullptr, *stage_status = nullptr, *stage_iters = nullptr;
 };
@@ -115,9 +120,29 @@ struct chd_phys_batch {
   double *poly_T0 = nullptr, *poly_tend0 = nullptr, *phase_tend0 = nullptr;
   int* ent_col0 = nullptr;
   ChdQueue* queue = nullptr;   // a queue handle: the batch's sequences are slots that clips pass through
+  ChdSolveOut out;
 };
 
 namespace {
+
+// the staged schedule of a full solve (phys_optim.cpp:554-749)
+const int full_schedule[6] = {CHD_STAGE_11, CHD_STAGE_12, CHD_STAGE_21, CHD_STAGE_22, CHD_STAGE_3, CHD_STAGE_4};
+
+// doubles of a SaveSolution sample row (chd.phys.sample_stride)
+size_t sample_stride(const ChdHostBatch& hb) { return 6 + 7 * (size_t)hb.n_ee_max; }
+
+// success flags, stage statuses, iterations and (when asked for) stage statistics of sequence (clip) c from its solver
+// state
+void write_status(const ChdSolveOut& o, size_t c, const ChdIpm& I) {
+  // dynamics_succeed (:655); durations_succeed = stage 3 (:709), overwritten by stage 4 when that had to run (:746)
+  if (o.success) o.success[2 * c] = I.st_status[CHD_STAGE_22] == 0, o.success[2 * c + 1] = I.st_status[CHD_STAGE_3] == 0 || I.st_status[CHD_STAGE_4] == 0;
+  for (size_t s = 0; s < 6; ++s) {
+    if (o.stage_status) o.stage_status[s * o.n + c] = I.st_status[s];
+    if (o.stage_iters) o.stage_iters[s * o.n + c] = I.st_iters[s];
+    if (o.stage_stats)
+      for (int k = 0; k < 4; ++k) o.stage_stats[(s * o.n + c) * 4 + k] = I.st_stat[s][k];
+  }
+}
 
 template <class T>
 int dev_upload(chd_phys_batch* b, const std::vector<T>& v, const T** out) {
@@ -354,7 +379,7 @@ int queue_device(chd_phys_batch* b, int sms) {
   for (const double* p : {D.sol, D.rhs0, D.rhs1}) seg(p, kb, -1);
   if (D.scratch) seg(D.scratch, D.scratch_stride * sizeof(double), -1);
   seg(b->d_frames, sizeof(int), -1);
-  const size_t snap = (size_t)hb.fo_max * (6 + 7 * (size_t)hb.n_ee_max) * sizeof(double);
+  const size_t snap = hb.fo_max * sample_stride(hb) * sizeof(double);
   for (int s = 0; s < 3; ++s) {
     // the three SaveSolution snapshots are 3 x B x fo_max x stride: one row per slot in each
     if (A.nseg == CHD_ADMIT_SEGS) ok = false;
@@ -415,23 +440,17 @@ int queue_harvest(chd_phys_batch* b, int slot) {
   const int c = q.clip[slot];
   if (c < 0) return 0;
   const ChdHostBatch& hb = b->hb;
-  const size_t S = hb.B, n = q.n, row = (size_t)hb.fo_max * (6 + 7 * (size_t)hb.n_ee_max);
-  if (q.samples)
+  const ChdSolveOut& o = b->out;
+  const size_t S = hb.B, row = hb.fo_max * sample_stride(hb);
+  if (o.samples)
     for (size_t s = 0; s < 3; ++s)
-      CHD_CUDA(cudaMemcpyAsync(q.samples + (s * n + c) * row, b->D.snapshots + (s * S + slot) * row, row * sizeof(double),
+      CHD_CUDA(cudaMemcpyAsync(o.samples + (s * o.n + c) * row, b->D.snapshots + (s * S + slot) * row, row * sizeof(double),
                                cudaMemcpyDeviceToHost, b->stream));
-  if (q.frames) CHD_CUDA(cudaMemcpyAsync(q.frames + c, b->d_frames + slot, sizeof(int), cudaMemcpyDeviceToHost, b->stream));
-  if (q.terms)
-    CHD_CUDA(cudaMemcpyAsync(q.terms + (size_t)c * CHD_PHYS_N_TERMS, b->d_terms + (size_t)slot * CHD_PHYS_N_TERMS,
+  if (o.frames) CHD_CUDA(cudaMemcpyAsync(o.frames + c, b->d_frames + slot, sizeof(int), cudaMemcpyDeviceToHost, b->stream));
+  if (o.terms)
+    CHD_CUDA(cudaMemcpyAsync(o.terms + (size_t)c * CHD_PHYS_N_TERMS, b->d_terms + (size_t)slot * CHD_PHYS_N_TERMS,
                              CHD_PHYS_N_TERMS * sizeof(double), cudaMemcpyDeviceToHost, b->stream));
-  const ChdIpm& I = b->h_ipm[slot];
-  if (q.success) q.success[2 * c] = I.st_status[CHD_STAGE_22] == 0, q.success[2 * c + 1] = I.st_status[CHD_STAGE_3] == 0 || I.st_status[CHD_STAGE_4] == 0;
-  for (size_t s = 0; s < 6; ++s) {
-    if (q.stage_status) q.stage_status[s * n + c] = I.st_status[s];
-    if (q.stage_iters) q.stage_iters[s * n + c] = I.st_iters[s];
-    if (q.stage_stats)
-      for (int k = 0; k < 4; ++k) q.stage_stats[(s * n + c) * 4 + k] = I.st_stat[s][k];
-  }
+  write_status(o, c, b->h_ipm[slot]);
   q.clip[slot] = -1;
   return 0;
 }
@@ -451,7 +470,7 @@ int queue_refill(chd_phys_batch* b, int it, int* last_it) {
   if (q.claim && (rc = queue_claim(b, k, &first, &k))) return rc;
   // this iteration's side-stream kernels (chd_k_kcopy, chd_k_curv, chd_k_hess_dur) may still read the slots' state
   CHD_CUDA(cudaStreamWaitEvent(b->stream, b->ev_copy, 0));
-  if (q.terms) launch_cost_terms(b, 1);   // before admission overwrites the finished slots
+  if (b->out.terms) launch_cost_terms(b, 1);   // before admission overwrites the finished slots
   for (int s : freed)
     if ((rc = queue_harvest(b, s))) return rc;
   if (k == 0) return 0;
@@ -634,7 +653,7 @@ static int batch_create_impl(const chd_phys_problem* problems, int32_t batch, in
   CHD_CUDA(cudaFuncSetAttribute(b->iter.eval, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)b->iter.smem_eval));
   CHD_CUDA(cudaFuncSetAttribute(P.win_smem ? chd_k_kkt : chd_k_kkt_gwin, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)b->smem_kkt));
   CHD_CUDA(cudaFuncSetAttribute(b->iter.linesearch, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)b->iter.smem_ls));
-  const size_t stride = 6 + 7 * (size_t)hb.n_ee_max;
+  const size_t stride = sample_stride(hb);
   CHD_CUDA(cudaMallocAsync((void**)&b->d_samples, B * hb.fo_max * stride * sizeof(double), b->stream));
   CHD_CUDA(cudaMallocAsync((void**)&b->d_frames, B * sizeof(int), b->stream));
   b->allocs.push_back(b->d_samples);
@@ -842,7 +861,7 @@ int chd_phys_sample_device(chd_phys_batch* b, double* out_device, void* stream) 
 int chd_phys_sample(chd_phys_batch* b, double* out, int32_t* frames_out) {
   if (!b || !out || b->host_only || b->queue) return -1;
   const ChdHostBatch& hb = b->hb;
-  const size_t stride = 6 + 7 * (size_t)hb.n_ee_max, cnt = (size_t)hb.B * hb.fo_max * stride;
+  const size_t cnt = (size_t)hb.B * hb.fo_max * sample_stride(hb);
   CHD_CUDA(cudaMemsetAsync(b->d_samples, 0, cnt * sizeof(double), b->stream));
   int rc = chd_phys_sample_device(b, b->d_samples, nullptr);
   if (rc) return rc;
@@ -861,26 +880,20 @@ int chd_phys_solve(chd_phys_batch* b, double* samples, int32_t* frames_out, int3
   if (!b || b->host_only || b->queue) return -1;
   const ChdHostBatch& hb = b->hb;
   const int B = hb.B;
-  const size_t stride = 6 + 7 * (size_t)hb.n_ee_max, snap = (size_t)B * hb.fo_max * stride;
-  int sched[6] = {CHD_STAGE_11, CHD_STAGE_12, CHD_STAGE_21, CHD_STAGE_22, CHD_STAGE_3, CHD_STAGE_4};
-  int rc = set_schedule(b, sched, 6, -1, 0);
+  const size_t snap = (size_t)B * hb.fo_max * sample_stride(hb);
+  int rc = set_schedule(b, full_schedule, 6, -1, 0);
   if (rc) return rc;
-  if (samples) CHD_CUDA(cudaMemsetAsync(b->D.snapshots, 0, 3 * snap * sizeof(double), b->stream));
+  b->out = {(size_t)B, samples, nullptr, b->terms_out, frames_out, success, stage_status, stage_iters};
+  const ChdSolveOut& o = b->out;
+  if (o.samples) CHD_CUDA(cudaMemsetAsync(b->D.snapshots, 0, 3 * snap * sizeof(double), b->stream));
   if ((rc = run_schedule(b))) return rc;
-  for (int i = 0; i < B; ++i) {
-    const ChdIpm& I = b->h_ipm[i];
-    // dynamics_succeed (:655); durations_succeed = stage 3 (:709), overwritten by stage 4 when that had to run (:746)
-    if (success) success[2 * i] = I.st_status[CHD_STAGE_22] == 0, success[2 * i + 1] = I.st_status[CHD_STAGE_3] == 0 || I.st_status[CHD_STAGE_4] == 0;
-    for (int s = 0; s < 6; ++s) {
-      if (stage_status) stage_status[(size_t)s * B + i] = I.st_status[s];
-      if (stage_iters) stage_iters[(size_t)s * B + i] = I.st_iters[s];
-    }
-  }
-  if (samples) CHD_CUDA(cudaMemcpyAsync(samples, b->D.snapshots, 3 * snap * sizeof(double), cudaMemcpyDeviceToHost, b->stream));
-  if (frames_out) CHD_CUDA(cudaMemcpyAsync(frames_out, b->d_frames, B * sizeof(int), cudaMemcpyDeviceToHost, b->stream));
-  if (b->terms_out) {   // x is every sequence's final iterate, the one of the durations snapshot
+  for (int i = 0; i < B; ++i) write_status(o, i, b->h_ipm[i]);
+  // one copy of every sequence's snapshots, frame counts and cost terms
+  if (o.samples) CHD_CUDA(cudaMemcpyAsync(o.samples, b->D.snapshots, 3 * snap * sizeof(double), cudaMemcpyDeviceToHost, b->stream));
+  if (o.frames) CHD_CUDA(cudaMemcpyAsync(o.frames, b->d_frames, B * sizeof(int), cudaMemcpyDeviceToHost, b->stream));
+  if (o.terms) {   // x is every sequence's final iterate, the one of the durations snapshot
     launch_cost_terms(b, 0);
-    CHD_CUDA(cudaMemcpyAsync(b->terms_out, b->d_terms, (size_t)B * CHD_PHYS_N_TERMS * sizeof(double), cudaMemcpyDeviceToHost, b->stream));
+    CHD_CUDA(cudaMemcpyAsync(o.terms, b->d_terms, (size_t)B * CHD_PHYS_N_TERMS * sizeof(double), cudaMemcpyDeviceToHost, b->stream));
   }
   CHD_CUDA(cudaStreamSynchronize(b->stream));
   return 0;
@@ -901,10 +914,8 @@ int chd_phys_queue_solve(chd_phys_batch* b, double* samples, int32_t* frames_out
     if ((rc = queue_claim(b, S, &first, &k))) return rc;
     if (k == 0) return 0;   // nothing for this handle: no output is touched
   }
-  int sched[6] = {CHD_STAGE_11, CHD_STAGE_12, CHD_STAGE_21, CHD_STAGE_22, CHD_STAGE_3, CHD_STAGE_4};
-  if ((rc = set_schedule(b, sched, 6, -1, 0))) return rc;
-  q.samples = samples, q.frames = frames_out, q.success = success, q.stage_status = stage_status;
-  q.stage_iters = stage_iters, q.stage_stats = stage_stats, q.terms = b->terms_out;
+  if ((rc = set_schedule(b, full_schedule, 6, -1, 0))) return rc;
+  b->out = {(size_t)q.n, samples, stage_stats, b->terms_out, frames_out, success, stage_status, stage_iters};
   q.clip.assign(S, -1);
   std::vector<int> slots(S);
   std::iota(slots.begin(), slots.end(), 0);
@@ -919,7 +930,7 @@ int chd_phys_queue_solve(chd_phys_batch* b, double* samples, int32_t* frames_out
     b->h2d_bytes += (int64_t)(idle.size() * sizeof(ChdIpm));
   }
   if ((rc = run_schedule(b))) return rc;
-  if (q.terms) launch_cost_terms(b, 0);
+  if (b->out.terms) launch_cost_terms(b, 0);
   for (int i = 0; i < S; ++i)
     if ((rc = queue_harvest(b, i))) return rc;
   CHD_CUDA(cudaStreamSynchronize(b->stream));

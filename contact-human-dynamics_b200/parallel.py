@@ -60,7 +60,9 @@ def unshard(gathered: np.ndarray, shards: List[List[int]], slots: int) -> np.nda
 # ---------------------------------------------------------------------------------------------------------------------
 # The product's multi-GPU entry point: shard -> solve -> sample into the send buffer -> ONE gather -> unshard.
 # ---------------------------------------------------------------------------------------------------------------------
-N_EXTRA = 16  # per-sequence trailer of the gathered block: frames, success[2], stage_status[6], stage_iters[6], pad
+# per-sequence trailer of the gathered block: these fields (`phys.pack_rows`, 15 columns), zero-padded to N_EXTRA
+TRAILER_KEYS = ("frames", "success", "stage_status", "stage_iters")
+N_EXTRA = 16
 
 
 def work_estimate(problems) -> List[float]:
@@ -94,11 +96,9 @@ class StoreClaim:
         return lo, hi - lo
 
 
-# Row of a rank's block in the merge of queue results (merge_solved): clip index, the three SaveSolution snapshots
-# (3 x fo x stride), then frames, success[2], stage_status[6], stage_iters[6], stage_stats[6 x 4] and, when the results
-# carry them, the cost terms[10].
-Q_EXTRA = 1 + 2 + 6 + 6 + 24
-Q_TERMS = len(phys.COST_TERMS)
+# Fields of a row of a rank's block in the merge of queue results (merge_solved), after the clip index
+# (`phys.pack_rows`); the cost terms follow when the results carry them.
+MERGE_KEYS = phys.SOLVE_KEYS + ("stage_stats",)
 
 
 def merge_solved(local: dict, world: int, group=None, tensor_device=None) -> dict:
@@ -115,11 +115,11 @@ def merge_solved(local: dict, world: int, group=None, tensor_device=None) -> dic
     import torch.distributed as dist
     dev = tensor_device or torch.device("cpu")
     _, N, fo, stride = local["samples"].shape
-    snap = 3 * fo * stride
-    terms = "cost_terms" in local
-    width = 1 + snap + Q_EXTRA + (Q_TERMS if terms else 0)
+    keys = MERGE_KEYS + (("cost_terms",) if "cost_terms" in local else ())
     mine = np.nonzero(local["solved"])[0]
     n = len(mine)
+    packed = phys.pack_rows(local, keys, mine)
+    width = 1 + packed.shape[1]
     collective = world > 1 and dist.is_initialized()
     counts = torch.tensor([n], dtype=torch.int64, device=dev)
     if collective:
@@ -129,15 +129,7 @@ def merge_solved(local: dict, world: int, group=None, tensor_device=None) -> dic
     cmax = int(counts.max())
     blk = np.zeros((cmax, width))
     blk[:n, 0] = mine
-    blk[:n, 1:1 + snap] = local["samples"][:, mine].transpose(1, 0, 2, 3).reshape(n, snap)
-    tr = blk[:n, 1 + snap:]
-    tr[:, 0] = local["frames"][mine]
-    tr[:, 1:3] = local["success"][mine]
-    tr[:, 3:9] = local["stage_status"][:, mine].T
-    tr[:, 9:15] = local["stage_iters"][:, mine].T
-    tr[:, 15:39] = local["stage_stats"][:, mine].transpose(1, 0, 2).reshape(n, 24)
-    if terms:
-        tr[:, 39:39 + Q_TERMS] = local["cost_terms"][mine]
+    blk[:n, 1:] = packed
     g = blk
     if collective and cmax > 0:
         send = torch.from_numpy(blk).to(dev)
@@ -149,20 +141,10 @@ def merge_solved(local: dict, world: int, group=None, tensor_device=None) -> dic
     idx = rows[:, 0].astype(np.int64)
     if len(np.unique(idx)) != len(idx) or (len(idx) and (idx.min() < 0 or idx.max() >= N)):
         raise RuntimeError("merge of queue results: a clip was solved by more than one rank, or a clip index is out of range")
-    tr = rows[:, 1 + snap:]
-    out = dict(samples=np.zeros((3, N, fo, stride)), frames=np.zeros(N, np.int32), success=np.zeros((N, 2), np.int32),
-               stage_status=np.zeros((6, N), np.int32), stage_iters=np.zeros((6, N), np.int32),
-               stage_stats=np.zeros((6, N, 4)), solved=np.zeros(N, bool), solved_by=np.full(N, -1, np.int32))
-    out["samples"][:, idx] = rows[:, 1:1 + snap].reshape(len(idx), 3, fo, stride).transpose(1, 0, 2, 3)
-    out["frames"][idx] = tr[:, 0]
-    out["success"][idx] = tr[:, 1:3]
-    out["stage_status"][:, idx] = tr[:, 3:9].T
-    out["stage_iters"][:, idx] = tr[:, 9:15].T
-    out["stage_stats"][:, idx] = tr[:, 15:39].reshape(len(idx), 6, 4).transpose(1, 0, 2)
-    if terms:
-        out["cost_terms"] = np.zeros((N, Q_TERMS))
-        out["cost_terms"][idx] = tr[:, 39:39 + Q_TERMS]
+    out = phys.result_arrays(N, keys + ("solved",), fo, stride)
+    phys.unpack_rows(rows[:, 1:], out, keys, idx)
     out["solved"][idx] = True
+    out["solved_by"] = np.full(N, -1, np.int32)
     out["solved_by"][idx] = rank_of
     out["d2h_bytes"] = int(g.nbytes)
     return out
@@ -269,14 +251,13 @@ class ShardedSolver:
             f = np.asarray(r["final"])
             blk[:n, :f.shape[1], :f.shape[2]] = f
             self.send[:, :self.fo * self.stride] = torch.from_numpy(blk.reshape(self.slots, -1)).to(self.tdev)
-            frames, success, sstat, siter = r["frames"], r["success"], r["stage_status"], r["stage_iters"]
         else:
             b = self.batch
             if resident:
                 b.reset()
-            B = b.B
-            sstat, siter, success = np.zeros((6, B), np.int32), np.zeros((6, B), np.int32), np.zeros((B, 2), np.int32)
-            b._chk(b.L.chd_phys_solve(b.h, None, None, success.ctypes.data, sstat.ctypes.data, siter.ctypes.data))
+            keys = phys.SOLVE_KEYS[2:]               # the snapshots are sampled below, the frame counts known
+            r = phys.result_arrays(b.B, keys)
+            b._chk(b.L.chd_phys_solve(b.h, None, None, *[r[k].ctypes.data for k in keys]))
             # final iterate sampled on the device straight into the send buffer (no host round trip)
             fo_l, st_l = b.dims["frames_out_max"], phys.sample_stride(b.n_ee_max)
             if fo_l == self.fo and st_l == self.stride:
@@ -293,11 +274,8 @@ class ShardedSolver:
                 blk = torch.zeros((n, self.fo, self.stride), dtype=torch.float64, device=self.tdev)
                 blk[:, :fo_l, :st_l] = tmp
                 self.send[:n, :self.fo * self.stride] = blk.reshape(n, -1)
-            frames = np.array([frames_out(self.problems[i]) for i in self.mine], np.int32)
-        trailer[:n, 0] = frames
-        trailer[:n, 1:3] = np.asarray(success).reshape(n, 2)
-        trailer[:n, 3:9] = np.asarray(sstat).T
-        trailer[:n, 9:15] = np.asarray(siter).T
+            r["frames"] = np.array([frames_out(self.problems[i]) for i in self.mine], np.int32)
+        trailer[:n] = phys.pack_rows(r, TRAILER_KEYS, np.arange(n), N_EXTRA)
         self.send[:, self.fo * self.stride:] = torch.from_numpy(trailer).to(self.tdev)
         return trailer
 
@@ -330,10 +308,11 @@ class ShardedSolver:
         g = g.cpu().numpy()
         full = unshard(g, self.shards, self.slots)
         N = len(self.problems)
-        tr = full[:, self.fo * self.stride:]
-        return dict(samples=full[:, :self.fo * self.stride].reshape(N, self.fo, self.stride), frames=tr[:, 0].astype(np.int32),
-                    success=tr[:, 1:3].astype(np.int32), stage_status=tr[:, 3:9].astype(np.int32).T,
-                    stage_iters=tr[:, 9:15].astype(np.int32).T, d2h_bytes=int(g.nbytes))
+        out = dict(samples=full[:, :self.fo * self.stride].reshape(N, self.fo, self.stride))
+        out.update(phys.result_arrays(N, TRAILER_KEYS))
+        phys.unpack_rows(full[:, self.fo * self.stride:], out, TRAILER_KEYS, np.arange(N))
+        out["d2h_bytes"] = int(g.nbytes)
+        return out
 
 
 def solve_sharded(problems, weights=phys.DEFAULT_WEIGHTS, device: int = 0, rank: int = 0, world: int = 1, group=None,

@@ -43,6 +43,77 @@ def sample_columns(n_ee: int, n_ee_max: int):
             np.arange(6 + 6 * n_ee_max, 6 + 6 * n_ee_max + n_ee))
 
 
+# Every per-clip result a solve can return: name -> (dtype, shape), "N" marking the clip axis ("fo": SaveSolution frames
+# of the longest clip, "stride": `sample_stride`).  The batch, the queue and the merges of `chd.parallel` allocate,
+# reorder, concatenate and pack results through the functions below, so that no caller needs a field's clip axis.
+RESULT_FIELDS = {
+    "samples": (np.float64, (3, "N", "fo", "stride")),   # the three SaveSolution snapshots (SOLUTION_FILES)
+    "frames": (np.int32, ("N",)),
+    "success": (np.int32, ("N", 2)),                     # dynamics, durations (success_log.txt)
+    "stage_status": (np.int32, (6, "N")),
+    "stage_iters": (np.int32, (6, "N")),
+    "stage_stats": (np.float64, (6, "N", 4)),            # `PhysBatch.stage_stats`
+    "cost_terms": (np.float64, ("N", len(COST_TERMS))),
+    "solved": (np.bool_, ("N",)),
+}
+SOLVE_KEYS = ("samples", "frames", "success", "stage_status", "stage_iters")   # chd_phys_solve's outputs, in its order
+
+
+def clip_axis(key: str) -> int:
+    """The clip axis of result field `key`."""
+    return RESULT_FIELDS[key][1].index("N")
+
+
+def result_arrays(n: int, keys, fo: int = 0, stride: int = 0) -> dict:
+    """Zeroed arrays of the result fields `keys` for n clips."""
+    size = dict(N=n, fo=fo, stride=stride)
+    return {k: np.zeros([size.get(s, s) for s in RESULT_FIELDS[k][1]], RESULT_FIELDS[k][0]) for k in keys}
+
+
+def take_clips(res: dict, idx) -> dict:
+    """Every field of `res` for the clips `idx` (an index array: selects or reorders)."""
+    return {k: np.take(v, idx, axis=clip_axis(k)) for k, v in res.items()}
+
+
+def concat_results(parts) -> dict:
+    """Results of consecutive batches as one, clips in batch order; `samples` padded to the largest fo."""
+    fo = max((p["samples"].shape[2] for p in parts if "samples" in p), default=0)
+    pad = lambda k, v: np.pad(v, ((0, 0), (0, 0), (0, fo - v.shape[2]), (0, 0))) if k == "samples" else v
+    return {k: np.concatenate([pad(k, p[k]) for p in parts], axis=clip_axis(k)) for k in parts[0]}
+
+
+def _clips_first(res: dict, key: str) -> np.ndarray:
+    """View of field `key` of `res` with its clip axis first."""
+    return np.moveaxis(res[key], clip_axis(key), 0)
+
+
+def pack_rows(res: dict, keys, idx, width: Optional[int] = None) -> np.ndarray:
+    """Fields `keys` of the clips `idx` as one float64 row per clip: the fields side by side in the order of `keys`, each
+    in C order with its clip axis removed; zero-padded to `width` columns.  Exact: int32 values and -0.0 pass through
+    float64 unchanged, and `unpack_rows` writes them back."""
+    idx = np.asarray(idx, np.int64)
+    blocks = [_clips_first(res, k)[idx] for k in keys]
+    cols = [int(np.prod(b.shape[1:])) for b in blocks]
+    rows = np.zeros((len(idx), sum(cols) if width is None else width))
+    c = 0
+    for b, w in zip(blocks, cols):
+        rows[:, c:c + w] = b.reshape(len(idx), w)
+        c += w
+    return rows
+
+
+def unpack_rows(rows: np.ndarray, res: dict, keys, idx) -> None:
+    """Writes rows packed by `pack_rows(..., keys, ...)` into the clips `idx` of the arrays of `res`; columns after the
+    fields are ignored."""
+    idx = np.asarray(idx, np.int64)
+    c = 0
+    for k in keys:
+        dst = _clips_first(res, k)
+        w = int(np.prod(dst.shape[1:]))
+        dst[idx] = rows[:, c:c + w].reshape((len(idx),) + dst.shape[1:])
+        c += w
+
+
 class _Problem(C.Structure):
     _fields_ = [("n_frames", C.c_int32), ("n_ee", C.c_int32), ("dt", C.c_double),
                 ("hip_left", C.POINTER(C.c_double)), ("hip_right", C.POINTER(C.c_double)),
@@ -219,7 +290,54 @@ def make_problem_array(problems):
     return arr, keep
 
 
-class PhysBatch:
+class _Handle:
+    """A libchd phys handle (`h`, from chd_phys_batch_create or chd_phys_queue_create): its dims, its release and its
+    instrumentation.  `KERNELS`: the kernel groups of chd_phys_kernel_times the handle reports."""
+    KERNELS = ("eval", "kkt", "linesearch", "init", "sample")
+
+    def _read_dims(self):
+        d = _Dims()
+        self.L.chd_phys_get_dims(self.h, C.byref(d))
+        self.dims = {k: getattr(d, k) for k, _ in _Dims._fields_}
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def close(self):
+        if getattr(self, "h", None):
+            self.L.chd_phys_batch_destroy(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def _chk(self, rc):
+        if rc != 0:
+            raise RuntimeError("libchd call failed with code %d" % rc)
+
+    def launch_count(self) -> int:
+        return int(self.L.chd_phys_launch_count(self.h))
+
+    def h2d_bytes(self) -> int:
+        """Bytes uploaded so far: the tables at creation, and in a queue the records of every admitted clip."""
+        return int(self.L.chd_phys_h2d_bytes(self.h))
+
+    def set_timing(self, on: bool):
+        self.L.chd_phys_set_timing(self.h, int(on))
+
+    def kernel_times(self, reset=False):
+        ms, cnt = np.zeros(8), np.zeros(8, np.int64)
+        self.L.chd_phys_kernel_times(self.h, _ptr(ms), _ptr(cnt), int(reset))
+        return {k: (float(ms[i]), int(cnt[i])) for i, k in enumerate(self.KERNELS)}
+
+
+class PhysBatch(_Handle):
     """`weights`: one 5-tuple (w_com_lin, w_com_ang, w_ee, w_smooth, w_dur) for every sequence, or one per sequence
     (`clip_weights`).  `stage3_band_above`: sequences with more phase-duration variables than this carry their switch
     times as banded KKT unknowns, which lets stage 3 run beyond the 96 the dense border holds (0 bands every sequence;
@@ -239,31 +357,12 @@ class PhysBatch:
             raise RuntimeError("chd_phys_batch_create failed with code %d (no CUDA device? no CPU fallback exists)" % rc)
         self.h = h
         self.host_only = host_only
-        d = _Dims()
-        self.L.chd_phys_get_dims(self.h, C.byref(d))
-        self.dims = {k: getattr(d, k) for k, _ in _Dims._fields_}
+        self._read_dims()
         self.B = B
         sz = np.zeros((B, 6), dtype=np.int32)
         self.L.chd_phys_get_sizes(self.h, _ptr(sz))
         self.sizes = sz  # n, m, nslots, Na, nb, w
         self.n_ee_max = max(p.n_ee for p in self.problems)
-
-    def __enter__(self):
-        return self
-
-    def __exit__(self, *exc):
-        self.close()
-
-    def close(self):
-        if getattr(self, "h", None):
-            self.L.chd_phys_batch_destroy(self.h)
-            self.h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
     # ---- iterate -------------------------------------------------------------------------------
     def get_x(self) -> np.ndarray:
@@ -365,15 +464,9 @@ class PhysBatch:
     def solve(self, cost_terms: bool = False) -> dict:
         """Full staged schedule.  Returns the three SaveSolution snapshots, frame counts, success flags; with
         `cost_terms` also `cost_terms` (B, 10): the unweighted cost terms (`COST_TERMS`) of every final iterate."""
-        B, d = self.B, self.dims
-        samples = np.zeros((3, B, d["frames_out_max"], sample_stride(self.n_ee_max)))
-        frames = np.zeros(B, np.int32)
-        success = np.zeros((B, 2), np.int32)
-        sstat = np.zeros((6, B), np.int32)
-        siter = np.zeros((6, B), np.int32)
-        out = dict(samples=samples, frames=frames, success=success, stage_status=sstat, stage_iters=siter)
-        with _terms_out(self, B, cost_terms) as terms:
-            self._chk(self.L.chd_phys_solve(self.h, _ptr(samples), _ptr(frames), _ptr(success), _ptr(sstat), _ptr(siter)))
+        out = result_arrays(self.B, SOLVE_KEYS, self.dims["frames_out_max"], sample_stride(self.n_ee_max))
+        with _terms_out(self, self.B, cost_terms) as terms:
+            self._chk(self.L.chd_phys_solve(self.h, *[_ptr(out[k]) for k in SOLVE_KEYS]))
         if terms is not None:
             out["cost_terms"] = terms
         return out
@@ -385,28 +478,8 @@ class PhysBatch:
         self._chk(self.L.chd_phys_sample(self.h, _ptr(out), _ptr(frames)))
         return out, frames
 
-    # ---- instrumentation -----------------------------------------------------------------------
-    def launch_count(self) -> int:
-        return int(self.L.chd_phys_launch_count(self.h))
-
-    def h2d_bytes(self) -> int:
-        return int(self.L.chd_phys_h2d_bytes(self.h))
-
     def reset(self):
         self._chk(self.L.chd_phys_reset(self.h))
-
-    def set_timing(self, on: bool):
-        self.L.chd_phys_set_timing(self.h, int(on))
-
-    def kernel_times(self, reset=False):
-        ms, cnt = np.zeros(8), np.zeros(8, np.int64)
-        self.L.chd_phys_kernel_times(self.h, _ptr(ms), _ptr(cnt), int(reset))
-        names = ["eval", "kkt", "linesearch", "init", "sample"]
-        return {k: (float(ms[i]), int(cnt[i])) for i, k in enumerate(names)}
-
-    def _chk(self, rc):
-        if rc != 0:
-            raise RuntimeError("libchd call failed with code %d" % rc)
 
 
 class _terms_out:
@@ -414,7 +487,7 @@ class _terms_out:
     back to NULL afterwards, so that the library never holds a pointer into freed memory."""
 
     def __init__(self, obj, n: int, on: bool):
-        self.obj, self.terms = obj, (np.zeros((n, len(COST_TERMS))) if on else None)
+        self.obj, self.terms = obj, (result_arrays(n, ("cost_terms",))["cost_terms"] if on else None)
 
     def __enter__(self):
         if self.terms is not None:
@@ -426,7 +499,7 @@ class _terms_out:
             self.obj.L.chd_phys_set_cost_terms_out(self.obj.h, None)
 
 
-class PhysQueue:
+class PhysQueue(_Handle):
     """Any number of clips solved through `slots` device slots: a slot takes the next clip as soon as its clip has
     finished, so device memory scales with `slots` and the slowest clip's tail is paid once per queue rather than once
     per batch.  The clips enter in descending `chd.parallel.work_estimate` order (the longest first, so that the queue's
@@ -443,6 +516,7 @@ class PhysQueue:
     them, the other clips' rows stay zero.
 
     `weights`: as `PhysBatch`'s, one 5-tuple per problem in input order (each clip keeps its own through every slot)."""
+    KERNELS = _Handle.KERNELS + ("admit",)
 
     def __init__(self, problems: Sequence[PhysProblem], slots: int, weights=DEFAULT_WEIGHTS, device: int = -1,
                  stage3_band_above: Optional[int] = None, claim=None):
@@ -459,9 +533,7 @@ class PhysQueue:
         if rc != 0:
             raise RuntimeError("chd_phys_queue_create failed with code %d" % rc)
         self.h = h
-        d = _Dims()
-        self.L.chd_phys_get_dims(self.h, C.byref(d))
-        self.dims = {k: getattr(d, k) for k, _ in _Dims._fields_}
+        self._read_dims()
         self.N, self.slots = N, self.dims["batch"]
         self.n_ee_max = max(p.n_ee for p in self.problems)
         self.claim, self._claimed, self._claim_error = claim, [], None
@@ -486,41 +558,20 @@ class PhysQueue:
             self._claimed.append((f, k))
         return k
 
-    def __enter__(self):
-        return self
-
-    def __exit__(self, *exc):
-        self.close()
-
-    def close(self):
-        if getattr(self, "h", None):
-            self.L.chd_phys_batch_destroy(self.h)
-            self.h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
     def solve(self, cost_terms: bool = False) -> dict:
         """Full staged schedule of every clip (with `claim`: of the clips it hands out); the same keys and shapes as
         `PhysBatch.solve()` for N sequences (`cost_terms` included), plus stage_stats (6, N, 4)
         (`PhysBatch.stage_stats`) and solved (N bools)."""
-        N, d = self.N, self.dims
-        out = dict(samples=np.zeros((3, N, d["frames_out_max"], sample_stride(self.n_ee_max))),
-                   frames=np.zeros(N, np.int32), success=np.zeros((N, 2), np.int32),
-                   stage_status=np.zeros((6, N), np.int32), stage_iters=np.zeros((6, N), np.int32),
-                   stage_stats=np.zeros((6, N, 4)))
+        N = self.N
+        keys = SOLVE_KEYS + ("stage_stats",)      # chd_phys_queue_solve's outputs, in its order
+        out = result_arrays(N, keys, self.dims["frames_out_max"], sample_stride(self.n_ee_max))
         self._claimed, self._claim_error = [], None
         with _terms_out(self, N, cost_terms) as terms:
-            rc = self.L.chd_phys_queue_solve(self.h, *[_ptr(out[k]) for k in ("samples", "frames", "success",
-                                                                              "stage_status", "stage_iters", "stage_stats")])
+            rc = self.L.chd_phys_queue_solve(self.h, *[_ptr(out[k]) for k in keys])
         if self._claim_error is not None:
             e, self._claim_error = self._claim_error, None
             raise RuntimeError("the claim source of the queue failed") from e
-        if rc != 0:
-            raise RuntimeError("libchd call failed with code %d" % rc)
+        self._chk(rc)
         solved = np.ones(N, bool)
         if self.claim is not None:
             solved[:] = False
@@ -529,29 +580,7 @@ class PhysQueue:
         out["solved"] = solved
         if terms is not None:
             out["cost_terms"] = terms
-        inv = np.argsort(self.order)          # queue position of every input clip
-        axis = dict(samples=1, frames=0, success=0, stage_status=1, stage_iters=1, stage_stats=1, solved=0, cost_terms=0)
-        return {k: np.take(v, inv, axis=axis[k]) for k, v in out.items()}
-
-    def launch_count(self) -> int:
-        return int(self.L.chd_phys_launch_count(self.h))
-
-    def _chk(self, rc):
-        if rc != 0:
-            raise RuntimeError("libchd call failed with code %d" % rc)
-
-    def h2d_bytes(self) -> int:
-        """Bytes uploaded so far: the slots' tables at creation and the records of every admitted clip."""
-        return int(self.L.chd_phys_h2d_bytes(self.h))
-
-    def set_timing(self, on: bool):
-        self.L.chd_phys_set_timing(self.h, int(on))
-
-    def kernel_times(self, reset=False):
-        ms, cnt = np.zeros(8), np.zeros(8, np.int64)
-        self.L.chd_phys_kernel_times(self.h, _ptr(ms), _ptr(cnt), int(reset))
-        names = ["eval", "kkt", "linesearch", "init", "sample", "admit"]
-        return {k: (float(ms[i]), int(cnt[i])) for i, k in enumerate(names)}
+        return take_clips(out, np.argsort(self.order))   # queue position of every input clip
 
 
 SOLUTION_FILES = ("sol_out_no_dynamics.txt", "sol_out_dynamics.txt", "sol_out_durations.txt")

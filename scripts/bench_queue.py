@@ -52,7 +52,6 @@ class PoolMeter:
 
 def solve_batches(chd, ps, per, timing=False):
     """Consecutive batches of `per` clips; results concatenated in clip order, plus the instrumentation of all."""
-    keys = ("samples", "frames", "success", "stage_status", "stage_iters")
     parts, kkt_ms, kkt_n = [], 0.0, 0
     for a in range(0, len(ps), per):
         b = chd.phys.PhysBatch(ps[a:a + per])
@@ -62,11 +61,7 @@ def solve_batches(chd, ps, per, timing=False):
         kkt_ms, kkt_n = kkt_ms + kt["kkt"][0], kkt_n + kt["kkt"][1]
         b.close()
         parts.append(out)
-    fo = max(p["samples"].shape[2] for p in parts)
-    pad = lambda s: np.pad(s, ((0, 0), (0, 0), (0, fo - s.shape[2]), (0, 0)))
-    axis = dict(samples=1, frames=0, success=0, stage_status=1, stage_iters=1)
-    out = {k: np.concatenate([(pad(p[k]) if k == "samples" else p[k]) for p in parts], axis=axis[k]) for k in keys}
-    return out, {"kkt_ms": kkt_ms, "kkt_launches": kkt_n}
+    return chd.phys.concat_results(parts), {"kkt_ms": kkt_ms, "kkt_launches": kkt_n}
 
 
 def solve_queue(chd, ps, slots, timing=False, meter=None, claim=None):

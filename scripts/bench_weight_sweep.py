@@ -41,13 +41,12 @@ def main():
         return out
 
     def singles():
-        st, it = np.zeros((6, n), np.int32), np.zeros((6, n), np.int32)
-        for k, w in enumerate(grid):
+        parts = []
+        for w in grid:
             b = chd.phys.PhysBatch([p], weights=w)
-            r = b.solve()
+            parts.append(b.solve())
             b.close()
-            st[:, k], it[:, k] = r["stage_status"][:, 0], r["stage_iters"][:, 0]
-        return dict(stage_status=st, stage_iters=it)
+        return chd.phys.concat_results(parts)
 
     arms = dict(queue=queue, singles=singles)
     queue()                                                           # warm-up of both arms

@@ -8,6 +8,8 @@ import sys
 import numpy as np
 import pytest
 
+from tests.util import QueueLib, random_result
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
@@ -32,59 +34,6 @@ def test_set_claim_refuses_batch_and_null_handles(chd):
         L.chd_phys_batch_destroy(h)
 
 
-class _ClaimingLib:
-    """Stands in for libchd: asks the claim source registered with chd_phys_queue_set_claim for `slots` positions, then
-    for `wants` in turn (as finished slots would), until the source returns fewer than asked; answers every output of
-    the positions handed out with the position k and the clip's frame count."""
-
-    def __init__(self, wants):
-        self.wants, self.cb, self.asked = list(wants), None, []
-
-    def chd_phys_queue_create(self, arr, n, slots, w, dev, opt, out):
-        self.frames_in = [arr[k].n_frames for k in range(n)]
-        self.slots = min(slots, n)
-        out._obj.value = 1
-        return 0
-
-    def chd_phys_get_dims(self, h, d):
-        d._obj.batch, d._obj.frames_out_max = self.slots, max(self.frames_in)
-        return 0
-
-    def chd_phys_queue_set_claim(self, h, cb, ctx):
-        import chd
-        self.cb = C.cast(cb, chd.phys.CLAIM_FN)
-        return 0
-
-    def chd_phys_queue_solve(self, h, samples, frames, success, status, iters, stats):
-        n, fo = len(self.frames_in), max(self.frames_in)
-        view = lambda p, ct, shape: np.ctypeslib.as_array(C.cast(p, C.POINTER(ct)), shape=shape)
-        smp = view(samples, C.c_double, (3, n, fo, 20))
-        st, it = view(status, C.c_int32, (6, n)), view(iters, C.c_int32, (6, n))
-        sc, ss = view(success, C.c_int32, (n, 2)), view(stats, C.c_double, (6, n, 4))
-        fr = view(frames, C.c_int32, (n,))
-        given = []
-        for want in [self.slots] + self.wants:
-            first = C.c_int32(-7)
-            k = self.cb(None, want, C.byref(first))
-            self.asked.append(want)
-            if k < 0:
-                return -1
-            given += range(first.value, first.value + k)
-            if k < want:
-                break
-        for k in given:
-            f = self.frames_in[k]
-            smp[:, k, :f, 0] = f
-            fr[k] = f
-            sc[k] = (k, f)
-            st[:, k], it[:, k] = k, f
-            ss[:, k, :] = f
-        return 0
-
-    def chd_phys_batch_destroy(self, h):
-        pass
-
-
 def _from_the_back(n, stop=None):
     """claim source handing out the last `want` positions not yet handed out (at most `stop` in all)"""
     left = [n if stop is None else stop]
@@ -100,7 +49,7 @@ def _from_the_back(n, stop=None):
 def test_claim_chunks_give_input_order_and_solved_mask(chd, monkeypatch, stop):
     """Uneven chunks (3 at the start, then 1, 2, 1, 3, ...) taken from the back of the queue: every clip handed out is
     answered in its input place, `solved` marks exactly those clips, the others' rows stay zero."""
-    fake = _ClaimingLib([1, 2, 1, 3, 2, 2, 1, 3])
+    fake = QueueLib([1, 2, 1, 3, 2, 2, 1, 3])
     monkeypatch.setattr(chd.phys, "load_lib", lambda: fake)
     F = [50, 90, 40, 120, 90, 70, 66, 48, 101, 75]
     N = len(F)
@@ -126,7 +75,7 @@ def test_claim_chunks_give_input_order_and_solved_mask(chd, monkeypatch, stop):
 
 
 def test_claim_exception_is_raised_by_solve(chd, monkeypatch):
-    fake = _ClaimingLib([2])
+    fake = QueueLib([2])
     monkeypatch.setattr(chd.phys, "load_lib", lambda: fake)
     ps = [chd.synth.make_problem(i, n_frames=40 + i, n_ee=2) for i in range(4)]
     calls = []
@@ -181,19 +130,6 @@ def test_store_claim_hands_out_every_position_once(tmp_path):
 N_MERGE = 11
 
 
-def _fake_queue_result(n, fo=7, stride=20):
-    """What every rank's queue would compute for every clip: random values with -0.0 entries and mixed signs"""
-    rng = np.random.default_rng(5)
-    smp = rng.standard_normal((3, n, fo, stride))
-    smp[rng.random(smp.shape) < 0.1] = -0.0
-    stats = rng.standard_normal((6, n, 4))
-    stats[0, :, 0] = -0.0
-    return dict(samples=smp, frames=rng.integers(1, fo + 1, n).astype(np.int32),
-                success=rng.integers(0, 2, (n, 2)).astype(np.int32),
-                stage_status=rng.integers(-3, 2, (6, n)).astype(np.int32),
-                stage_iters=rng.integers(0, 3000, (6, n)).astype(np.int32), stage_stats=stats)
-
-
 def _subset(rank, world, n):
     """interleaved random subsets: a random owner for every clip (rank 1 gets clip 0 so that both ranks hold some)"""
     owner = np.random.default_rng(9).integers(0, world, n)
@@ -212,11 +148,11 @@ def _merge_worker(rank, world, port, tmp):
 
     def solve_fn(problems):
         assert len(problems) == N_MERGE
-        full = _fake_queue_result(len(problems))
+        full = random_result(len(problems), 7)
         mine = _subset(rank, world, len(problems))
         out = {k: v.copy() for k, v in full.items()}
-        for k, ax in dict(samples=1, frames=0, success=0, stage_status=1, stage_iters=1, stage_stats=1).items():
-            np.moveaxis(out[k], ax, 0)[~mine] = 0                      # rows of clips another rank solved stay zero
+        for k in out:
+            np.moveaxis(out[k], chd.phys.clip_axis(k), 0)[~mine] = 0   # rows of clips another rank solved stay zero
         out["solved"] = mine
         return out
 
@@ -232,7 +168,7 @@ def test_merge_is_bitwise_union_in_input_order(tmp_path):
     port = 35500 + (os.getpid() % 2000)
     mp.spawn(_merge_worker, args=(2, port, str(tmp_path)), nprocs=2, join=True)
     r0, r1 = np.load(str(tmp_path / "m0.npz")), np.load(str(tmp_path / "m1.npz"))
-    full = _fake_queue_result(N_MERGE)
+    full = random_result(N_MERGE, 7)
     owner = np.where(_subset(1, 2, N_MERGE), 1, 0)
     for k in r0.files:                                                  # every rank returns the same bits
         assert r0[k].tobytes() == r1[k].tobytes(), k
@@ -244,7 +180,7 @@ def test_merge_is_bitwise_union_in_input_order(tmp_path):
 
 
 def test_merge_on_one_rank_keeps_unsolved_rows_empty(chd):
-    full = _fake_queue_result(6)
+    full = random_result(6, 7)
     local = dict(full, solved=np.array([1, 0, 1, 1, 0, 0], bool))
     out = chd.parallel.merge_solved(local, 1)
     np.testing.assert_array_equal(out["solved_by"], [0, -1, 0, 0, -1, -1])

@@ -20,11 +20,6 @@ def _mixed(chd, n, seed0):
     return [chd.synth.make_problem(seed0 + i, n_frames=f, n_ee=2) for i, f in enumerate(F)]
 
 
-def _take(out, idx):
-    axis = dict(samples=1, frames=0, success=0, stage_status=1, stage_iters=1, stage_stats=1, solved=0)
-    return {k: np.take(v, idx, axis=axis[k]) for k, v in out.items() if k in axis}
-
-
 class _Back:
     """Hands out the last `want` positions not handed out yet (at most `stop` in all), recording every chunk."""
 
@@ -70,7 +65,7 @@ def test_source_that_stops_leaves_the_rest_unsolved(chd):
     mine = np.sort(q.order[:N // 2])                                  # the first N/2 queue positions, as input clips
     rest = np.setdiff1d(np.arange(N), mine)
     np.testing.assert_array_equal(np.nonzero(got["solved"])[0], mine)
-    a, b = _take(ref, mine), _take(got, mine)
+    a, b = chd.phys.take_clips(ref, mine), chd.phys.take_clips(got, mine)
     assert_solves_agree(a, b, 2)
     np.testing.assert_array_equal(b["frames"], a["frames"])
     np.testing.assert_array_equal(b["success"], a["success"])

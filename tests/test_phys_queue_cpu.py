@@ -5,6 +5,8 @@ import ctypes as C
 import numpy as np
 import pytest
 
+from tests.util import QueueLib
+
 
 def _create(chd, problems, n, slots, device=-2, band=None):
     P = chd.phys
@@ -72,45 +74,8 @@ def test_batch_handle_refuses_queue_solve(chd):
     assert b.L.chd_phys_queue_solve(b.h, None, None, None, None, None, None) == -1
 
 
-class _FakeLib:
-    """Stands in for libchd: records the clip order it is given and answers every output with the clip's queue
-    position k and its frame count, so that the caller's un-permutation can be checked."""
-
-    def __init__(self):
-        self.frames_in = None
-        self.n_ee_max = 0
-
-    def chd_phys_queue_create(self, arr, n, slots, w, dev, opt, out):
-        self.frames_in = [arr[k].n_frames for k in range(n)]
-        self.slots = min(slots, n)
-        out._obj.value = 1
-        return 0
-
-    def chd_phys_get_dims(self, h, d):
-        d._obj.batch, d._obj.frames_out_max = self.slots, max(self.frames_in)
-        return 0
-
-    def chd_phys_queue_solve(self, h, samples, frames, success, status, iters, stats):
-        n, fo = len(self.frames_in), max(self.frames_in)
-        view = lambda p, ct, shape: np.ctypeslib.as_array(C.cast(p, C.POINTER(ct)), shape=shape)
-        smp = view(samples, C.c_double, (3, n, fo, 20))
-        st, it = view(status, C.c_int32, (6, n)), view(iters, C.c_int32, (6, n))
-        sc, ss = view(success, C.c_int32, (n, 2)), view(stats, C.c_double, (6, n, 4))
-        fr = view(frames, C.c_int32, (n,))
-        for k, f in enumerate(self.frames_in):
-            smp[:, k, :f, 0] = f
-            fr[k] = f
-            sc[k] = (k, f)
-            st[:, k], it[:, k] = k, f
-            ss[:, k, :] = f
-        return 0
-
-    def chd_phys_batch_destroy(self, h):
-        pass
-
-
 def test_queue_orders_by_work_and_returns_input_order(chd, monkeypatch):
-    fake = _FakeLib()
+    fake = QueueLib()
     monkeypatch.setattr(chd.phys, "load_lib", lambda: fake)
     F = [50, 90, 40, 120, 90, 70]
     ps = [chd.synth.make_problem(i, n_frames=f, n_ee=2) for i, f in enumerate(F)]

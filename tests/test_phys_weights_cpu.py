@@ -8,6 +8,8 @@ import sys
 import numpy as np
 import pytest
 
+from tests.util import QueueLib, random_result
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SCRIPTS = os.path.join(ROOT, "scripts")
 
@@ -179,44 +181,10 @@ def test_weight_sweep_grid_and_rows(chd):
         assert r["iters_2.2"] == out["stage_iters"][3, i]
 
 
-class _TermsLib:
-    """Stands in for libchd's queue: writes every clip's cost terms as (queue position, column) into the buffer set
-    with chd_phys_set_cost_terms_out, and records the per-clip weights it was created with."""
-
-    def __init__(self):
-        self.terms_ptr, self.set_calls = None, []
-
-    def chd_phys_queue_create(self, arr, n, slots, w, dev, opt, out):
-        self.n, self.slots = n, min(slots, n)
-        self.frames_in = [arr[k].n_frames for k in range(n)]
-        self.weights = [tuple(getattr(opt._obj.clip_weights[k], f) for f, _ in opt._obj.clip_weights[k]._fields_)
-                        for k in range(n)]
-        out._obj.value = 1
-        return 0
-
-    def chd_phys_get_dims(self, h, d):
-        d._obj.batch, d._obj.frames_out_max = self.slots, max(self.frames_in)
-        return 0
-
-    def chd_phys_set_cost_terms_out(self, h, p):
-        self.terms_ptr = p
-        self.set_calls.append(p is not None)
-        return 0
-
-    def chd_phys_queue_solve(self, h, *outs):
-        if self.terms_ptr is not None:
-            t = np.ctypeslib.as_array(C.cast(self.terms_ptr, C.POINTER(C.c_double)), shape=(self.n, 10))
-            t[:] = np.arange(self.n)[:, None] * 100 + np.arange(10)
-        return 0
-
-    def chd_phys_batch_destroy(self, h):
-        pass
-
-
 def test_queue_terms_and_weights_follow_the_clips(chd, monkeypatch):
     """PhysQueue hands each clip's weights to the library in queue order and returns the terms in input order; the
     output pointer is cleared after the solve."""
-    fake = _TermsLib()
+    fake = QueueLib()
     monkeypatch.setattr(chd.phys, "load_lib", lambda: fake)
     F = [50, 90, 40, 120, 70]
     ps = [chd.synth.make_problem(i, n_frames=f, n_ee=2) for i, f in enumerate(F)]
@@ -233,16 +201,6 @@ def test_queue_terms_and_weights_follow_the_clips(chd, monkeypatch):
 N_MERGE = 9
 
 
-def _fake_result(n):
-    rng = np.random.default_rng(5)
-    terms = rng.random((n, 10))
-    terms[rng.random(terms.shape) < 0.2] = -0.0
-    return dict(samples=rng.standard_normal((3, n, 5, 20)), frames=rng.integers(1, 6, n).astype(np.int32),
-                success=rng.integers(0, 2, (n, 2)).astype(np.int32), stage_status=rng.integers(-3, 2, (6, n)).astype(np.int32),
-                stage_iters=rng.integers(0, 3000, (6, n)).astype(np.int32), stage_stats=rng.standard_normal((6, n, 4)),
-                cost_terms=terms)
-
-
 def _merge_worker(rank, world, port, tmp):
     sys.path.insert(0, ROOT)
     import torch.distributed as dist
@@ -255,9 +213,9 @@ def _merge_worker(rank, world, port, tmp):
     mine[0] = rank == 1
 
     def solve_fn(problems):
-        out = {k: v.copy() for k, v in _fake_result(len(problems)).items()}
-        for k, ax in dict(samples=1, frames=0, success=0, stage_status=1, stage_iters=1, stage_stats=1, cost_terms=0).items():
-            np.moveaxis(out[k], ax, 0)[~mine] = 0
+        out = {k: v.copy() for k, v in random_result(len(problems), 5, terms=True).items()}
+        for k in out:
+            np.moveaxis(out[k], chd.phys.clip_axis(k), 0)[~mine] = 0
         out["solved"] = mine
         return out
 
@@ -274,7 +232,7 @@ def test_merge_carries_the_terms_bitwise(tmp_path):
     port = 37600 + (os.getpid() % 2000)
     mp.spawn(_merge_worker, args=(2, port, str(tmp_path)), nprocs=2, join=True)
     r0, r1 = np.load(str(tmp_path / "m0.npz")), np.load(str(tmp_path / "m1.npz"))
-    full = _fake_result(N_MERGE)
+    full = random_result(N_MERGE, 5, terms=True)
     for k in r0.files:
         assert r0[k].tobytes() == r1[k].tobytes(), k
     for k, v in full.items():
@@ -283,14 +241,14 @@ def test_merge_carries_the_terms_bitwise(tmp_path):
 
 
 def test_merge_without_terms_keeps_its_row(chd):
-    full = _fake_result(4)
+    full = random_result(4, 5, terms=True)
     local = {k: v for k, v in full.items() if k != "cost_terms"}
     local["solved"] = np.ones(4, bool)
     out = chd.parallel.merge_solved(local, 1)
     assert "cost_terms" not in out
-    assert out["d2h_bytes"] == 4 * (1 + 3 * 5 * 20 + chd.parallel.Q_EXTRA) * 8
+    assert out["d2h_bytes"] == 4 * (1 + 3 * 5 * 20 + 39) * 8
     with_terms = chd.parallel.merge_solved(dict(full, solved=np.ones(4, bool)), 1)
-    assert with_terms["d2h_bytes"] == 4 * (1 + 3 * 5 * 20 + chd.parallel.Q_EXTRA + 10) * 8
+    assert with_terms["d2h_bytes"] == 4 * (1 + 3 * 5 * 20 + 39 + 10) * 8
 
 
 def test_unsharded_terms_need_slots(chd):

@@ -1,6 +1,8 @@
 """Shared helpers of the parity tests: mapping between the product's master row order and the
-oracle's ifopt row order (which follows phys_optim.cpp's per-stage AddConstraintSet order), and the checks that compare
-a GPU solve with the oracle's or with another form of the same solve."""
+oracle's ifopt row order (which follows phys_optim.cpp's per-stage AddConstraintSet order), the checks that compare
+a GPU solve with the oracle's or with another form of the same solve, and stand-ins for the queue's results and ABI."""
+import ctypes as C
+
 import numpy as np
 
 import chd
@@ -160,3 +162,93 @@ def assert_solves_agree(ref, got, n_ee, n_ee_max=None):
     assert len(same) >= 0.9 * B
     d3 = np.array([close(2, i) for i in same])
     print("stage 3: max |diff| positions %.2e, forces %.2e" % tuple(d3.max(axis=0)))
+
+
+QUEUE_KEYS = chd.phys.SOLVE_KEYS + ("stage_stats",)   # what a queue solve writes, before `solved` and the cost terms
+
+
+def random_result(n, fo, stride=20, terms=False, seed=5):
+    """What a queue would compute for n clips (`QUEUE_KEYS`, with `terms` also `cost_terms`): integers in each field's
+    range, normal floats with mixed signs and about one entry in ten -0.0 in every float field."""
+    rng = np.random.default_rng(seed)
+    out = chd.phys.result_arrays(n, QUEUE_KEYS + (("cost_terms",) if terms else ()), fo, stride)
+    ints = dict(frames=(1, fo + 1), success=(0, 2), stage_status=(-3, 2), stage_iters=(0, 3000))
+    for k, v in out.items():
+        if k in ints:
+            v[:] = rng.integers(*ints[k], v.shape)
+        else:
+            v[:] = rng.standard_normal(v.shape)
+            v[rng.random(v.shape) < 0.1] = -0.0
+    return out
+
+
+class QueueLib:
+    """Stands in for libchd's queue: records the clip order (`frames_in`) and the per-clip weights (`weights`, None
+    without them) it is created with, and answers every clip a solve covers with its queue position k and frame count f:
+    samples[:, k, :f, 0] = f, frames f, success (k, f), stage_status k, stage_iters f, stage_stats f and, into a buffer
+    set with chd_phys_set_cost_terms_out, cost terms 100 k + column.  A solve covers every clip, or with a claim source
+    (chd_phys_queue_set_claim) the positions it hands out: it is asked for `slots` positions, then for `wants` in turn (as
+    finished slots would ask) until it returns fewer than asked."""
+
+    def __init__(self, wants=()):
+        self.wants, self.cb, self.asked = list(wants), None, []
+        self.terms_ptr, self.set_calls = None, []
+
+    def chd_phys_queue_create(self, arr, n, slots, w, dev, opt, out):
+        self.n, self.slots = n, min(slots, n)
+        self.frames_in = [arr[k].n_frames for k in range(n)]
+        self.stride = chd.phys.sample_stride(max(arr[k].n_ee for k in range(n)))
+        cw = opt._obj.clip_weights if opt is not None else None
+        self.weights = [tuple(getattr(cw[k], f) for f, _ in cw[k]._fields_) for k in range(n)] if cw else None
+        out._obj.value = 1
+        return 0
+
+    def chd_phys_get_dims(self, h, d):
+        d._obj.batch, d._obj.frames_out_max = self.slots, max(self.frames_in)
+        return 0
+
+    def chd_phys_queue_set_claim(self, h, cb, ctx):
+        self.cb = C.cast(cb, chd.phys.CLAIM_FN)
+        return 0
+
+    def chd_phys_set_cost_terms_out(self, h, p):
+        self.terms_ptr = p
+        self.set_calls.append(p is not None)
+        return 0
+
+    def _claimed(self):
+        """positions handed out by the claim source, None: it failed"""
+        given = []
+        for want in [self.slots] + self.wants:
+            first = C.c_int32(-7)
+            k = self.cb(None, want, C.byref(first))
+            self.asked.append(want)
+            if k < 0:
+                return None
+            given += range(first.value, first.value + k)
+            if k < want:
+                break
+        return given
+
+    def chd_phys_queue_solve(self, h, *ptrs):
+        given = range(self.n) if self.cb is None else self._claimed()
+        if given is None:
+            return -1
+        res = chd.phys.result_arrays(self.n, QUEUE_KEYS + ("cost_terms",), max(self.frames_in), self.stride)
+        view = lambda p, a: np.ctypeslib.as_array(C.cast(p, C.POINTER(np.ctypeslib.as_ctypes_type(a.dtype))), a.shape)
+        out = {k: view(p, res[k]) for k, p in zip(QUEUE_KEYS, ptrs)}
+        if self.terms_ptr is not None:
+            out["cost_terms"] = view(self.terms_ptr, res["cost_terms"])
+        for k in given:
+            f = self.frames_in[k]
+            out["samples"][:, k, :f, 0] = f
+            out["frames"][k] = f
+            out["success"][k] = (k, f)
+            out["stage_status"][:, k], out["stage_iters"][:, k] = k, f
+            out["stage_stats"][:, k, :] = f
+            if "cost_terms" in out:
+                out["cost_terms"][k] = 100 * k + np.arange(len(chd.phys.COST_TERMS))
+        return 0
+
+    def chd_phys_batch_destroy(self, h):
+        pass
