@@ -1,6 +1,7 @@
 // C ABI of the phys-optim path (see include/chd.h).  Host driver: device memory, stage loops, launches.
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
@@ -111,6 +112,8 @@ struct chd_phys_batch {
   double* d_x0 = nullptr;
   int64_t h2d_bytes = 0;
   std::vector<ChdStageDev> stages;   // B x 6 rows of the stage table (a queue: of the slots; its records hold every clip's)
+  std::vector<ChdStageEnd> ends;     // B records behind the stage rows on the device (a queue: as `stages`)
+  std::vector<chd_phys_solver_options> opts;   // every sequence's (a queue: every clip's) options, defaults resolved
   ChdStageDev* d_stages = nullptr;
   double* terms_out = nullptr;        // chd_phys_set_cost_terms_out: [host] where a solve writes the final cost terms
   double* d_terms = nullptr;          // B x CHD_PHYS_N_TERMS (chd_k_cost_terms)
@@ -144,6 +147,11 @@ void write_status(const ChdSolveOut& o, size_t c, const ChdIpm& I) {
   }
 }
 
+// the SaveSolution snapshots clip c does not take, those after its last stage, are NaN (row: doubles of one snapshot)
+void write_untaken(const ChdSolveOut& o, size_t c, int last_stage, size_t row) {
+  for (size_t s = last_stage + 1; o.samples && s < 3; ++s) std::fill_n(o.samples + (s * o.n + c) * row, row, NAN);
+}
+
 template <class T>
 int dev_upload(chd_phys_batch* b, const std::vector<T>& v, const T** out) {
   void* p = nullptr;
@@ -165,15 +173,44 @@ int dev_alloc(chd_phys_batch* b, size_t count, T** out) {
   return 0;
 }
 
-ChdStageDev stage_dev(const ChdStageCfg& c, int stage) {
+// the stage a last_stage option ends with (CHD_LAST_DURATIONS: none, the schedule's own end)
+int last_stage_id(int last_stage) {
+  return last_stage == CHD_LAST_NO_DYNAMICS ? CHD_STAGE_12 : (last_stage == CHD_LAST_DYNAMICS ? CHD_STAGE_22 : -1);
+}
+
+// row `stage` of a sequence's stage table: its layout's configuration with the cap of its solver options
+ChdStageDev stage_dev(const ChdStageCfg& c, int stage, const chd_phys_solver_options& o) {
   ChdStageDev s;
   s.set_mask = c.set_mask;
-  s.max_iter = c.max_iter;
+  s.max_iter = o.max_iter[stage];
   s.snap_after = stage == CHD_STAGE_12 ? 0 : (stage == CHD_STAGE_22 ? 1 : ((stage == CHD_STAGE_4 || stage == CHD_STAGE_3) ? 2 : -1));
   s.opt_dur = stage == CHD_STAGE_3;
   for (int i = 0; i < 3; ++i) s.w_data[i] = c.w_data[i], s.w_vel[i] = c.w_vel[i], s.w_acc[i] = c.w_acc[i];
   s.w_dur = c.w_dur;
   return s;
+}
+
+ChdStageEnd stage_end(const chd_phys_solver_options& o) {
+  return {o.tol, o.constr_viol_tol, o.dual_inf_tol, o.compl_inf_tol, last_stage_id(o.last_stage), 0};
+}
+
+// options of a clip as given (NULL: the defaults), with every cap of 0 resolved to the stage's own in `stages` (its six
+// rows of the layout)
+chd_phys_solver_options resolve_options(const chd_phys_solver_options* given, const ChdStageCfg* stages) {
+  chd_phys_solver_options o = {CHD_TOL, CHD_CONSTR_VIOL_TOL, CHD_DUAL_INF_TOL, CHD_COMPL_INF_TOL, {0}, CHD_LAST_DURATIONS};
+  if (given) o = *given;
+  for (int s = 0; s < 6; ++s)
+    if (o.max_iter[s] == 0) o.max_iter[s] = stages[s].max_iter;
+  return o;
+}
+
+// a tolerance not finite or not > 0, a negative cap or an unknown last stage
+bool bad_options(const chd_phys_solver_options& o) {
+  for (double v : {o.tol, o.constr_viol_tol, o.dual_inf_tol, o.compl_inf_tol})
+    if (!std::isfinite(v) || !(v > 0.0)) return true;
+  for (int s = 0; s < 6; ++s)
+    if (o.max_iter[s] < 0) return true;
+  return o.last_stage < CHD_LAST_NO_DYNAMICS || o.last_stage > CHD_LAST_DURATIONS;
 }
 
 struct Timer {
@@ -206,12 +243,18 @@ int set_schedule(chd_phys_batch* b, const int* sched, int nsched, int override_s
   if (override_stage >= 0 && override_max_iter > 0)
     for (size_t i = 0; i < tab.size(); i += 6) tab[i + override_stage].max_iter = override_max_iter;
   CHD_CUDA(cudaMemcpyAsync(b->d_stages, tab.data(), tab.size() * sizeof(ChdStageDev), cudaMemcpyHostToDevice, b->stream));
-  const ChdStageDev* t = tab.data();   // the caps of every sequence are the same
   b->D.nsched = nsched;
   for (int i = 0; i < nsched; ++i) b->D.sched[i] = sched[i];
-  b->sched_max_iter = 0;
   b->sched_has_dur = false;
-  for (int i = 0; i < nsched; ++i) b->sched_max_iter += t[sched[i]].max_iter + 2, b->sched_has_dur |= sched[i] == CHD_STAGE_3;
+  for (int i = 0; i < nsched; ++i) b->sched_has_dur |= sched[i] == CHD_STAGE_3;
+  // bound of the launch loop: the largest sum of a sequence's caps over the schedule (a queue: of any of its clips)
+  b->sched_max_iter = 0;
+  for (const chd_phys_solver_options& o : b->opts) {
+    int sum = 0;
+    for (int i = 0; i < nsched; ++i)
+      sum += (sched[i] == override_stage && override_max_iter > 0 ? override_max_iter : o.max_iter[sched[i]]) + 2;
+    b->sched_max_iter = std::max(b->sched_max_iter, sum);
+  }
   chd_k_sched_reset<<<(b->hb.B + 127) / 128, 128, 0, b->stream>>>(b->D);
   b->launches++;
   return 0;
@@ -317,6 +360,7 @@ void queue_tables(chd_phys_batch* b, F&& f) {
   f(hb.row_lo, D.row_lo), f(hb.row_hi, D.row_hi), f(hb.dur0, D.dur0), f(hb.x0, D.x, b->d_x0);
   f(hb.poly_T, D.poly_T, b->poly_T0, D.poly_Tt), f(hb.poly_tend, D.poly_tend, b->poly_tend0, D.poly_tendt);
   f(hb.phase_tend, D.phase_tend, b->phase_tend0), f(b->stages, D.stages);
+  f(b->ends, D.stages ? (const void*)(D.stages + b->stages.size()) : nullptr);
 }
 
 // Packs the layout of all hb.B clips into one record per clip and keeps the first `slots` rows of every table as the
@@ -442,8 +486,9 @@ int queue_harvest(chd_phys_batch* b, int slot) {
   const ChdHostBatch& hb = b->hb;
   const ChdSolveOut& o = b->out;
   const size_t S = hb.B, row = hb.fo_max * sample_stride(hb);
+  const int last = b->opts[c].last_stage;
   if (o.samples)
-    for (size_t s = 0; s < 3; ++s)
+    for (size_t s = 0; s <= (size_t)last; ++s)
       CHD_CUDA(cudaMemcpyAsync(o.samples + (s * o.n + c) * row, b->D.snapshots + (s * S + slot) * row, row * sizeof(double),
                                cudaMemcpyDeviceToHost, b->stream));
   if (o.frames) CHD_CUDA(cudaMemcpyAsync(o.frames + c, b->d_frames + slot, sizeof(int), cudaMemcpyDeviceToHost, b->stream));
@@ -451,6 +496,7 @@ int queue_harvest(chd_phys_batch* b, int slot) {
     CHD_CUDA(cudaMemcpyAsync(o.terms + (size_t)c * CHD_PHYS_N_TERMS, b->d_terms + (size_t)slot * CHD_PHYS_N_TERMS,
                              CHD_PHYS_N_TERMS * sizeof(double), cudaMemcpyDeviceToHost, b->stream));
   write_status(o, c, b->h_ipm[slot]);
+  write_untaken(o, c, last, row);
   q.clip[slot] = -1;
   return 0;
 }
@@ -523,7 +569,7 @@ static int batch_create_impl(const chd_phys_problem* problems, int32_t batch, in
 // a batch (slots = 0) or a queue of `batch` clips through `slots` slots
 static int create(const chd_phys_problem* problems, int32_t batch, int32_t slots, const chd_phys_weights* weights,
                   int32_t device, const chd_phys_options* opt, chd_phys_batch** out) {
-  chd_phys_options o = {-1, nullptr};
+  chd_phys_options o = {-1, nullptr, nullptr};
   if (opt) o = *opt;
   if (o.stage3_band_above < -1 || o.stage3_band_above > CHD_MAX_DUR) return -1;
   // a weight must be finite and not negative
@@ -538,6 +584,9 @@ static int create(const chd_phys_problem* problems, int32_t batch, int32_t slots
   } else if (weights && bad(*weights)) {
     return -1;
   }
+  if (o.clip_options)
+    for (int i = 0; i < batch; ++i)
+      if (bad_options(o.clip_options[i])) return -1;
   chd_phys_batch* b = new chd_phys_batch();
   std::memset(&b->D, 0, sizeof(b->D));
   const int rc = batch_create_impl(problems, batch, slots, weights, device, o, b);
@@ -573,8 +622,14 @@ static int batch_create_impl(const chd_phys_problem* problems, int32_t batch, in
   int rc = chd_build_layout(problems, batch, wv.data(), b->hb, opt.stage3_band_above);
   if (rc) return rc;
   ChdHostBatch& hb = b->hb;
+  b->opts.resize(batch);
+  b->ends.resize(batch);
   b->stages.resize(hb.stage.size());
-  for (size_t i = 0; i < hb.stage.size(); ++i) b->stages[i] = stage_dev(hb.stage[i], (int)(i % 6));
+  for (int i = 0; i < batch; ++i) {
+    b->opts[i] = resolve_options(opt.clip_options ? opt.clip_options + i : nullptr, hb.stage.data() + (size_t)i * 6);
+    b->ends[i] = stage_end(b->opts[i]);
+    for (int s = 0; s < 6; ++s) b->stages[(size_t)i * 6 + s] = stage_dev(hb.stage[(size_t)i * 6 + s], s, b->opts[i]);
+  }
   ChdDev& D = b->D;
   std::memset(&D, 0, sizeof(D));
   b->host_only = host_only;
@@ -660,9 +715,14 @@ static int batch_create_impl(const chd_phys_problem* problems, int32_t batch, in
   b->allocs.push_back(b->d_frames);
   b->h_ipm = (ChdIpm*)std::malloc(B * sizeof(ChdIpm));   // pageable: pinned allocation / release is slow per batch
   if (!b->h_ipm) return -3;
-  CHD_CUDA(cudaMallocAsync((void**)&b->d_stages, b->stages.size() * sizeof(ChdStageDev), b->stream));
+  // the stage rows (uploaded by every solve, set_schedule, and like them not counted in h2d_bytes) and behind them the
+  // sequences' ChdStageEnd records
+  const size_t rows_bytes = b->stages.size() * sizeof(ChdStageDev);
+  CHD_CUDA(cudaMallocAsync((void**)&b->d_stages, rows_bytes + b->ends.size() * sizeof(ChdStageEnd), b->stream));
   b->allocs.push_back(b->d_stages);
   D.stages = b->d_stages;
+  CHD_CUDA(cudaMemcpyAsync((char*)b->d_stages + rows_bytes, b->ends.data(), b->ends.size() * sizeof(ChdStageEnd),
+                           cudaMemcpyHostToDevice, b->stream));
   if ((rc = dev_alloc(b, B * CHD_PHYS_N_TERMS, &b->d_terms))) return rc;
   if ((rc = dev_alloc(b, 3 * B * hb.fo_max * stride, &D.snapshots))) return rc;
   if (b->queue && (rc = queue_device(b, sms))) return rc;
@@ -896,6 +956,7 @@ int chd_phys_solve(chd_phys_batch* b, double* samples, int32_t* frames_out, int3
     CHD_CUDA(cudaMemcpyAsync(o.terms, b->d_terms, (size_t)B * CHD_PHYS_N_TERMS * sizeof(double), cudaMemcpyDeviceToHost, b->stream));
   }
   CHD_CUDA(cudaStreamSynchronize(b->stream));
+  for (int i = 0; i < B; ++i) write_untaken(o, i, b->opts[i].last_stage, hb.fo_max * sample_stride(hb));
   return 0;
 }
 
@@ -950,6 +1011,12 @@ int chd_phys_get_stage_weights(const chd_phys_batch* b, double* w) {
     w[9] = s.w_dur;
     w += 10;
   }
+  return 0;
+}
+
+int chd_phys_get_solver_options(const chd_phys_batch* b, chd_phys_solver_options* opts) {
+  if (!b || !opts) return -1;
+  std::copy(b->opts.begin(), b->opts.begin() + b->hb.B, opts);
   return 0;
 }
 

@@ -29,7 +29,7 @@ __global__ void chd_k_stage_begin(ChdDev D) {
     __syncthreads();
     if (threadIdx.x == 0) {
       D.ipm[b].iter = 0;
-      chd_stage_advance(D, D.ipm[b], -3, sg.snap_after);
+      chd_stage_advance(D, b, D.ipm[b], -3);
     }
     return;
   }

@@ -533,12 +533,13 @@ __device__ __forceinline__ bool chd_kkt_errors(const ChdDev& D, ChdKktCtx& c, in
   auto compl_err = [&](double mm) { return nbnd > 0 ? fmax(fabs(cmax - mm), fabs(cmin - mm)) : 0.0; };
   const double E0 = fmax(fmax(dual_inf / s_d, cviol), compl_err(0.0) / s_c);
   const double dual_u = dual_inf / sf, compl_u = compl_err(0.0) / sf;
+  const ChdStageEnd& se = chd_stage_end(D, b);   // the sequence's termination tolerances
   bool done = false;
   int new_status = 1;
-  if (E0 <= CHD_TOL && violu <= CHD_CONSTR_VIOL_TOL && dual_u <= CHD_DUAL_INF_TOL && compl_u <= CHD_COMPL_INF_TOL) new_status = 0, done = true;
+  if (E0 <= se.tol && violu <= se.constr_viol_tol && dual_u <= se.dual_inf_tol && compl_u <= se.compl_inf_tol) new_status = 0, done = true;
   else if (I.iter >= I.max_iter) new_status = -1, done = true;
   if (!done) {
-    const double mu_min = fmin(CHD_TOL, CHD_COMPL_INF_TOL) / (CHD_KAPPA_EPS + 1.0);
+    const double mu_min = fmin(se.tol, se.compl_inf_tol) / (CHD_KAPPA_EPS + 1.0);
     while (true) {
       const double Emu = fmax(fmax(dual_inf / s_d, cviol), compl_err(mu) / s_c);
       if (Emu <= CHD_KAPPA_EPS * mu && mu > mu_min) mu = fmax(mu_min, fmin(CHD_KAPPA_MU * mu, pow(mu, CHD_THETA_MU)));
@@ -551,7 +552,7 @@ __device__ __forceinline__ bool chd_kkt_errors(const ChdDev& D, ChdKktCtx& c, in
     I.E0 = E0, I.viol_u = violu, I.dual_u = dual_u, I.compl_u = compl_u;
     I.status = new_status;
     s_fail = 0;
-    if (done) chd_stage_advance(D, I, new_status, c.sg.snap_after);
+    if (done) chd_stage_advance(D, b, I, new_status);
     if (!done) {
       I.mu = mu;
       I.tau = fmax(CHD_TAU_MIN, 1.0 - mu);
@@ -566,7 +567,7 @@ __device__ __forceinline__ bool chd_kkt_errors(const ChdDev& D, ChdKktCtx& c, in
   // feasibility polish: every test but the unscaled constraint violation passes -> this step only restores feasibility
   // (a large Levenberg-Marquardt weight makes it the least-norm Newton correction of the constraints; the adaptive
   // weight itself is left alone)
-  c.polish = E0 <= CHD_TOL && dual_u <= CHD_DUAL_INF_TOL && compl_u <= CHD_COMPL_INF_TOL && violu > CHD_CONSTR_VIOL_TOL &&
+  c.polish = E0 <= se.tol && dual_u <= se.dual_inf_tol && compl_u <= se.compl_inf_tol && violu > se.constr_viol_tol &&
              I.delta_w < CHD_DW_POLISH;
   c.delta_w = c.polish ? CHD_DW_POLISH : I.delta_w;
   return false;
@@ -991,7 +992,7 @@ __device__ __forceinline__ bool chd_kkt_no_step(const ChdDev& D, const ChdKktCtx
     // a coupling left the band (stage 3 moved a polynomial boundary further than the layout allows): the stage fails and
     // the schedule goes on with the fixed-duration stage 4, as the reference does after a failed stage 3
     __syncthreads();
-    if (tid == 0) I.status = -2, chd_stage_advance(D, I, -2, c.sg.snap_after);
+    if (tid == 0) I.status = -2, chd_stage_advance(D, c.b, I, -2);
     return true;
   }
   if (s_fail) {
@@ -1002,7 +1003,7 @@ __device__ __forceinline__ bool chd_kkt_no_step(const ChdDev& D, const ChdKktCtx
       I.ls_fail += 1;
       I.step_ready = 1;
       I.kw_req = 1;
-      if (I.delta_w > CHD_DW_MAX) I.status = -2, chd_stage_advance(D, I, -2, c.sg.snap_after);
+      if (I.delta_w > CHD_DW_MAX) I.status = -2, chd_stage_advance(D, c.b, I, -2);
     }
     for (int i = tid; i < n; i += nt) D.dx[vo + i] = 0.0;
     for (int r = tid; r < m; r += nt) D.ds[ro + r] = 0.0, D.dy[ro + r] = 0.0, D.dzL[ro + r] = 0.0, D.dzU[ro + r] = 0.0;

@@ -171,16 +171,21 @@ class ShardedSolver:
     stands in for `PhysQueue.solve()` over all N problems and returns its dict, `solved` marking the clips this rank
     solved.
 
-    `weights`: one 5-tuple for every problem or one per problem (`phys.clip_weights`).  `solve(cost_terms=True)`
-    (with `slots` only) also returns every clip's unweighted cost terms (`phys.COST_TERMS`), merged by clip index."""
+    `weights`: one 5-tuple for every problem or one per problem (`phys.clip_weights`); `options`: one
+    `phys.SolverOptions` for every problem or one per problem (`phys.clip_options`).  Without `slots` only the final
+    iterate travels, which for a clip that stopped early (`SolverOptions.last_stage`) is that of its last stage.
+    `solve(cost_terms=True)` (with `slots` only) also returns every clip's unweighted cost terms (`phys.COST_TERMS`),
+    merged by clip index."""
 
     def __init__(self, problems, weights=phys.DEFAULT_WEIGHTS, device: int = 0, rank: int = 0, world: int = 1,
-                 group=None, solve_fn=None, tensor_device=None, stage3_band_above=None, slots=None, store=None):
+                 group=None, solve_fn=None, tensor_device=None, stage3_band_above=None, slots=None, store=None,
+                 options=None):
         self.problems, self.rank, self.world, self.group = list(problems), rank, world, group
         self.queue_slots, self.queue = slots, None
         per = phys.clip_weights(weights, len(self.problems))
+        per_opt = phys.clip_options(options, len(self.problems))
         if slots is not None:
-            self._init_queue(weights, device, solve_fn, tensor_device, stage3_band_above, slots, store)
+            self._init_queue(weights, device, solve_fn, tensor_device, stage3_band_above, slots, store, options)
             return
         self.shards = shard_by_work(work_estimate(self.problems), world)
         self.slots = pad_to(self.shards)
@@ -195,6 +200,7 @@ class ShardedSolver:
         if solve_fn is None:
             self.batch = phys.PhysBatch([self.problems[i] for i in self.mine], device=device,
                                         weights=weights if per is None else per[self.mine],
+                                        options=None if per_opt is None else [per_opt[i] for i in self.mine],
                                         stage3_band_above=stage3_band_above) if self.mine else None
             tensor_device = tensor_device or torch.device("cuda", device)
         self.tdev = tensor_device or torch.device("cpu")
@@ -202,7 +208,7 @@ class ShardedSolver:
         self.recv = torch.zeros((world * self.slots, self.width), dtype=torch.float64, device=self.tdev) if world > 1 else None
         self.last_ms = {}
 
-    def _init_queue(self, weights, device, solve_fn, tensor_device, stage3_band_above, slots, store):
+    def _init_queue(self, weights, device, solve_fn, tensor_device, stage3_band_above, slots, store, options):
         import torch
         self.solve_fn, self.batch, self.last_ms = solve_fn, None, {}
         self.n_ee_max = max(p.n_ee for p in self.problems)
@@ -212,7 +218,7 @@ class ShardedSolver:
                 store = distributed_c10d._get_default_store()
             self.claim = StoreClaim(store, "chd/phys_queue/%d" % next(_QUEUE_KEYS), len(self.problems))
             self.queue = phys.PhysQueue(self.problems, slots, weights=weights, device=device,
-                                        stage3_band_above=stage3_band_above, claim=self.claim)
+                                        stage3_band_above=stage3_band_above, claim=self.claim, options=options)
             tensor_device = tensor_device or torch.device("cuda", device)
         self.tdev = tensor_device or torch.device("cpu")
 
@@ -317,11 +323,12 @@ class ShardedSolver:
 
 def solve_sharded(problems, weights=phys.DEFAULT_WEIGHTS, device: int = 0, rank: int = 0, world: int = 1, group=None,
                   solve_fn=None, tensor_device=None, stage3_band_above=None, slots=None, store=None,
-                  cost_terms: bool = False) -> dict:
+                  cost_terms: bool = False, options=None) -> dict:
     """shard -> solve -> one gather -> unshard for a list of `PhysProblem`s (see ShardedSolver; `slots`: a queue on
-    every rank, claimed from one shared counter, merged by clip index; `weights` and `cost_terms` as there)."""
+    every rank, claimed from one shared counter, merged by clip index; `weights`, `options` and `cost_terms` as
+    there)."""
     s = ShardedSolver(problems, weights, device, rank, world, group, solve_fn, tensor_device, stage3_band_above, slots,
-                      store)
+                      store, options)
     try:
         return s.solve(cost_terms=cost_terms)
     finally:

@@ -8,7 +8,10 @@ batch (that is where the GPU pays off); `--n_ee 2` selects the toes-only paramet
 through a queue of S device slots (`chd.phys.PhysQueue`: memory for S clips, each slot refilled as its clip finishes).
 Under torchrun, `--slots S` runs such a queue on every rank's GPU, the ranks claiming their next clips from one shared
 counter (`chd.parallel.ShardedSolver(slots=S)`), and rank 0 writes the four files of every clip.  Every `--w_*` flag takes
-one value for all clips or a comma separated list aligned with `--in_dir`, one value per clip.
+one value for all clips or a comma separated list aligned with `--in_dir`, one value per clip, and so do the solver
+options (`chd.phys.SolverOptions`): IPOPT's `--tol`, `--constr_viol_tol`, `--dual_inf_tol`, `--compl_inf_tol`, the
+iteration caps `--max_iter_<stage>` (0: the stage's own) and `--last_stage` (no_dynamics, dynamics or durations: a clip
+that stops early writes the solution files of the snapshots it took).
 """
 import argparse
 import os
@@ -47,6 +50,45 @@ def parse_weights(args, n):
     return [tuple(v[i] if len(v) > 1 else v[0] for v in cols) for i in range(n)]
 
 
+TOL_FLAGS = ("tol", "constr_viol_tol", "dual_inf_tol", "compl_inf_tol")
+STAGE_NAMES = ("1.1", "1.2", "2.1", "2.2", "3", "4")
+CAP_FLAGS = tuple("max_iter_" + s for s in STAGE_NAMES)
+
+
+def add_option_flags(ap):
+    """The solver-option flags; unset they leave the defaults (`chd.phys.SolverOptions`)."""
+    per = ", or one per clip (comma separated)"
+    for k in TOL_FLAGS:
+        ap.add_argument("--" + k, default=None, help="IPOPT's %s%s" % (k, per))
+    for k in CAP_FLAGS:
+        ap.add_argument("--" + k, default=None, help="iteration cap of stage %s, 0: its own%s" % (k[9:], per))
+    ap.add_argument("--last_stage", default=None, help="no_dynamics, dynamics or durations (the default)%s" % per)
+
+
+def parse_options(args, n):
+    """The solver-option flags as the solvers take them: None when none is set (the defaults), else one
+    `chd.phys.SolverOptions` per clip, a single value standing for every clip.  A list whose length is not n raises
+    ValueError."""
+    import chd
+    cols = {}
+    for k, conv in [(k, float) for k in TOL_FLAGS] + [(k, int) for k in CAP_FLAGS] + [("last_stage", str)]:
+        v = getattr(args, k, None)
+        if v is None:
+            continue
+        vals = [conv(x) for x in str(v).split(",")]
+        if len(vals) not in (1, n):
+            raise ValueError("--%s: %d values for %d clips" % (k, len(vals), n))
+        cols[k] = vals * n if len(vals) == 1 else vals
+    if not cols:
+        return None
+    out = []
+    for i in range(n):
+        kw = {k: v[i] for k, v in cols.items() if k in TOL_FLAGS or k == "last_stage"}
+        caps = tuple(cols[k][i] if k in cols else 0 for k in CAP_FLAGS)
+        out.append(chd.phys.SolverOptions(max_iter=caps, **kw))
+    return out
+
+
 def main(argv=None):
     ap = argparse.ArgumentParser(allow_abbrev=False)
     ap.add_argument("--out_dir", default="sol_out")
@@ -59,6 +101,7 @@ def main(argv=None):
                     help="run stage 3 on sequences with more than 96 phase durations too (switch times as band unknowns)")
     ap.add_argument("--slots", type=int, default=0,
                     help="solve the clips through a queue of this many device slots instead of one batch")
+    add_option_flags(ap)
     args = ap.parse_args(argv)
     import chd
     in_dirs = args.in_dir.split(",")
@@ -73,6 +116,7 @@ def main(argv=None):
         print("Optim weights (%g, %g, %g, %g)\nDuration cost weight %g" % weights)
     else:
         print("Optim weights (%s, %s, %s, %s)\nDuration cost weight %s" % tuple(getattr(args, k) for k in WEIGHT_FLAGS))
+    options = parse_options(args, len(in_dirs))
     problems = [chd.io_formats.read_phys_inputs(d, f, n_ee=args.n_ee) for d, f in zip(in_dirs, nframes)]
     band = 96 if args.stage3_long else None
     world, rank, local = int(os.environ.get("WORLD_SIZE", 1)), int(os.environ.get("RANK", 0)), int(os.environ.get("LOCAL_RANK", 0))
@@ -84,7 +128,7 @@ def main(argv=None):
         torch.cuda.set_device(local)
         dist.init_process_group("nccl", device_id=torch.device("cuda", local))
         out = chd.parallel.solve_sharded(problems, weights=weights, device=local, rank=rank, world=world,
-                                         stage3_band_above=band, slots=args.slots)
+                                         stage3_band_above=band, slots=args.slots, options=options)
         dist.destroy_process_group()
         if rank == 0:
             write_results(out, problems, out_dirs, max(p.n_ee for p in problems))
@@ -97,20 +141,21 @@ def main(argv=None):
         torch.cuda.set_device(local)
         dist.init_process_group("nccl", device_id=torch.device("cuda", local))
         out = chd.parallel.solve_sharded(problems, weights=weights, device=local, rank=rank, world=world,
-                                         stage3_band_above=band)
+                                         stage3_band_above=band, options=options)
         dist.destroy_process_group()
         if rank == 0:
             ne_max = max(p.n_ee for p in problems)
             for i, (p, od) in enumerate(zip(problems, out_dirs)):
                 nf, n_ee = int(out["frames"][i]), p.n_ee
                 cols = np.concatenate(chd.phys.sample_columns(n_ee, ne_max))
-                chd.io_formats.write_solution(os.path.join(od, "sol_out_durations.txt"), p.dt, out["samples"][i, :nf][:, cols], n_ee)
+                if chd.phys.snapshots_taken(out, i)[2]:
+                    chd.io_formats.write_solution(os.path.join(od, "sol_out_durations.txt"), p.dt, out["samples"][i, :nf][:, cols], n_ee)
                 chd.io_formats.write_success_log(os.path.join(od, "success_log.txt"), out["success"][i, 0], out["success"][i, 1])
         return
     if args.slots:
-        batch = chd.phys.PhysQueue(problems, args.slots, weights=weights, stage3_band_above=band)
+        batch = chd.phys.PhysQueue(problems, args.slots, weights=weights, stage3_band_above=band, options=options)
     else:
-        batch = chd.phys.PhysBatch(problems, weights=weights, stage3_band_above=band)
+        batch = chd.phys.PhysBatch(problems, weights=weights, stage3_band_above=band, options=options)
     out = batch.solve()
     write_results(out, problems, out_dirs, batch.n_ee_max)
 

@@ -4,7 +4,9 @@ Cartesian grid of the comma separated `--w_*` values, every (clip, setting) pair
 `chd.phys.PhysQueue` with its own weights.  For every pair it writes one row (JSON or CSV, by the extension of
 `--results`): the clip, the setting, the stage statuses and iterations, the success flags, the ten unweighted cost terms
 (`chd.phys.COST_TERMS`) of the final iterate and its scaled NLP error and unscaled constraint violation.  With
-`--out_dir` it also writes phys_optim's four output files of every pair to <out_dir>/<clip name>/setting_<k>/.
+`--out_dir` it also writes phys_optim's four output files of every pair to <out_dir>/<clip name>/setting_<k>/.  `--tol`
+and `--last_stage` (`chd.phys.SolverOptions`) apply to every pair: a looser tolerance, or a sweep that stops after
+stage 2.2 (`--last_stage dynamics`, which writes only the solution files of the snapshots taken), is a cheaper preview.
 
     python scripts/weight_sweep.py --in_dir clip --nframes 120 --n_ee 2 --w_ee 0.1,0.3,1 --w_dur 0.1,1 \\
         --results sweep.csv --slots 64
@@ -30,9 +32,17 @@ def weight_grid(args):
     return list(itertools.product(*[[float(x) for x in str(getattr(args, k)).split(",")] for k in WEIGHT_FLAGS]))
 
 
+def sweep_options(args):
+    """The `SolverOptions` of every setting, None when neither `--tol` nor `--last_stage` is set (the defaults)."""
+    import chd
+    kw = {k: getattr(args, k) for k in ("tol", "last_stage") if getattr(args, k, None) is not None}
+    return chd.phys.SolverOptions(**kw) if kw else None
+
+
 def final_stage(stage_status):
-    """Stage id whose iterate is the final one (sol_out_durations.txt): 4 (stage 4) when it ran, else 3 (stage 3)."""
-    return 5 if stage_status[5] != -9 else 4
+    """Stage id whose iterate is the final one: the last stage that ran (stage 4 when it ran after stage 3, or the
+    clip's last_stage)."""
+    return max(s for s in range(6) if stage_status[s] != -9)
 
 
 def sweep_rows(out, clips, grid):
@@ -82,6 +92,8 @@ def main(argv=None):
     ap.add_argument("--out_dir", default=None, help="also write phys_optim's four files of every (clip, setting)")
     ap.add_argument("--stage3_long", action="store_true",
                     help="run stage 3 on sequences with more than 96 phase durations too (switch times as band unknowns)")
+    ap.add_argument("--tol", type=float, default=None, help="IPOPT's tol of every setting (default 1e-3)")
+    ap.add_argument("--last_stage", default=None, help="no_dynamics, dynamics or durations (the default) for every setting")
     args = ap.parse_args(argv)
     import chd
     in_dirs = args.in_dir.split(",")
@@ -95,7 +107,9 @@ def main(argv=None):
     problems = [p for p in clips for _ in grid]
     weights = [w for _ in clips for w in grid]
     t0 = time.perf_counter()
-    q = chd.phys.PhysQueue(problems, args.slots, weights=weights, stage3_band_above=96 if args.stage3_long else None)
+    options = sweep_options(args)
+    q = chd.phys.PhysQueue(problems, args.slots, weights=weights, stage3_band_above=96 if args.stage3_long else None,
+                           options=options)
     out = q.solve(cost_terms=True)
     q.close()
     wall = time.perf_counter() - t0
